@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""Benchmark of the OpenIBL hot path on B200 (contract: see the task prompt / DESIGN.md).
+"""Benchmark of the OpenIBL hot path on H100 (sm_90a; see DESIGN.md).
 
-    python bench.py [--gpus N --steps K --warmup W]          # B200 engine (libiblb200.so)
+    python bench.py [--gpus N --steps K --warmup W]          # H100 engine (libiblb200.so)
+    python bench.py --dump-outputs DIR [...]                 # also write the last timed step's outputs as .npy
     python bench.py --impl reference [...]                   # reference CPU arithmetic (oracle port)
 
 Primary metric (BASELINE.json): images/sec of VGG16+NetVLAD+PCA descriptor extraction at batch 32,
@@ -36,11 +37,12 @@ def peaks():
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"],
                 "bf16_tflops_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]), "src": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "src": "fallback"}
+    # NVIDIA data sheet, H100 SXM at 700 W (dense bf16): an upper bound, not a measured rate
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "src": "H100 SXM data sheet"}
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -206,8 +208,15 @@ def run_reference(args):
     print(json.dumps(line), flush=True)
 
 
+def dump_output(directory, name, t):
+    """One output array of the timed path as directory/name.npy (the bench writes nothing else there)."""
+    import numpy as np
+    os.makedirs(directory, exist_ok=True)
+    np.save(os.path.join(directory, name + ".npy"), t.detach().cpu().numpy())
+
+
 def gpu_eager_images_per_sec(xs, sd_dev, steps=3):
-    """What stock PyTorch gets on the SAME B200 (SURVEY 2.1 'the bar', BASELINE.md 3.4): the reference forward as
+    """What stock PyTorch gets on the SAME GPU (SURVEY 2.1 'the bar', BASELINE.md 3.4): the reference forward as
     eager torch ops on CUDA tensors -- cuDNN convs (cudnn.benchmark=True as examples/test.py:80), cuBLAS GEMMs, ATen
     normalisations -- batch 32, same inputs and weights.  Two variants: fp32-strict (TF32 off; the arithmetic the
     1e-4 tolerance is stated against) and torch defaults (cuDNN convs may use TF32).  The NetVLAD aggregation is the
@@ -257,6 +266,9 @@ def main():
     ap.add_argument("--strong-db", type=int, default=250000)
     ap.add_argument("--strong-budget-s", type=float, default=240.0,
                     help="skip the strong-scaling leg if its projected extraction time exceeds this")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed extraction step and of the last retrieval call as "
+                         "DIR/<name>.npy (float32 / float64), for output-for-output comparison of two builds")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -269,7 +281,7 @@ def main():
     rank = int(os.environ.get("RANK", "0"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a B200: the engine has no CPU fallback (use --impl reference for the CPU arm)")
+        raise SystemExit("bench.py needs an H100: the engine has no CPU fallback (use --impl reference for the CPU arm)")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     if world > 1:
@@ -303,11 +315,14 @@ def main():
     l0 = eng.launch_count
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
+    last = None
     for i in range(args.steps):
-        eng.extract(xs[i % 2], pca=True)
+        last, _ = eng.extract(xs[i % 2], pca=True)
     e1.record()
     torch.cuda.synchronize()
     launches = eng.launch_count - l0
+    if args.dump_outputs and rank == 0 and last is not None:
+        dump_output(args.dump_outputs, "extract_descriptors", last.float())       # [32, 4096] PCA descriptors
     ms = torch.tensor([e0.elapsed_time(e1)], device=dev)
     barrier()
     clocks = sampler.stop() if rank == 0 else None
@@ -343,33 +358,24 @@ def main():
         else:
             shapes.append((hh, ww, item[1], item[2]))
     conv_ms, conv_gflop = 0.0, 0.0
-    fused1 = os.environ.get("IBL_CONV1_FUSED", "1") != "0"
     for li, (lh, lw, cin, cout) in enumerate(shapes):
-        if li == 0 and not fused1:
+        if li == 0:
             continue                      # conv1_1 alone (Cin = 3, output-write bound) is not part of the family
-        if li == 1 and fused1:
-            continue                      # conv1_2 is inside the fused conv1 kernel timed at li == 0
         msl = ctypes.c_float()
-        if li == 0:                       # conv1_1 + conv1_2 + pool in ONE kernel: layer id 13, NCHW image input
-            check(eng.lib.ibl_debug_time_layer(eng.h, 13, _ptr(xs[0]), BATCH, lh, lw, 0, 3, ctypes.byref(msl)), "time_layer")
-            conv_gflop += 2.0 * BATCH * lh * lw * 9 * (3 * 64 + 64 * 64) / 1e9
-        else:
-            xin = torch.randn(BATCH, lh, lw, cin, device=dev).relu_()
-            check(eng.lib.ibl_debug_time_layer(eng.h, li, _ptr(xin), BATCH, lh, lw, 0, 3, ctypes.byref(msl)), "time_layer")
-            conv_gflop += 2.0 * BATCH * lh * lw * 9 * cin * cout / 1e9
-            del xin
+        xin = torch.randn(BATCH, lh, lw, cin, device=dev).relu_()
+        check(eng.lib.ibl_debug_time_layer(eng.h, li, _ptr(xin), BATCH, lh, lw, 0, 3, ctypes.byref(msl)), "time_layer")
+        conv_gflop += 2.0 * BATCH * lh * lw * 9 * cin * cout / 1e9
+        del xin
         conv_ms += msl.value
     ach_k = conv_gflop / conv_ms
     conv_traffic = load_conv_traffic()
     roofline = {"bound": "tensor",
-                "kernel": ("conv1_fused_tc_kernel (conv1_1+conv1_2+pool) + conv3x3_tc_kernel x 11 (conv2_1..conv5_3): 12 launches, "
-                           "tcgen05 implicit GEMM, bf16x3") if fused1 else
-                          "conv3x3_tc_kernel (12 launches: conv1_2..conv5_3, tcgen05 implicit GEMM, bf16x3)",
+                "kernel": "conv3x3_tc_kernel (12 launches: conv1_2..conv5_3, wgmma implicit GEMM, bf16x3)",
                 "achieved": ach_k, "peak": pk["bf16_tflops_sustained"], "unit": "TFLOP/s",
                 "frac": ach_k / pk["bf16_tflops_sustained"],
                 "traffic": conv_traffic.get("dram_bytes_per_step"), "traffic_note": conv_traffic.get("note"),
                 "traffic_vs_algorithmic": conv_traffic.get("vs_algorithmic"),
-                "peak_source": pk["src"] + " bf16 sustained (cuBLAS)",
+                "peak_source": pk["src"] + " bf16",
                 "note": "achieved = algorithmic fp32-grade FLOPs / sum of the 12 launch durations; the bf16x3 split issues "
                         "3 MMA passes per product, so the tensor pipe executes 3x the algorithmic figure (mma_issue_frac)",
                 "ms_per_launch_group": conv_ms, "mma_issue_frac": 3 * ach_k / pk["bf16_tflops_sustained"],
@@ -441,9 +447,12 @@ def main():
     r0.record()
     rsteps = 3
     for _ in range(rsteps):
-        sharded_topk(qd, dbd, TOPK, idx_base=rank * NDB, n_valid=NDB)
+        r_dist, r_idx = sharded_topk(qd, dbd, TOPK, idx_base=rank * NDB, n_valid=NDB)
     r1.record()
     torch.cuda.synchronize()
+    if args.dump_outputs and rank == 0:
+        dump_output(args.dump_outputs, "retrieval_dist", r_dist.float())          # [6800, 10]
+        dump_output(args.dump_outputs, "retrieval_idx", r_idx.double())           # [6800, 10] database indices
     r_ms = torch.tensor([r0.elapsed_time(r1) / rsteps], device=dev)
     if world > 1:
         dist.all_reduce(r_ms, op=dist.ReduceOp.MAX)
@@ -485,7 +494,7 @@ def main():
             "metric": "images_per_sec_extraction", "value": value, "unit": "images/s", "n_gpus": world,
             "steps": args.steps, "warmup": max(args.warmup, 3), "ms_per_step": ms_total / args.steps,
             "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-            "dtype": "f32 (bf16x3 split on tcgen05, fp32 accumulate)" if args.conv_mode == "tc" else "f32",
+            "dtype": "f32 (bf16x3 split on wgmma, fp32 accumulate)" if args.conv_mode == "tc" else "f32",
             "data": "synthetic",
             "config": {"workload": "batch-32 3x480x640 VGG16+NetVLAD+PCA(4096) extraction per GPU (configs[1])",
                        "global_batch": BATCH * world, "l2": "two alternating 118 MB input batches; 2.5 GB of "
@@ -506,7 +515,7 @@ def main():
                           "ms": float(r_ms.item()), "algorithmic_tflops": r_alg,
                           "roofline": {"bound": "tensor", "achieved": r_alg / world, "peak": pk_burst, "unit": "TFLOP/s",
                                        "frac": r_alg / world / pk_burst,
-                                       "peak_source": pk["src"] + " bf16 burst (cuBLAS), kernel timed alone",
+                                       "peak_source": pk["src"] + " bf16, kernel timed alone",
                                        "tensor_pipe_active_pct": dist_prof.get("tensor_pipe_active_pct"),
                                        "tensor_pipe_source": dist_prof.get("source"),
                                        "note": "achieved = 2*m*n*d algorithmic FLOP of the whole call (planes + screening "

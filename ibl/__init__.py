@@ -1,9 +1,9 @@
-"""`ibl` -- the reference's package name, served by the B200 engine.
+"""`ibl` -- the reference's package name, served by the H100 (sm_90a) engine.
 
 A thin alias layer so that code written against yxgeee/OpenIBL (`from ibl import models`,
 `from ibl.evaluators import Evaluator, extract_features, pairwise_distance`, `from ibl.pca import PCA`,
 `from ibl.utils.data.sampler import DistributedSliceSampler`, ...; examples/test.py:17-26) imports
-the B200-native host mirror in openibl_b200/ unchanged."""
+the H100-native host mirror in openibl_b200/ unchanged."""
 import sys as _sys
 
 import openibl_b200 as _pkg

@@ -1,5 +1,5 @@
 /*
- * iblb200.h -- C ABI of the B200-native OpenIBL hot path (libiblb200.so).
+ * iblb200.h -- C ABI of the H100-native (sm_90a) OpenIBL hot path (libiblb200.so).
  *
  * Drop-in boundary for the one data-parallel path of yxgeee/OpenIBL:
  *   VGG16 conv1_1..conv5_3 -> NetVLAD (+intra-norm, L2) -> PCA-whiten + L2
@@ -39,7 +39,7 @@ typedef enum ibl_status {
   IBL_ERR_BAD_ARG = 1,       /* null pointer, non-positive size, unsupported shape */
   IBL_ERR_NOT_READY = 2,     /* weights for the requested stage were never set */
   IBL_ERR_CUDA = 3,          /* a CUDA runtime/driver call failed (see ibl_last_error) */
-  IBL_ERR_NO_DEVICE = 4,     /* no usable sm_100 device: there is NO CPU fallback */
+  IBL_ERR_NO_DEVICE = 4,     /* no usable sm_90 device: there is NO CPU fallback */
   IBL_ERR_OOM = 5,           /* workspace allocation failed */
   IBL_ERR_UNSUPPORTED = 6    /* valid request this build cannot serve */
 } ibl_status;
@@ -53,7 +53,7 @@ typedef struct ibl_engine ibl_engine;
 
 /* conv math mode (ibl_engine_set_conv_mode) */
 #define IBL_CONV_SIMT_FP32 0  /* fp32 CUDA-core implicit GEMM (verification path)              */
-#define IBL_CONV_TC_BF16X3 1  /* tcgen05 implicit GEMM, bf16 hi/lo split, 3 MMAs, fp32 accum   */
+#define IBL_CONV_TC_BF16X3 1  /* wgmma implicit GEMM, bf16 hi/lo split, 3 MMAs, fp32 accum     */
 
 int ibl_abi_version(void);
 const char* ibl_status_string(int status);
@@ -65,7 +65,7 @@ int ibl_engine_create(int device, ibl_engine** out);
 int ibl_engine_destroy(ibl_engine* e);
 int ibl_engine_set_conv_mode(ibl_engine* e, int mode);
 int ibl_engine_get_conv_mode(ibl_engine* e, int* mode);
-/* Math mode of the distance and PCA GEMMs (same two values; default tcgen05 bf16x3 with exact fp32
+/* Math mode of the distance and PCA GEMMs (same two values; default tensor-core bf16x3 with exact fp32
  * re-scoring of the top-k candidates). */
 int ibl_engine_set_gemm_mode(ibl_engine* e, int mode);
 /* Number of kernels this library has launched through `e` since creation. */
@@ -110,7 +110,7 @@ int ibl_maxpool2x2_backward(ibl_engine* e, const float* x_nhwc, const float* gy_
                             float* gx_nhwc, void* stream);
 /* Backward of one trainable layer (what autograd + cuDNN dgrad/wgrad compute for vgg.py:61-62): x = the layer's
  * input, y = its post-ReLU output (read only if the layer has a ReLU), gy = dL/dy.  gx = dL/dx (NULL for the first
- * trainable layer), gw [Cout,Cin,3,3], gb [Cout].  dgrad and wgrad run on tcgen05 (bf16x3). */
+ * trainable layer), gw [Cout,Cin,3,3], gb [Cout].  dgrad and wgrad run on the tensor cores (bf16x3). */
 int ibl_vgg16_layer_backward(ibl_engine* e, int layer, const float* x, const float* y, const float* gy, int N,
                              int H, int W, float* gx, float* gw, float* gb, void* stream);
 
@@ -216,7 +216,7 @@ int ibl_l2dist_topk_host(ibl_engine* e, const float* q_host, int m, const float*
                          int d, int k, float* out_dist_host, int64_t* out_idx_host, void* stream);
 
 /* C[m,n] = alpha * A[m,k] . B[n,k]^T on the engine's GEMM kernels: the products of PCA.train (pca.py:38-67,
- * torch.matmul there).  mode IBL_CONV_SIMT_FP32 (fp32 CUDA cores) or IBL_CONV_TC_BF16X3 (tcgen05, k % 64 == 0). */
+ * torch.matmul there).  mode IBL_CONV_SIMT_FP32 (fp32 CUDA cores) or IBL_CONV_TC_BF16X3 (tensor cores, k % 64 == 0). */
 int ibl_gemm_nt(ibl_engine* e, const float* A, int m, const float* B, int n, int k, float alpha, float* C, int mode,
                 void* stream);
 
@@ -224,22 +224,22 @@ int ibl_gemm_nt(ibl_engine* e, const float* A, int m, const float* B, int n, int
 /* Queries that the guard of the single-pass distance path re-ranked by exact brute force in the last
  * ibl_l2dist_topk call (-1: that path was not taken).  Synchronises. */
 int ibl_debug_dist_flagged(ibl_engine* e, int* count, void* stream);
-/* Runs the tcgen05/TMA building blocks against CUDA-core results on the device;
+/* Runs the wgmma/TMA building blocks against CUDA-core results on the device;
  * returns IBL_OK when all agree. max_rel_err (may be NULL) receives the worst error. */
 int ibl_selftest_tc(ibl_engine* e, float* max_rel_err);
 
 /* One 3x3/s1/p1 conv layer in isolation (test hook): x NHWC [N,H,W,Cin] fp32, w OIHW, optional
  * ReLU and fused 2x2 max-pool, y NHWC fp32.  mode: IBL_CONV_SIMT_FP32, IBL_CONV_TC_BF16X3 (fp32
- * epilogue) or 2 (tcgen05 with the bf16 hi/lo plane epilogue, converted back to fp32).
- * bn_override forces the N tile (64/128/256) when it divides Cout, 0 = default. Synchronises. */
+ * epilogue) or 2 (tensor cores with the bf16 hi/lo plane epilogue, converted back to fp32).
+ * bn_override forces the N tile (64/128) when it divides Cout, 0 = default. Synchronises. */
 int ibl_debug_conv3x3(ibl_engine* e, const float* x_nhwc, int N, int H, int W, int cin,
                       const float* w_oihw, const float* bias, int cout, int relu, int pool, int mode,
                       int bn_override, float* y_nhwc, void* stream);
 
-/* MN-major tcgen05 operand self-test: C[128,64] = A^T B for A [128 k,128 m], B [128 k,64 n] (fp32, device),
+/* MN-major wgmma operand self-test: C[128,64] = A^T B for A [128 k,128 m], B [128 k,64 n] (fp32, device),
  * bf16x3 on the tensor core.  Synchronises. */
 int ibl_debug_gemm_tn(ibl_engine* e, const float* A, const float* B, float* C, void* stream);
-/* Hardware probe (tools/probe_umma_stride.py): D[128,64] = view(A) . B^T on tcgen05 where view row m is row
+/* Hardware probe: D[128,64] = view(A) . B^T on the tensor cores (wgmma) where view row m is row
  * s0 + (m/8)*group_rows + (m%8) of the TMA-staged, 128B-swizzled [rows][64] bf16 tile A; base_mode 1 sets the
  * descriptor's base_offset field to the start row's swizzle phase.  Decides whether a conv can read its nine
  * taps out of one halo tile. */

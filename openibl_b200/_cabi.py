@@ -1,6 +1,6 @@
 """ctypes binding of libiblb200.so (include/iblb200.h).
 
-The library is the product: if it cannot be loaded, or there is no sm_100 GPU, every
+The library is the product: if it cannot be loaded, or there is no sm_90 GPU, every
 operation raises -- there is no PyTorch / CPU fallback behind these calls."""
 from __future__ import annotations
 

@@ -1,4 +1,4 @@
-// Shared declarations for libiblb200 (sm_100a only).
+// Shared declarations for libiblb200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -55,7 +55,7 @@ struct DeviceOnce {
 static inline int device_sm_count() {
   int dev = 0, sms = 0;
   cudaGetDevice(&dev);
-  if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 148;
+  if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
   return sms;
 }
 
@@ -92,7 +92,7 @@ int launch_planes_to_f32(const __nv_bfloat16* hi, const __nv_bfloat16* lo, size_
 int launch_f32_to_planes(const float* x, size_t n, __nv_bfloat16* hi, __nv_bfloat16* lo,
                          cudaStream_t s);
 
-// tc_conv.cu  (tcgen05 + TMA implicit GEMM, bf16 hi/lo split operands)
+// tc_conv.cu  (wgmma + TMA implicit GEMM, bf16 hi/lo split operands)
 struct TcConvPlan;   // opaque per-engine cache of TMA descriptors
 int tc_driver_init();   // resolves cuTensorMapEncodeTiled; IBL_ERR_NO_DEVICE if unavailable
 int launch_conv3x3_tc(const __nv_bfloat16* x_hi, const __nv_bfloat16* x_lo, const ConvParams& p,
@@ -111,7 +111,7 @@ int launch_argsort_rows(const float* dist, long long ld, int m, int n, long long
 int launch_resize_bilinear_u8(const uint8_t* x, int N, int Hin, int Win, int Hout, int Wout, const int* bounds_h,
                               const int* kk_h, int ksize_h, const int* bounds_v, const int* kk_v, int ksize_v,
                               uint8_t* tmp, uint8_t* out, cudaStream_t s, uint64_t* launches);
-// tc_conv_bwd.cu  (dgrad filter re-layout, tcgen05 wgrad, ReLU mask, pool backward, conv1_1 wgrad)
+// tc_conv_bwd.cu  (dgrad filter re-layout, wgmma wgrad, ReLU mask, pool backward, conv1_1 wgrad)
 int launch_repack_weights_dgrad(const float* w_tck, int cout, int cin, __nv_bfloat16* w_hi, __nv_bfloat16* w_lo,
                                 cudaStream_t s);
 int launch_relu_mask_planes(const float* g, const float* y, size_t n, bool relu, __nv_bfloat16* hi, __nv_bfloat16* lo,
@@ -126,12 +126,12 @@ int launch_conv1_1_wgrad(const float* x_nchw, const __nv_bfloat16* g_hi, const _
 // tc_conv1.cu
 int launch_conv1_1_tc(const float* x_nchw, const float* w_oihw, const float* bias, int N, int H, int W,
                       __nv_bfloat16* y_hi, __nv_bfloat16* y_lo, cudaStream_t s);
+// tc_probe.cu
+int debug_gmma_strided(const void* A, int rows, const void* B, int s0, int group_rows, int base_mode, float* D,
+                       cudaStream_t s);
 // tc_netvlad.cu
 int debug_gemm_tn(const float* A, const float* B, float* C, cudaStream_t s);
 int netvlad_tc_units(int B, int S);
-// tc_probe.cu
-int debug_umma_strided(const void* A, int rows, const void* B, int s0, int group_rows, int base_mode, float* D,
-                       cudaStream_t s);
 int launch_netvlad_tc(const __nv_bfloat16* x_hi, const __nv_bfloat16* x_lo, int B, int S,
                       const __nv_bfloat16* w_hi, const __nv_bfloat16* w_lo, const float* ssq, int ssq_parts,
                       const float* cent, bool normalize_input, float* part, float* asum_part, int* ticket,
@@ -139,21 +139,16 @@ int launch_netvlad_tc(const __nv_bfloat16* x_hi, const __nv_bfloat16* x_lo, int 
 int launch_global_maxpool_planes(const __nv_bfloat16* hi, const __nv_bfloat16* lo, int N, int S, int C, float* y,
                                  cudaStream_t s);
 
-// tc_gemm.cu  (tcgen05 NT GEMM on bf16 hi/lo planes: distance/top-16, dense distance, PCA partials)
-int dist_top16_max_runs(int m, int n_valid);
+// tc_gemm.cu  (wgmma NT GEMM on bf16 hi/lo planes: distance/top-16, dense distance, PCA partials)
+int dist_top16_max_runs(int m, int n_valid, bool pairs);
 int launch_dist_top16_tc(const __nv_bfloat16* q_hi, const __nv_bfloat16* q_lo, const float* qn, int m,
                          const __nv_bfloat16* d_hi, const __nv_bfloat16* d_lo, const float* dn, int n,
                          int n_valid, int K, float* cand_d, long long* cand_i, int max_runs, int* runs_out,
-                         cudaStream_t s);
+                         bool pairs, cudaStream_t s);
 int launch_dist_dense_tc(const __nv_bfloat16* q_hi, const __nv_bfloat16* q_lo, const float* qn, int m,
                          const __nv_bfloat16* d_hi, const __nv_bfloat16* d_lo, const float* dn, int n, int K,
                          float* out, long long ld_out, cudaStream_t s);
-// tc_gemm2.cu  (same contract on SM pairs: tcgen05.mma.cta_group::2, 256-row tiles)
-int dist_top16_2sm_max_runs(int m, int n_valid);
-int launch_dist_top16_2sm(const __nv_bfloat16* q_hi, const __nv_bfloat16* q_lo, const float* qn, int m,
-                          const __nv_bfloat16* d_hi, const __nv_bfloat16* d_lo, const float* dn, int n,
-                          int n_valid, int K, float* cand_d, long long* cand_i, int* runs_out, cudaStream_t s);
-// tc_dist1.cu  (single-pass fp16 screening on SM pairs + exact re-scoring + guard + exact fallback)
+// tc_dist1.cu  (single-pass fp16 screening + exact re-scoring + guard + exact fallback)
 size_t dist1_workspace_bytes(int m, int n, int d, size_t* off /*[9]*/);
 int launch_dist_topk_1pass(const float* q, int m, const float* db, int n, int n_valid, int d, int k, long long idx_base,
                            void* ws, float* out_dist, long long* out_idx, uint64_t* launches, cudaStream_t s);

@@ -61,7 +61,7 @@ struct ibl_engine {
   uint64_t launches = 0;
   bool vgg_ready = false;
   ConvParams conv[13];
-  float* w0_oihw = nullptr;   // conv1_1 filters in the reference OIHW layout (tcgen05 conv1_1 builds its own operand)
+  float* w0_oihw = nullptr;   // conv1_1 filters in the reference OIHW layout (the tensor-core conv1_1 builds its own operand)
   // borrowed NetVLAD / PCA parameters (owned by the caller's torch Parameters)
   const float* nv_w = nullptr;
   const float* nv_c = nullptr;
@@ -154,7 +154,7 @@ int vgg_forward_impl(ibl_engine* e, const float* x, int N, int H, int W, float* 
     }
     return IBL_OK;
   }
-  // tcgen05 path: activations are two bf16 planes, hi then lo, each `plane` elements apart
+  // tensor-core path: activations are two bf16 planes, hi then lo, each `plane` elements apart
   auto hi_of = [&](int b, size_t elems) { (void)elems; return e->act[b].as<__nv_bfloat16>(); };
   auto lo_of = [&](int b, size_t elems) { return e->act[b].as<__nv_bfloat16>() + elems; };
   size_t elems = (size_t)N * h * w * 64;
@@ -221,7 +221,7 @@ const char* ibl_status_string(int status) {
     case IBL_ERR_BAD_ARG: return "bad argument";
     case IBL_ERR_NOT_READY: return "parameters for this stage were not set";
     case IBL_ERR_CUDA: return "CUDA error";
-    case IBL_ERR_NO_DEVICE: return "no usable sm_100 CUDA device (this library has no CPU fallback)";
+    case IBL_ERR_NO_DEVICE: return "no usable sm_90 CUDA device (this library has no CPU fallback)";
     case IBL_ERR_OOM: return "out of device memory";
     case IBL_ERR_UNSUPPORTED: return "unsupported request";
     default: return "unknown status";
@@ -242,9 +242,9 @@ int ibl_engine_create(int device, ibl_engine** out) {
   IBL_REQUIRE(device >= 0 && device < count, "device index out of range");
   cudaDeviceProp prop;
   IBL_CUDA_OK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) {
+  if (prop.major != 9 || prop.minor != 0) {
     set_last_error(std::string("device '") + prop.name + "' is sm_" + std::to_string(prop.major) +
-                   std::to_string(prop.minor) + "; this library is built for sm_100a only");
+                   std::to_string(prop.minor) + "; this library is built for sm_90a only");
     return IBL_ERR_NO_DEVICE;
   }
   ibl_engine* e = new (std::nothrow) ibl_engine();
@@ -592,9 +592,9 @@ int ibl_pca_l2(ibl_engine* e, const float* v, int N, int D, const float* W, cons
     }
     return IBL_OK;
   }
-  // enough K-splits to fill the machine: tiles = ceil(P/128)*ceil(N/64)*splits >= ~2 waves of 148 SMs
+  // enough K-splits to fill the machine: tiles = ceil(P/128)*ceil(N/64)*splits >= ~2 waves of the SMs
   int tiles = cdiv(P, 128) * cdiv(N, 64);
-  int splits = cdiv(2 * 148, tiles);
+  int splits = cdiv(2 * device_sm_count(), tiles);
   if (splits < 1) splits = 1;
   if (splits > 32) splits = 32;
   while (splits > 1 && D / splits < 256) --splits;
@@ -638,7 +638,7 @@ int ibl_extract(ibl_engine* e, const float* x, int N, int H, int W, unsigned fla
     const bool fused = e->conv_mode == IBL_CONV_TC_BF16X3 && e->gemm_mode == IBL_CONV_TC_BF16X3 &&
                        e->nvw_pl_src == e->nv_w && K == 64 && C == 512;
     if (fused) {
-      // conv5_3 -> hi/lo planes + |x|^2 partials -> one tcgen05 NetVLAD kernel (+ finalize)
+      // conv5_3 -> hi/lo planes + |x|^2 partials -> one tensor-core NetVLAD kernel (+ finalize)
       FeatPlanes fp;
       IBL_RET(vgg_forward_impl(e, xb, nb, H, W, nullptr, S(stream), &fp));
       if (flags & IBL_OUT_POOL) {
@@ -873,7 +873,7 @@ int ibl_l2dist_dense(ibl_engine* e, const float* q, int m, const float* db, int 
 
 // C[m,n] = alpha * A[m,k] . B[n,k]^T on the engine's own GEMM kernels (PCA.train's covariance / dual products and
 // projection, reference ibl/pca.py:38-67, torch.matmul there).  mode: IBL_CONV_SIMT_FP32 = fp32 CUDA cores,
-// IBL_CONV_TC_BF16X3 = tcgen05 bf16x3 (k % 64 == 0).  Built on the distance tile with zero norm terms:
+// IBL_CONV_TC_BF16X3 = tensor-core bf16x3 (k % 64 == 0).  Built on the distance tile with zero norm terms:
 // (0 + 0 - 2 a.b) * (-alpha / 2).
 int ibl_gemm_nt(ibl_engine* e, const float* A, int m, const float* B, int n, int k, float alpha, float* C, int mode,
                 void* stream) {
@@ -938,7 +938,7 @@ int ibl_l2dist_topk(ibl_engine* e, const float* q, int m, const float* db, int n
   IBL_REQUIRE(n_valid >= 0 && n_valid <= n, "n_valid out of range");
   IBL_REQUIRE(k >= 1 && k <= 128, "top-k supports 1 <= k <= 128");
   DeviceGuard g(e->device);
-  // IBL_DIST_SCREEN=3 selects round 1's bf16x3 screening kernels (A/B measurements, variant tests)
+  // IBL_DIST_SCREEN=3 selects the bf16x3 screening kernel of tc_gemm.cu (A/B measurements, variant tests)
   static const int screen_env = [] { const char* v = getenv("IBL_DIST_SCREEN"); return v ? atoi(v) : 1; }();
   if (e->gemm_mode == IBL_CONV_TC_BF16X3 && d % 64 == 0 && n_valid > 0 && k <= 12 && m > 128 && screen_env != 3) {
     // single fp16 tensor-core pass to screen, exact fp32 to decide, guard + exact fallback on the device
@@ -962,22 +962,15 @@ int ibl_l2dist_topk(ibl_engine* e, const float* q, int m, const float* db, int n
     e->launches += 2;
     const int kc = 16;                           // candidates kept per query before exact re-scoring
     if (k <= 12) {
-      // SM pairs (tcgen05.mma.cta_group::2, tc_gemm2.cu) unless there is a single 128-query tile; IBL_DIST_2SM=0
-      // selects the one-SM kernel of tc_gemm.cu
-      static const bool two_sm_env = [] { const char* v = getenv("IBL_DIST_2SM"); return !v || atoi(v) != 0; }();
-      const bool two_sm = two_sm_env && m > 128;
-      const int max_runs = two_sm ? dist_top16_2sm_max_runs(m, n_valid) : dist_top16_max_runs(m, n_valid);
+      // SM pairs (2-CTA clusters multicasting the database tile, tc_gemm.cu) unless IBL_DIST_2SM=0
+      static const bool two_sm = [] { const char* v = getenv("IBL_DIST_2SM"); return !v || atoi(v) != 0; }();
+      const int max_runs = dist_top16_max_runs(m, n_valid, two_sm);
       IBL_RET(e->cand_d.ensure((size_t)max_runs * m * kc * sizeof(float)));
       IBL_RET(e->cand_i.ensure((size_t)max_runs * m * kc * sizeof(int64_t)));
       int runs = 0;
-      if (two_sm) {
-        IBL_RET(launch_dist_top16_2sm(qh, qh + qe, e->qn.as<float>(), m, dh, dh + de, e->dbn.as<float>(), n,
-                                      n_valid, d, e->cand_d.as<float>(), e->cand_i.as<long long>(), &runs, s));
-      } else {
-        IBL_RET(launch_dist_top16_tc(qh, qh + qe, e->qn.as<float>(), m, dh, dh + de, e->dbn.as<float>(), n,
-                                     n_valid, d, e->cand_d.as<float>(), e->cand_i.as<long long>(), max_runs,
-                                     &runs, s));
-      }
+      IBL_RET(launch_dist_top16_tc(qh, qh + qe, e->qn.as<float>(), m, dh, dh + de, e->dbn.as<float>(), n,
+                                   n_valid, d, e->cand_d.as<float>(), e->cand_i.as<long long>(), max_runs,
+                                   &runs, two_sm, s));
       e->launches++;
       const long long* ci = e->cand_i.as<long long>();
       if (runs > 1) {
@@ -1201,7 +1194,7 @@ int ibl_debug_umma_strided(ibl_engine* e, const void* A, int rows, const void* B
   IBL_REQUIRE(e && A && B && D, "null argument");
   DeviceGuard g(e->device);
   e->launches += 1;
-  return debug_umma_strided(A, rows, B, s0, group_rows, base_mode, D, S(stream));
+  return debug_gmma_strided(A, rows, B, s0, group_rows, base_mode, D, S(stream));
 }
 
 // Timing hooks (tools/bench_layers.py): average device time of one backbone layer over `reps`
@@ -1209,32 +1202,9 @@ int ibl_debug_umma_strided(ibl_engine* e, const void* A, int rows, const void* B
 // (x is NCHW [N,3,H,W]); layers 1..12 take x NHWC [N,H,W,Cin] fp32 (converted to planes once).
 int ibl_debug_time_layer(ibl_engine* e, int layer, const float* x, int N, int H, int W, int bn_override,
                          int reps, float* ms_out) {
-  IBL_REQUIRE(e && x && ms_out && layer >= 0 && layer <= 13 && reps >= 1, "bad argument");
+  IBL_REQUIRE(e && x && ms_out && layer >= 0 && layer <= 12 && reps >= 1, "bad argument");
   if (!e->vgg_ready) { set_last_error("ibl_engine_set_vgg16 was not called"); return IBL_ERR_NOT_READY; }
   DeviceGuard g(e->device);
-  if (layer == 13) {   // the fused conv1_1 + conv1_2 + pool kernel: x is the NCHW image batch
-    const size_t out_e = (size_t)N * (H / 2) * (W / 2) * 64;
-    IBL_RET(e->act[1].ensure(out_e * 4));
-    cudaEvent_t e0, e1;
-    IBL_CUDA_OK(cudaEventCreate(&e0));
-    IBL_CUDA_OK(cudaEventCreate(&e1));
-    __nv_bfloat16* oh_ = e->act[1].as<__nv_bfloat16>();
-    int rc = IBL_OK;
-    for (int r = -1; r < reps && rc == IBL_OK; ++r) {
-      if (r == 0) cudaEventRecord(e0, nullptr);
-      rc = launch_conv1_fused_tc(x, e->w0_oihw, e->conv[0].bias, e->conv[1], N, H, W, oh_, oh_ + out_e, nullptr);
-    }
-    cudaEventRecord(e1, nullptr);
-    cudaError_t ce = cudaEventSynchronize(e1);
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, e0, e1);
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
-    if (rc == IBL_OK && ce != cudaSuccess) { set_last_error(cudaGetErrorString(ce)); return IBL_ERR_CUDA; }
-    *ms_out = ms / reps;
-    e->launches += reps + 1;
-    return rc;
-  }
   const ConvLayer& L = kVgg16[layer];
   const size_t in_e = (size_t)N * H * W * L.cin;
   const int oh = L.pool ? H / 2 : H, ow = L.pool ? W / 2 : W;

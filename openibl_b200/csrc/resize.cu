@@ -76,7 +76,7 @@ int launch_resize_bilinear_u8(const uint8_t* x, int N, int Hin, int Win, int Hou
   const bool need_h = Wout != Win, need_v = Hout != Hin;
   auto blocks = [](long long total) {
     long long b = (total + 255) / 256;
-    return (unsigned)(b > 148 * 16 ? 148 * 16 : (b > 0 ? b : 1));
+    return (unsigned)(b > 132 * 16 ? 132 * 16 : (b > 0 ? b : 1));
   };
   if (!need_h && !need_v) {
     IBL_CUDA_OK(cudaMemcpyAsync(out, x, (size_t)N * Hin * Win * 3, cudaMemcpyDeviceToDevice, s));

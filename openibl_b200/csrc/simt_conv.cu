@@ -1,5 +1,5 @@
 // CUDA-core (fp32) kernels of the backbone: the verification path of the 3x3 convolutions,
-// conv1_1 (Cin=3, a K=27 contraction that does not tile onto tcgen05), pooling and the
+// conv1_1 (Cin=3, a K=27 contraction that does not tile onto a TMA-fed tensor-core GEMM), pooling and the
 // layout changes at the boundary.  Reference: ibl/models/vgg.py:40-42,61-70.
 #include "common.cuh"
 
@@ -144,7 +144,7 @@ int launch_conv3x3_simt(const float* x, const ConvParams& p, int N, int H, int W
 
 // ------------------------------------------------------------------------------------------
 // conv1_1: NCHW fp32 [N,3,H,W] -> NHWC [N,H,W,64], + bias + ReLU (vgg.py slot 0).  K = 27 does not
-// tile onto tcgen05, so this runs on the CUDA cores: one pixel per thread, 64 accumulators in
+// tile onto a TMA-fed tensor-core GEMM; this is the CUDA-core version: one pixel per thread, 64 accumulators in
 // registers, the 27x64 weights broadcast from shared memory (LDS.128 feeds 4 FMAs).  Each thread
 // writes its pixel's 64 channels as contiguous 16-byte stores (256 B fp32, or 128 B + 128 B of bf16
 // hi/lo planes), so every 128-byte line is fully written by one thread.
@@ -260,7 +260,7 @@ int launch_maxpool2x2(const float* x, int N, int H, int W, int C, float* y, cuda
   IBL_REQUIRE(C % 4 == 0, "maxpool needs C%4==0");
   long long total = (long long)N * (H / 2) * (W / 2) * (C / 4);
   unsigned blocks = (unsigned)((total + 255) / 256);
-  if (blocks > 148 * 32) blocks = 148 * 32;
+  if (blocks > 132 * 32) blocks = 132 * 32;
   if (blocks == 0) blocks = 1;
   maxpool2x2_kernel<<<blocks, 256, 0, s>>>(reinterpret_cast<const float4*>(x),
                                            reinterpret_cast<float4*>(y), N, H, W, C / 4);
@@ -317,7 +317,7 @@ int launch_u8_hwc_to_nchw_norm(const uint8_t* x, int N, int H, int W, const floa
                                cudaStream_t s) {
   const long long hw = (long long)H * W, total = hw * N;
   unsigned blocks = (unsigned)((total + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   if (!blocks) blocks = 1;
   u8_hwc_to_nchw_norm_kernel<<<blocks, 256, 0, s>>>(x, y, hw, total, mean[0], mean[1], mean[2], stdv[0], stdv[1],
                                                     stdv[2]);
@@ -388,7 +388,7 @@ __global__ void f32_to_planes_kernel(const float* __restrict__ x, size_t n,
 int launch_planes_to_f32(const __nv_bfloat16* hi, const __nv_bfloat16* lo, size_t n, float* y,
                          cudaStream_t s) {
   unsigned blocks = (unsigned)((n + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   if (!blocks) blocks = 1;
   planes_to_f32_kernel<<<blocks, 256, 0, s>>>(hi, lo, n, y);
   IBL_CUDA_OK(cudaGetLastError());
@@ -397,7 +397,7 @@ int launch_planes_to_f32(const __nv_bfloat16* hi, const __nv_bfloat16* lo, size_
 int launch_f32_to_planes(const float* x, size_t n, __nv_bfloat16* hi, __nv_bfloat16* lo,
                          cudaStream_t s) {
   unsigned blocks = (unsigned)((n + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   if (!blocks) blocks = 1;
   f32_to_planes_kernel<<<blocks, 256, 0, s>>>(x, n, hi, lo);
   IBL_CUDA_OK(cudaGetLastError());

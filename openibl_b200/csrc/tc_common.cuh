@@ -1,9 +1,12 @@
-// sm_100a building blocks: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (UMMA) and TMEM
-// wrappers as inline PTX, plus the descriptor encodings the tensor-core kernels share.
+// sm_90a building blocks: mbarrier, TMA (cp.async.bulk.tensor) and warpgroup MMA (wgmma) wrappers as
+// inline PTX, the shared-memory matrix descriptors the tensor-core kernels share, and the accumulator
+// transposition that hands a 128-row wgmma accumulator to row-per-thread epilogues.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include "wgmma.cuh"
 
 namespace ibl {
 namespace tc {
@@ -14,15 +17,13 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
 
 // Warp-uniform copy of a value that every lane of the (converged) warp holds.  REDUX writes a UNIFORM register, so the
 // compiler keeps everything derived from the result on the uniform datapath; a value that came from a shared-memory
-// load or a special register is per-thread as far as it knows, and each tcgen05 instruction fed from it is wrapped in
+// load or a special register is per-thread as far as it knows, and each TMA instruction fed from it is wrapped in
 // an ELECT / R2UR.BROADCAST loop.
 __device__ __forceinline__ uint32_t warp_uniform(uint32_t v) { return __reduce_or_sync(0xffffffffu, v); }
 
 // One lane of the converged warp (elect.sync).  ptxas knows that exactly one thread runs the guarded block and emits the
-// tcgen05 / TMA instructions inside it back to back; behind `if (lane == 0)` it cannot know, and wraps EVERY such
-// instruction in an ELECT / PLOP3 / BRA.U.ANY loop over the "possibly several" active threads -- ~90 clk of dependent
-// issue per MMA (ncu source view), more than an N <= 128 MMA occupies the tensor pipe.  A tcgen05.commit tracks the
-// MMAs of the executing thread: keep a commit in the same elected block as the MMAs it covers.
+// TMA instructions inside it back to back; behind `if (lane == 0)` it cannot know, and wraps EVERY such instruction in
+// an ELECT / PLOP3 / BRA.U.ANY loop over the "possibly several" active threads.
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile(
@@ -124,8 +125,6 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uin
       : "memory");
 }
 
-// 2D tiled load delivered to every CTA of the cluster whose bit is set in `mask` (same smem offset and same
-// mbarrier offset in each destination CTA)
 // ---- the same on shared-space addresses (producer warps that keep ring addresses as warp-uniform integers) --------
 __device__ __forceinline__ void mbar_arrive_expect_tx_a(uint32_t bar_addr, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar_addr), "r"(bytes) : "memory");
@@ -153,14 +152,9 @@ __device__ __forceinline__ void tma_load_4d_a(uint32_t dst, const CUtensorMap* m
       "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_addr), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
-__device__ __forceinline__ void tma_load_2d_mc(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
-                                               uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-      " [%0], [%1, {%4, %5}], [%2], %3;" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "h"(mask), "r"(c0), "r"(c1)
-      : "memory");
-}
+// ---- clusters of two CTAs ("SM pairs"): TMA multicast and cross-CTA barrier arrivals ------------------------------
+// 2D tiled load delivered to every CTA of the cluster whose bit is set in `mask` (same smem offset and same mbarrier
+// offset in each destination CTA)
 __device__ __forceinline__ void tma_load_2d_mc_a(uint32_t dst, const CUtensorMap* m, uint32_t bar_addr, int c0, int c1,
                                                  uint16_t mask) {
   asm volatile(
@@ -169,133 +163,18 @@ __device__ __forceinline__ void tma_load_2d_mc_a(uint32_t dst, const CUtensorMap
       "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_addr), "h"(mask), "r"(c0), "r"(c1)
       : "memory");
 }
+__device__ __forceinline__ void tma_load_3d_mc_a(uint32_t dst, const CUtensorMap* m, uint32_t bar_addr, int c0, int c1,
+                                                 int c2, uint16_t mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+      " [%0], [%1, {%4, %5, %6}], [%2], %3;" ::"r"(dst),
+      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_addr), "h"(mask), "r"(c0), "r"(c1), "r"(c2)
+      : "memory");
+}
 __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-
-// fire-and-forget: bring one box into L2
-__device__ __forceinline__ void tma_prefetch_3d(const CUtensorMap* m, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.prefetch.tensor.3d.L2.global [%0, {%1, %2, %3}];" ::"l"(
-                   reinterpret_cast<uint64_t>(m)),
-               "r"(c0), "r"(c1), "r"(c2)
-               : "memory");
-}
-
-// ---- TMEM management --------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-
-// ---- UMMA -----------------------------------------------------------------------------------
-// Shared-memory matrix descriptor, K-major operand, 128-byte swizzle, rows of 128 bytes
-// (64 bf16 / 32 tf32), 8-row swizzle atoms 1024 bytes apart (cute::UMMA::SmemDescriptor).
-__device__ __forceinline__ uint64_t umma_desc_kmajor_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3fffu);      // start address  [0,14)
-  d |= (uint64_t)1 << 16;                           // leading byte offset (unused for SW128 K-major)
-  d |= (uint64_t)(1024u >> 4) << 32;                // stride byte offset [32,46)
-  d |= (uint64_t)1 << 46;                           // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;                           // layout type: SWIZZLE_128B
-  return d;
-}
-// Same with 64-byte rows (32 bf16) and the 64B swizzle: 8-row atoms are 512 bytes.
-__device__ __forceinline__ uint64_t umma_desc_kmajor_sw64(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3fffu);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(512u >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)4 << 61;                           // layout type: SWIZZLE_64B
-  return d;
-}
-template <int BK>
-__device__ __forceinline__ uint64_t umma_desc_kmajor(uint32_t smem_addr) {
-  return BK == 64 ? umma_desc_kmajor_sw128(smem_addr) : umma_desc_kmajor_sw64(smem_addr);
-}
-// Instruction descriptor for kind::f16 with bf16 A/B (K-major), fp32 accumulator
-// (cute::UMMA::InstrDescriptor).
-__host__ __device__ constexpr uint32_t umma_idesc_bf16_f32(int M, int N) {
-  return (1u << 4)                      // c_format = F32
-         | (1u << 7)                    // a_format = BF16
-         | (1u << 10)                   // b_format = BF16
-         | ((uint32_t)(N >> 3) << 17)   // n_dim
-         | ((uint32_t)(M >> 4) << 24);  // m_dim
-}
-// kind::tf32 (fp32 containers, 10-bit mantissa used), fp32 accumulator
-__host__ __device__ constexpr uint32_t umma_idesc_tf32_f32(int M, int N) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                          uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                          uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// all previously issued MMAs of this thread arrive on `bar` when they complete
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-
-__device__ __forceinline__ void umma_commit_a(uint32_t bar_addr) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar_addr) : "memory");
-}
-
-// same, arriving on the barrier at this offset in every CTA of the cluster selected by `mask`
-__device__ __forceinline__ void umma_commit_mc(uint64_t* bar, uint16_t mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(mask)
-      : "memory");
-}
-
-__device__ __forceinline__ void umma_commit_mc_a(uint32_t bar_addr, uint16_t mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar_addr),
-      "h"(mask)
-      : "memory");
-}
-
-// ---- SM pairs (cta_group::2): one MMA spans the two CTAs of a cluster -------------------------------
-// The leader (cluster rank 0) issues the MMAs; each CTA stages its own 128 rows of A and its half of B,
-// accumulators live in each CTA's own TMEM.  All TMA bytes of a stage are accounted on the LEADER's
-// full barrier (peer loads name it by its shared::cluster address).
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -306,113 +185,98 @@ __device__ __forceinline__ uint32_t mapa_u32(uint32_t addr, uint32_t rank) {
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
   return r;
 }
-// no ordering of this thread's earlier memory operations (a cluster-scope release costs ~1 us when it
-// follows remote traffic): only for "I am done reading" signals whose reads have already been consumed
-__device__ __forceinline__ void mbar_arrive_remote_relaxed(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cta.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
+// arrive on the barrier at this shared::cluster address (another CTA's barrier)
 __device__ __forceinline__ void mbar_arrive_remote(uint32_t cluster_addr) {
   asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
 }
-__device__ __forceinline__ void tma_load_2d_2sm(void* dst, const CUtensorMap* m, uint32_t bar_cluster_addr, int c0,
-                                                int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_3d_2sm(void* dst, const CUtensorMap* m, uint32_t bar_cluster_addr, int c0,
-                                                int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_2sm(void* dst, const CUtensorMap* m, uint32_t bar_cluster_addr, int c0,
-                                                int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_2sm_a(uint32_t dst, const CUtensorMap* m, uint32_t bar_cluster_addr, int c0,
-                                                  int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];" ::"r"(dst),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_3d_2sm_a(uint32_t dst, const CUtensorMap* m, uint32_t bar_cluster_addr, int c0,
-                                                  int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(dst),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_2sm_a(uint32_t dst, const CUtensorMap* m, uint32_t bar_cluster_addr, int c0,
-                                                  int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(dst),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void umma_bf16_2sm(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                              uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrives on the barrier at this offset in both CTAs of the pair (mask 0x3) when the pair's MMAs retire
-__device__ __forceinline__ void umma_commit_2sm_mc(uint64_t* bar, uint16_t mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(mask)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_2sm_mc_a(uint32_t bar_addr, uint16_t mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar_addr),
-      "h"(mask)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* dst_smem, uint32_t ncols) {   // same warp id in both CTAs
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
+
+// fire-and-forget: bring one box into L2
+__device__ __forceinline__ void tma_prefetch_3d(const CUtensorMap* m, int c0, int c1, int c2) {
+  asm volatile("cp.async.bulk.prefetch.tensor.3d.L2.global [%0, {%1, %2, %3}];" ::"l"(
+                   reinterpret_cast<uint64_t>(m)),
+               "r"(c0), "r"(c1), "r"(c2)
                : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
 }
 
-// TMEM -> registers: this warp's 32 lanes x 32 consecutive fp32 columns
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
+// ---- warpgroup MMA ------------------------------------------------------------------------------
+// Shared-memory matrix descriptor (sm_90 GMMA), K-major operand, 128-byte swizzle: rows of 128 bytes (64 bf16), 8-row
+// swizzle atoms 1024 bytes apart.  Advancing the start address by 32 bytes (+2 in 16-byte units) steps 16 elements
+// along K inside the swizzled row.
+__device__ __forceinline__ uint64_t gmma_desc_kmajor_sw128(uint32_t smem_addr) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr >> 4) & 0x3fffu);      // start address  [0,14)
+  d |= (uint64_t)1 << 16;                           // leading byte offset (unused for swizzled K-major)
+  d |= (uint64_t)(1024u >> 4) << 32;                // stride byte offset [32,46)
+  d |= (uint64_t)1 << 62;                           // layout type: SWIZZLE_128B
+  return d;
 }
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// MN-major operand, 128-byte swizzle: rows (K index) of 64 elements = 128 B, 8-row atoms 1024 B apart (SBO); further
+// 64-element blocks along M/N are `lbo_bytes` apart (LBO).  16 K rows (one k16 step) are 2048 bytes.
+__device__ __forceinline__ uint64_t gmma_desc_mnmajor_sw128(uint32_t smem_addr, uint32_t lbo_bytes) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr >> 4) & 0x3fffu);
+  d |= (uint64_t)((lbo_bytes >> 4) & 0x3fffu) << 16;
+  d |= (uint64_t)(1024u >> 4) << 32;
+  d |= (uint64_t)1 << 62;
+  return d;
+}
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// named barrier of the consumer warpgroup (threads 0..127 of every tensor-core kernel)
+__device__ __forceinline__ void wg_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
+
+// A 128 x N fp32 accumulator held by one warpgroup as two m64 fragments: h[0] = rows 0-63, h[1] = rows 64-127.
+// In fragment h, thread t (warp w = t / 32, lane l) holds for every 8-column block i the elements
+//   [4i]   (16w + l/4,     8i + 2(l%4))   [4i+1] (same row, column + 1)
+//   [4i+2] (16w + l/4 + 8, 8i + 2(l%4))   [4i+3] (same row, column + 1).
+template <int N>
+struct Acc128 {
+  float h[2][N / 2];
+  // d += A . B^T over one k16 step; a0 / a1 describe rows 0-63 / 64-127 of A
+  template <bool F16 = false, int TA = 0, int TB = 0>
+  __device__ __forceinline__ void mma(uint64_t a0, uint64_t a1, uint64_t b, uint32_t accumulate) {
+    Wgmma<N, F16, TA, TB>::mma(h[0], a0, b, accumulate);
+    Wgmma<N, F16, TA, TB>::mma(h[1], a1, b, accumulate);
+  }
+  // keeps the compiler from moving accumulator accesses across the asynchronous MMAs
+  __device__ __forceinline__ void fence_operands() {
+#pragma unroll
+    for (int j = 0; j < 2; ++j)
+#pragma unroll
+      for (int i = 0; i < N / 2; ++i) asm volatile("" : "+f"(h[j][i])::"memory");
+  }
+  // Row-per-thread view of 32 accumulator columns [32 ch, 32 ch + 32): thread t of the warpgroup receives row t.
+  // The fragments go through `stg` (128 rows x ACC_STG_PITCH floats of shared memory); every thread of the warpgroup
+  // must call this with the same ch.
+  __device__ __forceinline__ void rows32(int ch, float* stg, uint32_t (&raw)[32]) const;
+};
+constexpr int ACC_STG_PITCH = 36;                          // 144-byte rows: conflict-free 16-byte row reads
+constexpr int ACC_STG_BYTES = 128 * ACC_STG_PITCH * 4;
+
+template <int N>
+__device__ __forceinline__ void Acc128<N>::rows32(int ch, float* stg, uint32_t (&raw)[32]) const {
+  const int t = threadIdx.x & 127, w = t >> 5, l = t & 31;
+  wg_sync();                                               // the previous chunk's reads are done
+#pragma unroll
+  for (int j = 0; j < 2; ++j)
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int r = 64 * j + 16 * w + (l >> 2), c = 8 * i + 2 * (l & 3);
+      const float* f = &h[j][4 * (4 * ch + i)];
+      *reinterpret_cast<float2*>(stg + r * ACC_STG_PITCH + c) = make_float2(f[0], f[1]);
+      *reinterpret_cast<float2*>(stg + (r + 8) * ACC_STG_PITCH + c) = make_float2(f[2], f[3]);
+    }
+  wg_sync();
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const float4 v = *reinterpret_cast<const float4*>(stg + t * ACC_STG_PITCH + 4 * i);
+    raw[4 * i] = __float_as_uint(v.x); raw[4 * i + 1] = __float_as_uint(v.y);
+    raw[4 * i + 2] = __float_as_uint(v.z); raw[4 * i + 3] = __float_as_uint(v.w);
+  }
 }
 
 // ---- host: TMA descriptor encoding through the driver entry point (no libcuda link) -----------

@@ -1,4 +1,4 @@
-// 3x3 / stride 1 / pad 1 convolution as a tcgen05 implicit GEMM (reference: the 12 convs
+// 3x3 / stride 1 / pad 1 convolution as a Hopper wgmma implicit GEMM (reference: the 12 convs
 // conv1_2..conv5_3 of ibl/models/vgg.py:40-42,61-62, cuDNN in the reference).
 //
 //   M = output pixels (128 per tile: TH x TW patch of one image)
@@ -7,17 +7,17 @@
 //
 // fp32 parity on a tensor core without an fp32 mode: every fp32 operand is carried as two bf16
 // planes (hi = bf16(x), lo = bf16(x - hi)) and each K-chunk issues three MMAs
-//   A_hi.B_hi + A_hi.B_lo + A_lo.B_hi      (fp32 accumulation in TMEM),
+//   A_lo.B_hi + A_hi.B_lo + A_hi.B_hi      (fp32 accumulation in registers),
 // dropping only the lo.lo term (~2^-16 relative).  Activations live in HBM as NHWC bf16 hi/lo
 // planes, weights as [tap][Cout][Cin] hi/lo planes, so every operand tile is one TMA box:
 // the activation box for tap (kh,kw) is the output patch shifted by (kh-1,kw-1) and the
 // hardware zero-fills the out-of-image part, which is exactly the conv's zero padding.
 //
-// Warp roles (192 threads, persistent over tiles):
-//   warp 0  TMA producer      warp 1  MMA issuer + TMEM owner      warps 2-5  epilogue
-// Two TMEM accumulator buffers let the epilogue of tile i overlap the main loop of tile i+1.
-// Epilogue: TMEM -> registers, + bias, ReLU, optional fused 2x2 max-pool (warp shuffles),
-// split into hi/lo planes (or fp32 for conv5_3), 16-byte stores.
+// Warp roles (160 threads, persistent over tiles):
+//   warps 0-3  consumer warpgroup: wgmma main loop (two m64 halves of the 128-pixel tile), then the epilogue
+//   warp 4     TMA producer
+// Epilogue: accumulator -> row-per-thread views (Acc128::rows32), + bias, ReLU, optional fused 2x2 max-pool
+// (warp shuffles), split into hi/lo planes (or fp32 for conv5_3), 16-byte stores.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -88,57 +88,27 @@ struct ConvTcArgs {
   float* y_f32;
   float* ssq;             // optional [n_tiles][N*H*W] per-pixel sum of squares of the outputs (no pool)
   long long ssq_stride;
-  float acc_scale;        // compensation of the tcgen05 accumulator's round-toward-zero bias (see tc_acc_scale)
+  float acc_scale;        // optional accumulator compensation factor (see tc_acc_scale)
 };
 
-// The tcgen05 fp32 accumulator truncates toward zero: every accumulating MMA loses on average 2^-26 of the running
-// sum (measured per layer shape, profiles/r01_diag_tc_accumulator_bias.txt: -1.31e-8 .. -1.38e-8 per MMA with ReLU'd
-// inputs, linear in the number of MMAs from 108 to 864).  Over the 12 layers that is one uniform factor (1 - 9e-5) on
-// the conv5_3 map -- harmless after the L2 normalisations, but it put VGG.forward's own output outside the 1e-4
-// tolerance.  The epilogue multiplies the accumulator by 1 + n_mma * 1.32e-8 (n_mma = MMAs accumulated into the
-// dominant accumulator block) before the bias is added.  IBL_TC_BIAS_COMP=0 switches it off (diagnosis).
-static float tc_acc_scale(int cin, bool concat) {
-  static const bool on = [] { const char* v = getenv("IBL_TC_BIAS_COMP"); return !v || atoi(v) != 0; }();
-  if (!on) return 1.f;
-  const int n_mma = (concat ? 9 : 27) * (cin / 16);
-  return 1.f + (float)n_mma * 1.32e-8f;
+// Optional compensation of a tensor-core accumulator that rounds toward zero: the epilogue multiplies the accumulator
+// by 1 + n_mma * c (n_mma = k16 MMA steps accumulated into the tile) before the bias is added.  IBL_TC_BIAS_COMP=<c>
+// sets c (default 0: the sm_90 accumulator needs no compensation at the 1e-4 descriptor tolerance).
+static float tc_acc_scale(int cin) {
+  static const float c = [] { const char* v = getenv("IBL_TC_BIAS_COMP"); return v ? (float)atof(v) : 0.f; }();
+  return 1.f + (float)(27 * (cin / 16)) * c;
 }
-
-constexpr int TC_BM = 128;
-constexpr int TC_BK = 64;                       // bf16 elements per K-chunk = one 128-byte row
-constexpr int TC_A_BYTES = TC_BM * TC_BK * 2;   // 16 KiB per plane
-
-// PAIR: the CTA is one half of an SM pair (tcgen05.mma.cta_group::2, 256-pixel M tile): it stages its own
-// 128-pixel patch and HALF of the BN-wide weight tile; per stage and SM the TMA fill drops from 96 to 64 KiB
-// (BN = 256) and the tensor core reads half of B from the peer's shared memory.
-//
-// HALO: instead of one [128 px][64 ch] im2col box per tap, the producer stages ONE halo tile per 64-channel
-// chunk -- the (16+2) x (8+2) pixel neighbourhood of a 16x8 patch, 180 rows of 128 B per plane -- and the
-// nine taps are nine views of it: tap (kh,kw) starts (kh*10 + kw) rows into the tile and consecutive 8-pixel
-// row groups are 10 rows (1280 B) apart.  The 128B swizzle is a pure function of the shared-memory address,
-// so a descriptor whose start is only 128-byte aligned and whose group stride is not a multiple of 1024 B
-// reads the TMA-written tile correctly (probed on hardware: tc_probe.cu / tools/probe_umma_stride.py).
-// L2->SM traffic of the A operand drops from 9 x 32 KiB to 45 KiB per chunk; the weights get their own ring.
-constexpr int TC_HALO_W = 10, TC_HALO_H = 18;
-constexpr int TC_HALO_PLANE = 23 * 1024;        // 180 rows x 128 B = 23040 B, padded to the swizzle period
-constexpr int TC_HALO_STAGE = 2 * TC_HALO_PLANE;
-template <int BN, bool PAIR = false, bool HALO = false, int NA = 0>
-struct ConvTcSmem {
-  static constexpr int B_BYTES = (PAIR ? BN / 2 : BN) * TC_BK * 2;
-  static constexpr int STAGE_BYTES = HALO ? 2 * B_BYTES : 2 * TC_A_BYTES + 2 * B_BYTES;
-  static constexpr int A_RING = HALO ? NA * TC_HALO_STAGE : 0;
-};
 
 __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
   __nv_bfloat162 t = __floats2bfloat162_rn(a, b);
   return *reinterpret_cast<uint32_t*>(&t);
 }
 
-// One accumulator tile (this warp's 32 pixel rows x BN output channels) from TMEM to global memory:
+// One accumulator tile (128 pixel rows x BN output channels, thread = pixel row) to global memory:
 // bias + ReLU + fused 2x2 max-pool + bf16 hi/lo split (or fp32), optional per-pixel sum of squares.
-template <int BN, bool kConcat>
-__device__ __forceinline__ void conv_epilogue_tile(const ConvTcArgs& a, uint32_t t_row, int img, int h0, int w0, int n0,
-                                                   int nt, int r, int c, int TW) {
+template <int BN>
+__device__ __forceinline__ void conv_epilogue_tile(const ConvTcArgs& a, const Acc128<BN>& acc, float* stg, int img, int h0,
+                                                   int w0, int n0, int nt, int r, int c, int TW) {
   const int h = h0 + r, w = w0 + c;
   bool valid;
   long long pix;
@@ -152,20 +122,10 @@ __device__ __forceinline__ void conv_epilogue_tile(const ConvTcArgs& a, uint32_t
     pix = ((long long)img * a.H + h) * a.W + w;
   }
   float ssq_acc = 0.f;   // per-pixel sum of squares over this N tile (feeds NetVLAD's input norm)
-#pragma unroll 1
-  for (int ch = 0; ch < BN / 32; ++ch) {
-    uint32_t raw[32];
-    tmem_ld_32x32(t_row + ch * 32, raw);
-    if (kConcat) {   // add the hi.lo and lo.hi blocks (fp32, small terms first)
-      uint32_t r1[32], r2[32];
-      tmem_ld_32x32(t_row + BN + ch * 32, r1);
-      tmem_ld_32x32(t_row + 2 * BN + ch * 32, r2);
-      tmem_ld_wait();
 #pragma unroll
-      for (int j = 0; j < 32; ++j)
-        raw[j] = __float_as_uint((__uint_as_float(r1[j]) + __uint_as_float(r2[j])) + __uint_as_float(raw[j]));
-    }
-    tmem_ld_wait();
+  for (int ch = 0; ch < BN / 32; ++ch) {     // unrolled: the accumulator is indexed with constants only
+    uint32_t raw[32];
+    acc.rows32(ch, stg, raw);
     if (a.pool) {
       // 2x2 max-pool BEFORE bias / ReLU / split (fmaf(., scale > 0, b) and max(., 0) are monotone, so the results are
       // the same bits) as a two-step exchange: against the w-neighbour (lane ^ 1) every lane keeps one half of the 32
@@ -264,111 +224,116 @@ __device__ __forceinline__ void conv_epilogue_tile(const ConvTcArgs& a, uint32_t
   if (a.ssq && valid && !a.pool) a.ssq[(long long)nt * a.ssq_stride + pix] = ssq_acc;
 }
 
-template <int BN, int STAGES, bool PAIR, bool HALO, int NA>
-__global__ void __launch_bounds__(192, 1)
+constexpr int TC_BM = 128;
+constexpr int TC_BK = 64;                       // bf16 elements per K-chunk = one 128-byte row
+constexpr int TC_A_BYTES = TC_BM * TC_BK * 2;   // 16 KiB per plane
+
+// HALO: instead of one [128 px][64 ch] im2col box per tap, the producer stages ONE halo tile per 64-channel
+// chunk -- the (16+2) x (8+2) pixel neighbourhood of a 16x8 patch, 180 rows of 128 B per plane -- and the
+// nine taps are nine views of it: tap (kh,kw) starts (kh*10 + kw) rows into the tile and consecutive 8-pixel
+// row groups are 10 rows (1280 B) apart.  The 128B swizzle is a function of the shared-memory address, so a
+// descriptor whose start is only 128-byte aligned and whose group stride is not a multiple of 1024 B reads the
+// TMA-written tile correctly (pinned on hardware by tests/test_gpu_variants.py through tc_probe.cu).
+// L2->SM traffic of the A operand drops from 9 x 32 KiB to 45 KiB per chunk; the weights get their own ring.
+constexpr int TC_HALO_W = 10, TC_HALO_H = 18;
+constexpr int TC_HALO_PLANE = 23 * 1024;        // 180 rows x 128 B = 23040 B, padded to the swizzle period
+constexpr int TC_HALO_STAGE = 2 * TC_HALO_PLANE;
+
+template <int BN, int STAGES, bool HALO = false, int NA = 0>
+struct ConvTcSmem {
+  static constexpr int B_BYTES = BN * TC_BK * 2;
+  static constexpr int STAGE_BYTES = HALO ? 2 * B_BYTES : 2 * TC_A_BYTES + 2 * B_BYTES;
+  static constexpr int A_RING = HALO ? NA * TC_HALO_STAGE : 0;
+  static constexpr int BYTES = A_RING + STAGES * STAGE_BYTES + ACC_STG_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+};
+
+// PAIR: the grid is launched as clusters of two CTAs ("SM pairs") that share one work item = (two adjacent patches, one
+// N tile).  Each CTA stages its own activations and fetches only HALF of every weight tap, TMA-multicasting it into both
+// CTAs' shared memory: the per-SM L2->SM weight traffic halves.  A weight slot may be refilled only when the consumers
+// of BOTH CTAs have released it (arrival count 8: every consumer warp arrives on both CTAs' barriers).
+template <int BN, int STAGES, bool HALO, int NA, bool PAIR>
+__global__ void __launch_bounds__(160, 1)
 conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tm_xhi, const __grid_constant__ CUtensorMap tm_xlo,
                   const __grid_constant__ CUtensorMap tm_whi, const __grid_constant__ CUtensorMap tm_wlo,
                   const ConvTcArgs a) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // 1024-byte alignment is required by the 128B swizzle; dynamic smem base is only 16B-aligned
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  constexpr int B_BYTES = ConvTcSmem<BN, PAIR, HALO, NA>::B_BYTES;
-  constexpr int STAGE_BYTES = ConvTcSmem<BN, PAIR, HALO, NA>::STAGE_BYTES;
-  constexpr int A_RING = ConvTcSmem<BN, PAIR, HALO, NA>::A_RING;
-  uint8_t* ring = smem + A_RING;              // HALO: the halo ring sits in front of the weight ring
-  static_assert(!(PAIR && BN == 64), "the pair variant is for BN = 128 / 256");
-  const uint32_t rank = PAIR ? cluster_ctarank() : 0u;
-  const bool leader = rank == 0;
-  // pair mode: the two CTAs of a cluster share one work item = (two adjacent patches, one N tile)
-  const int worker = PAIR ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-  const int n_workers = PAIR ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(ring + STAGES * STAGE_BYTES);
+  using L = ConvTcSmem<BN, STAGES, HALO, NA>;
+  constexpr int B_BYTES = L::B_BYTES;
+  constexpr int STAGE_BYTES = L::STAGE_BYTES;
+  constexpr int A_RING = L::A_RING;           // HALO: the halo ring sits in front of the weight ring
+  uint8_t* ring = smem + A_RING;
+  float* stg = reinterpret_cast<float*>(ring + STAGES * STAGE_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(ring + STAGES * STAGE_BYTES + ACC_STG_BYTES);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + STAGES;
-  uint64_t* tfull_bar = bars + 2 * STAGES;
-  uint64_t* tempty_bar = bars + 2 * STAGES + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
-  uint64_t* afull_bar = bars + 2 * STAGES + 5;          // HALO only: [NA] + [NA]
+  uint64_t* afull_bar = bars + 2 * STAGES;    // HALO only: [NA] + [NA]
   uint64_t* aempty_bar = afull_bar + NA;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // BN = 64 (conv1_2): an M=128,N=64 MMA is bound by the 4 KiB shared-memory read of its A operand
-  // (128 B/clk).  B_hi and B_lo are adjacent in the stage, so ONE N=128 MMA  A_hi . [B_hi;B_lo]^T
-  // yields hi.hi (columns 0-63) and hi.lo (64-127) for a single read of A_hi; A_lo.B_hi goes to a
-  // third 64-column block.  Per 16-wide K step: 64 + 48 clk instead of 3 x 48.  The epilogue adds the
-  // three blocks.  ACC_COLS = TMEM columns per accumulator buffer.
-  constexpr bool kConcat = (BN == 64);
-  constexpr uint32_t ACC_COLS = kConcat ? 3 * BN : BN;
-  constexpr uint32_t TMEM_COLS = kConcat ? 512 : 2 * BN;  // a power of two >= 32
-
-  if (warp == 0 && lane == 0) {
+  const uint32_t rank = PAIR ? cluster_ctarank() : 0u;
+  const int worker = PAIR ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
+  const int n_workers = PAIR ? (int)(gridDim.x >> 1) : (int)gridDim.x;
+  if (warp == 4 && lane == 0) {
     tma_prefetch_desc(&tm_xhi);
     tma_prefetch_desc(&tm_xlo);
     tma_prefetch_desc(&tm_whi);
     tma_prefetch_desc(&tm_wlo);
     for (int i = 0; i < STAGES; ++i) {
-      mbar_init(&full_bar[i], 1);    // pair: the leader's arrive.expect_tx covers both CTAs' bytes; the peer only loads (tc_dist1.cu)
-      mbar_init(&empty_bar[i], 1);
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], PAIR ? 8 : 4);   // one arrival per consumer warp (of both CTAs of a pair)
     }
     for (int i = 0; i < NA; ++i) {
       mbar_init(&afull_bar[i], 1);
-      mbar_init(&aempty_bar[i], 1);
+      mbar_init(&aempty_bar[i], 4);
     }
-    mbar_init(&tfull_bar[0], 1);
-    mbar_init(&tfull_bar[1], 1);
-    mbar_init(&tempty_bar[0], PAIR ? 8 : 4);    // pair: the epilogue warps of both CTAs (leader's barrier)
-    mbar_init(&tempty_bar[1], PAIR ? 8 : 4);
     fence_barrier_init();
     fence_proxy_async();
   }
-  if (warp == 1) {
-    if (PAIR) {
-      tmem_alloc_2sm(tmem_slot, TMEM_COLS);
-    } else {
-      tmem_alloc(tmem_slot, TMEM_COLS);
-      tmem_relinquish();
-    }
-  }
-  tc_fence_before();
   __syncthreads();
-  if (PAIR) cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  if (PAIR) cluster_sync_all();     // the peer's barriers exist before anything is multicast into this CTA
 
   const int TW = 1 << a.tw_log2;
   const int kchunks = a.cin / TC_BK;
   const int kiters = 9 * kchunks;
   const int tiles_per_img = a.tiles_h * a.tiles_w;
+  auto coords = [&](int tile, int& img, int& h0, int& w0, int& nt) {
+    nt = tile % a.n_tiles;
+    // pair: an odd patch count leaves img == N for the last peer: TMA zero-fills, the epilogue stores nothing
+    const int pt = PAIR ? 2 * (tile / a.n_tiles) + (int)rank : tile / a.n_tiles;
+    img = pt / tiles_per_img;
+    const int rem = pt - img * tiles_per_img;
+    h0 = (rem / a.tiles_w) * (TC_BM >> a.tw_log2);
+    w0 = (rem % a.tiles_w) * TW;
+  };
 
-  if (warp == 0) {
-    // ================= TMA producer =================
-    // same discipline as the MMA issuer below: convergent warp, one elected lane issues, ring positions / coordinates warp-uniform
-    {
-      const uint32_t smem_a = warp_uniform(smem_u32(smem));
-      const uint32_t ring_a = smem_a + A_RING;
-      const uint32_t bars_a = ring_a + STAGES * STAGE_BYTES;
-      const uint32_t full_a = bars_a, empty_a = bars_a + 8 * STAGES;
-      const uint32_t afull_a = bars_a + 8 * (2 * STAGES + 5), aempty_a = afull_a + 8 * NA;
-      // pair: all bytes of a stage are accounted on the LEADER's barrier, named by its shared::cluster address
-      const uint32_t full_c = PAIR ? warp_uniform(mapa_u32(full_a, 0)) : full_a;
-      const uint32_t afull_c = PAIR ? warp_uniform(mapa_u32(afull_a, 0)) : afull_a;
-      (void)afull_a; (void)aempty_a; (void)afull_c;
-      const uint32_t rank_u = warp_uniform(rank);
-      int stage = 0, astage = 0;
-      uint32_t phase = 0, aphase = 0;
-      (void)astage; (void)aphase;
-      auto coords = [&](int tile, int& img, int& h0, int& w0, int& n0) {
-        const int nt = tile % a.n_tiles;
-        const int pt = PAIR ? 2 * (tile / a.n_tiles) + (int)rank_u : tile / a.n_tiles;
-        img = pt / tiles_per_img;               // pair: an odd patch count leaves img == N for the last peer:
-        const int rem = pt - img * tiles_per_img;     // TMA zero-fills, the epilogue stores nothing
-        h0 = (rem / a.tiles_w) * (TC_BM >> a.tw_log2);
-        w0 = (rem % a.tiles_w) * TW;
-        n0 = PAIR ? nt * BN + (int)rank_u * (BN / 2) : nt * BN;
-        img = (int)warp_uniform((uint32_t)img); h0 = (int)warp_uniform((uint32_t)h0);
-        w0 = (int)warp_uniform((uint32_t)w0); n0 = (int)warp_uniform((uint32_t)n0);
-      };
-      // lane 0 polls once; the answer is broadcast so that the branch on it is warp-uniform
+  if (warp == 4) {
+    // ================= TMA producer: convergent warp, one elected lane issues, coordinates warp-uniform =================
+    const uint32_t smem_a = warp_uniform(smem_u32(smem));
+    const uint32_t ring_a = smem_a + A_RING;
+    const uint32_t bars_a = ring_a + STAGES * STAGE_BYTES + ACC_STG_BYTES;
+    const uint32_t full_a = bars_a, empty_a = bars_a + 8 * STAGES;
+    const uint32_t afull_a = bars_a + 16 * STAGES, aempty_a = afull_a + 8 * NA;
+    const int rank_u = (int)warp_uniform(rank);
+    // the two weight planes of one tap (into `st`, planes B_BYTES apart); a pair's CTAs each fetch one half of the rows
+    auto load_w = [&](uint32_t st, uint32_t fb, int c0, int n0, int tap) {
+      if (PAIR) {
+        constexpr int HB = B_BYTES / 2;
+        tma_load_3d_mc_a(st + rank_u * HB, &tm_whi, fb, c0, n0 + rank_u * (BN / 2), tap, 0x3);
+        tma_load_3d_mc_a(st + B_BYTES + rank_u * HB, &tm_wlo, fb, c0, n0 + rank_u * (BN / 2), tap, 0x3);
+      } else {
+        tma_load_3d_a(st, &tm_whi, fb, c0, n0, tap);
+        tma_load_3d_a(st + B_BYTES, &tm_wlo, fb, c0, n0, tap);
+      }
+    };
+    int stage = 0;
+    uint32_t phase = 0;
+    if constexpr (HALO) {
+      // Two independent streams -- halo tiles (one per tile and 64-channel chunk) and weight taps (nine per halo) --
+      // each issued as soon as its ring has a free slot, so the halo of the NEXT chunk is in flight while the taps of
+      // the current one are still being fed.  Lane 0 polls once; the answer is broadcast so that the branch on it is
+      // warp-uniform.
       auto try_wait_warp = [&](uint32_t bar, uint32_t parity) -> bool {
         uint32_t ok = 0;
         if (lane == 0) {
@@ -384,286 +349,208 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tm_xhi, const __grid_const
         }
         return warp_uniform(ok) != 0;
       };
-      (void)try_wait_warp;
-      if constexpr (HALO) {
-        // Two independent streams -- halo tiles (one per tile and 64-channel chunk) and weight taps (nine per
-        // halo) -- each issued as soon as its ring has a free slot, so the halo of the NEXT chunk is in flight
-        // while the taps of the current one are still being fed.
-        int tA = worker, kcA = 0, tB = worker, kcB = 0, tapB = 0;
-        while (tB < a.total_tiles) {
-          const uint32_t as_u = warp_uniform((uint32_t)astage);
-          if (tA < a.total_tiles && try_wait_warp(aempty_a + 8 * as_u, aphase ^ 1)) {
-            int img, h0, w0, n0;
-            coords(tA, img, h0, w0, n0);
-            (void)n0;
-            const int c0 = (int)warp_uniform((uint32_t)(kcA * TC_BK));
-            const uint32_t sa = smem_a + as_u * TC_HALO_STAGE;
-            constexpr uint32_t kHaloBytes = 2u * TC_HALO_W * TC_HALO_H * 128u;
-            if (elect_one()) {
-              if (PAIR) {
-                if (leader) mbar_arrive_expect_tx_a(afull_a + 8 * as_u, 2 * kHaloBytes);
-                tma_load_4d_2sm_a(sa, &tm_xhi, afull_c + 8 * as_u, c0, w0 - 1, h0 - 1, img);
-                tma_load_4d_2sm_a(sa + TC_HALO_PLANE, &tm_xlo, afull_c + 8 * as_u, c0, w0 - 1, h0 - 1, img);
-              } else {
-                mbar_arrive_expect_tx_a(afull_a + 8 * as_u, kHaloBytes);
-                tma_load_4d_a(sa, &tm_xhi, afull_a + 8 * as_u, c0, w0 - 1, h0 - 1, img);
-                tma_load_4d_a(sa + TC_HALO_PLANE, &tm_xlo, afull_a + 8 * as_u, c0, w0 - 1, h0 - 1, img);
-              }
-            }
-            __syncwarp();
-            if (++astage == NA) { astage = 0; aphase ^= 1; }
-            if (++kcA == kchunks) { kcA = 0; tA += n_workers; }
-            continue;
+      int astage = 0;
+      uint32_t aphase = 0;
+      int tA = worker, kcA = 0, tB = worker, kcB = 0, tapB = 0;
+      while (tB < a.total_tiles) {
+        const uint32_t as_u = warp_uniform((uint32_t)astage);
+        if (tA < a.total_tiles && try_wait_warp(aempty_a + 8 * as_u, aphase ^ 1)) {
+          int img, h0, w0, nt;
+          coords(tA, img, h0, w0, nt);
+          img = (int)warp_uniform((uint32_t)img); h0 = (int)warp_uniform((uint32_t)h0);
+          w0 = (int)warp_uniform((uint32_t)w0);
+          const int c0 = (int)warp_uniform((uint32_t)(kcA * TC_BK));
+          const uint32_t sa = smem_a + as_u * TC_HALO_STAGE;
+          constexpr uint32_t kHaloBytes = 2u * TC_HALO_W * TC_HALO_H * 128u;
+          if (elect_one()) {
+            mbar_arrive_expect_tx_a(afull_a + 8 * as_u, kHaloBytes);
+            tma_load_4d_a(sa, &tm_xhi, afull_a + 8 * as_u, c0, w0 - 1, h0 - 1, img);
+            tma_load_4d_a(sa + TC_HALO_PLANE, &tm_xlo, afull_a + 8 * as_u, c0, w0 - 1, h0 - 1, img);
           }
-          const uint32_t st_u = warp_uniform((uint32_t)stage);
-          if (try_wait_warp(empty_a + 8 * st_u, phase ^ 1)) {
-            int img, h0, w0, n0;
-            coords(tB, img, h0, w0, n0);
-            const int c0 = (int)warp_uniform((uint32_t)(kcB * TC_BK));
-            const int tap = (int)warp_uniform((uint32_t)tapB);
-            const uint32_t st = ring_a + st_u * STAGE_BYTES;
-            if (elect_one()) {
-              if (PAIR) {
-                if (leader) mbar_arrive_expect_tx_a(full_a + 8 * st_u, 2 * STAGE_BYTES);
-                tma_load_3d_2sm_a(st, &tm_whi, full_c + 8 * st_u, c0, n0, tap);
-                tma_load_3d_2sm_a(st + B_BYTES, &tm_wlo, full_c + 8 * st_u, c0, n0, tap);
-              } else {
-                mbar_arrive_expect_tx_a(full_a + 8 * st_u, STAGE_BYTES);
-                tma_load_3d_a(st, &tm_whi, full_a + 8 * st_u, c0, n0, tap);
-                tma_load_3d_a(st + B_BYTES, &tm_wlo, full_a + 8 * st_u, c0, n0, tap);
-              }
-            }
-            __syncwarp();
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
-            if (++tapB == 9) { tapB = 0; if (++kcB == kchunks) { kcB = 0; tB += n_workers; } }
-          }
+          __syncwarp();
+          if (++astage == NA) { astage = 0; aphase ^= 1; }
+          if (++kcA == kchunks) { kcA = 0; tA += n_workers; }
+          continue;
         }
-      } else {
-        for (int tile = worker; tile < a.total_tiles; tile += n_workers) {
-          int img, h0, w0, n0;
-          coords(tile, img, h0, w0, n0);
-          for (int kit = 0; kit < kiters; ++kit) {
-            const int tap = (int)warp_uniform((uint32_t)(kit / kchunks));
-            const int c0 = (int)warp_uniform((uint32_t)((kit - tap * kchunks) * TC_BK));
-            const int kh = tap / 3 - 1, kw = tap % 3 - 1;
-            const uint32_t st_u = warp_uniform((uint32_t)stage);
-            mbar_wait_warp_a(empty_a + 8 * st_u, phase ^ 1);
-            const uint32_t st = smem_a + st_u * STAGE_BYTES;
-            if (elect_one()) {
-              if (PAIR) {
-                const uint32_t fb = full_c + 8 * st_u;
-                if (leader) mbar_arrive_expect_tx_a(full_a + 8 * st_u, 2 * STAGE_BYTES);   // bytes of both CTAs
-                tma_load_4d_2sm_a(st, &tm_xhi, fb, c0, w0 + kw, h0 + kh, img);
-                tma_load_4d_2sm_a(st + TC_A_BYTES, &tm_xlo, fb, c0, w0 + kw, h0 + kh, img);
-                tma_load_3d_2sm_a(st + 2 * TC_A_BYTES, &tm_whi, fb, c0, n0, tap);
-                tma_load_3d_2sm_a(st + 2 * TC_A_BYTES + B_BYTES, &tm_wlo, fb, c0, n0, tap);
-              } else {
-                const uint32_t fb = full_a + 8 * st_u;
-                mbar_arrive_expect_tx_a(fb, STAGE_BYTES);
-                tma_load_4d_a(st, &tm_xhi, fb, c0, w0 + kw, h0 + kh, img);
-                tma_load_4d_a(st + TC_A_BYTES, &tm_xlo, fb, c0, w0 + kw, h0 + kh, img);
-                tma_load_3d_a(st + 2 * TC_A_BYTES, &tm_whi, fb, c0, n0, tap);
-                tma_load_3d_a(st + 2 * TC_A_BYTES + B_BYTES, &tm_wlo, fb, c0, n0, tap);
-              }
-            }
-            __syncwarp();
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        const uint32_t st_u = warp_uniform((uint32_t)stage);
+        if (try_wait_warp(empty_a + 8 * st_u, phase ^ 1)) {
+          int img, h0, w0, nt;
+          coords(tB, img, h0, w0, nt);
+          const int n0 = (int)warp_uniform((uint32_t)(nt * BN));
+          const int c0 = (int)warp_uniform((uint32_t)(kcB * TC_BK));
+          const int tap = (int)warp_uniform((uint32_t)tapB);
+          const uint32_t st = ring_a + st_u * STAGE_BYTES;
+          if (elect_one()) {
+            mbar_arrive_expect_tx_a(full_a + 8 * st_u, STAGE_BYTES);
+            load_w(st, full_a + 8 * st_u, c0, n0, tap);
           }
+          __syncwarp();
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+          if (++tapB == 9) { tapB = 0; if (++kcB == kchunks) { kcB = 0; tB += n_workers; } }
         }
       }
+    } else
+    for (int tile = worker; tile < a.total_tiles; tile += n_workers) {
+      int img, h0, w0, nt;
+      coords(tile, img, h0, w0, nt);
+      img = (int)warp_uniform((uint32_t)img); h0 = (int)warp_uniform((uint32_t)h0);
+      w0 = (int)warp_uniform((uint32_t)w0);
+      const int n0 = (int)warp_uniform((uint32_t)(nt * BN));
+      for (int kit = 0; kit < kiters; ++kit) {
+        const int tap = (int)warp_uniform((uint32_t)(kit / kchunks));
+        const int c0 = (int)warp_uniform((uint32_t)((kit - tap * kchunks) * TC_BK));
+        const int kh = tap / 3 - 1, kw = tap % 3 - 1;
+        const uint32_t st_u = warp_uniform((uint32_t)stage);
+        mbar_wait_warp_a(empty_a + 8 * st_u, phase ^ 1);
+        const uint32_t st = smem_a + st_u * STAGE_BYTES;
+        if (elect_one()) {
+          const uint32_t fb = full_a + 8 * st_u;
+          mbar_arrive_expect_tx_a(fb, STAGE_BYTES);
+          tma_load_4d_a(st, &tm_xhi, fb, c0, w0 + kw, h0 + kh, img);
+          tma_load_4d_a(st + TC_A_BYTES, &tm_xlo, fb, c0, w0 + kw, h0 + kh, img);
+          load_w(st + 2 * TC_A_BYTES, fb, c0, n0, tap);
+        }
+        __syncwarp();
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
     }
-  } else if (warp == 1) {
-    // ================= MMA issuer =================
-    // The whole warp walks the schedule in convergent code; ONE ELECTED lane (elect.sync) executes the tcgen05
-    // instructions of a stage, and the ring position, TMEM base and shared-memory base pass through a REDUX
-    // (warp_uniform) once per stage, so every operand lives in a uniform register.  With the loop inside
-    // `if (lane == 0)` ptxas (a) treated descriptors and TMEM addresses as per-thread values (5 R2UR.BROADCASTs per MMA)
-    // and (b) wrapped EACH MMA in an ELECT / PLOP3 / BRA.U.ANY loop over the possibly-several active threads: ~90 clk of
-    // dependent issue per MMA (ncu source view of the fused conv1 kernel: the issuing thread was busy 75 % of the time
-    // with the tensor pipe 40 % active), more than an N <= 128 MMA occupies the tensor pipe.  Behind elect.sync the
-    // MMAs of a stage are consecutive UTCHMMA instructions.
-    if (warp_uniform(leader ? 1u : 0u)) {
-      const uint32_t tmem_u = warp_uniform(tmem_base);
-      const uint32_t smem_a = warp_uniform(smem_u32(smem));
-      const uint32_t ring_a = smem_a + A_RING;
-      const uint32_t bars_a = ring_a + STAGES * STAGE_BYTES;
-      const uint32_t full_a = bars_a, empty_a = bars_a + 8 * STAGES;
-      const uint32_t tfull_a = bars_a + 16 * STAGES, tempty_a = tfull_a + 16;
-      const uint32_t afull_a = bars_a + 8 * (2 * STAGES + 5), aempty_a = afull_a + 8 * NA;
-      (void)afull_a; (void)aempty_a;
-      constexpr uint32_t idesc = umma_idesc_bf16_f32(PAIR ? 2 * TC_BM : TC_BM, BN);
-      auto commit = [&](uint32_t bar) {
-        if (PAIR) umma_commit_2sm_mc_a(bar, 0x3);
-        else umma_commit_a(bar);
-      };
-      auto mma_step = [&](uint32_t d_tmem, uint64_t a_hi, uint64_t a_lo, uint64_t b_hi, uint64_t b_lo, bool fresh) {
+  } else {
+    // ================= consumer warpgroup: main loop + epilogue =================
+    const int m = threadIdx.x;              // accumulator row = pixel index inside the patch
+    const int r = m >> a.tw_log2, c = m & (TW - 1);
+    const uint32_t smem_a = smem_u32(smem);
+    const uint32_t ring_a = smem_a + A_RING;
+    int stage = 0, astage = 0;
+    uint32_t phase = 0, aphase = 0;
+    (void)ring_a; (void)astage; (void)aphase;
+    auto release_w = [&](int st) {          // this warp is done reading weight slot st (in both CTAs' rings of a pair)
+      if (lane == 0) {
+        mbar_arrive(&empty_bar[st]);
+        if (PAIR) mbar_arrive_remote(mapa_u32(smem_u32(&empty_bar[st]), rank ^ 1u));
+      }
+    };
+    for (int tile = worker; tile < a.total_tiles; tile += n_workers) {
+      int img, h0, w0, nt;
+      coords(tile, img, h0, w0, nt);
+      Acc128<BN> acc;
+      int prev = -1;
+      if constexpr (HALO) {
+        // K-major SW128 view of the halo tile: 8-pixel row groups 10 rows apart; pixel rows 64-127 = groups 8-15
+        constexpr uint64_t kHaloDesc = ((uint64_t)1 << 16) | ((uint64_t)((TC_HALO_W * 128) >> 4) << 32) | ((uint64_t)1 << 62);
+        constexpr uint64_t kHalf = 8 * TC_HALO_W * 128 / 16;
+        for (int kc = 0; kc < kchunks; ++kc) {
+          mbar_wait(&afull_bar[astage], aphase);
+          const uint32_t ha = smem_a + astage * TC_HALO_STAGE;
+          for (int tap = 0; tap < 9; ++tap) {
+            mbar_wait(&full_bar[stage], phase);
+            const uint32_t toff = (uint32_t)((tap / 3) * TC_HALO_W + tap % 3) * 128u;
+            const uint64_t a_hi = kHaloDesc | (uint64_t)(((ha + toff) >> 4) & 0x3fffu);
+            const uint64_t a_lo = kHaloDesc | (uint64_t)(((ha + TC_HALO_PLANE + toff) >> 4) & 0x3fffu);
+            const uint32_t sb = ring_a + stage * STAGE_BYTES;
+            const uint64_t b_hi = gmma_desc_kmajor_sw128(sb), b_lo = gmma_desc_kmajor_sw128(sb + B_BYTES);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < TC_BK / 16; ++k) {
+              const uint64_t ko = (uint64_t)(k * 2);
+              acc.mma(a_lo + ko, a_lo + kHalf + ko, b_hi + ko, (kc > 0 || tap > 0 || k > 0) ? 1u : 0u);
+              acc.mma(a_hi + ko, a_hi + kHalf + ko, b_lo + ko, 1u);
+              acc.mma(a_hi + ko, a_hi + kHalf + ko, b_hi + ko, 1u);
+            }
+            wgmma_commit();
+            if (tap < 8) {
+              wgmma_wait<1>();
+              if (prev >= 0) release_w(prev);
+              prev = stage;
+            } else {                              // the halo slot is free once all nine taps have retired
+              wgmma_wait<0>();
+              if (prev >= 0) release_w(prev);
+              release_w(stage);
+              if (lane == 0) mbar_arrive(&aempty_bar[astage]);
+              prev = -1;
+            }
+            if (++stage == STAGES) { stage = 0; phase ^= 1; }
+          }
+          if (++astage == NA) { astage = 0; aphase ^= 1; }
+        }
+      } else
+      for (int kit = 0; kit < kiters; ++kit) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = ring_a + stage * STAGE_BYTES;
+        const uint64_t a_hi = gmma_desc_kmajor_sw128(sa), a_lo = gmma_desc_kmajor_sw128(sa + TC_A_BYTES);
+        const uint64_t b_hi = gmma_desc_kmajor_sw128(sa + 2 * TC_A_BYTES);
+        const uint64_t b_lo = gmma_desc_kmajor_sw128(sa + 2 * TC_A_BYTES + B_BYTES);
+        constexpr uint64_t kHalf = (TC_BM / 2) * 128 / 16;   // pixel rows 64-127: +8 KiB
+        wgmma_fence();
 #pragma unroll
         for (int k = 0; k < TC_BK / 16; ++k) {
           // advance 16 bf16 = 32 bytes inside the 128-byte swizzle row: +2 in 16-byte units
           const uint64_t ko = (uint64_t)(k * 2);
-          const uint32_t first = (!fresh || k > 0) ? 1u : 0u;
-          if (kConcat) {
-            constexpr uint32_t idesc2n = umma_idesc_bf16_f32(TC_BM, 2 * BN);
-            umma_bf16(d_tmem, a_hi + ko, b_hi + ko, idesc2n, first);          // [hi.hi | hi.lo]
-            umma_bf16(d_tmem + 2 * BN, a_lo + ko, b_hi + ko, idesc, first);   // lo.hi
-          } else if (PAIR) {
-            umma_bf16_2sm(d_tmem, a_lo + ko, b_hi + ko, idesc, first);
-            umma_bf16_2sm(d_tmem, a_hi + ko, b_lo + ko, idesc, 1u);
-            umma_bf16_2sm(d_tmem, a_hi + ko, b_hi + ko, idesc, 1u);
-          } else {
-            umma_bf16(d_tmem, a_lo + ko, b_hi + ko, idesc, first);
-            umma_bf16(d_tmem, a_hi + ko, b_lo + ko, idesc, 1u);
-            umma_bf16(d_tmem, a_hi + ko, b_hi + ko, idesc, 1u);
-          }
+          acc.mma(a_lo + ko, a_lo + kHalf + ko, b_hi + ko, (kit > 0 || k > 0) ? 1u : 0u);
+          acc.mma(a_hi + ko, a_hi + kHalf + ko, b_lo + ko, 1u);
+          acc.mma(a_hi + ko, a_hi + kHalf + ko, b_hi + ko, 1u);
         }
-      };
-      int stage = 0, hstage = 0;
-      uint32_t phase = 0, hphase = 0;
-      (void)hstage; (void)hphase;
-      int it = 0;
-      for (int tile = worker; tile < a.total_tiles; tile += n_workers, ++it) {
-        const uint32_t as = warp_uniform((uint32_t)(it & 1));
-        const uint32_t aphase = (it >> 1) & 1;
-        mbar_wait_warp_a(tempty_a + 8 * as, aphase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_u + as * ACC_COLS;
-        if constexpr (HALO) {
-          // K-major SW128 view of the halo tile: 8-pixel row groups 10 rows apart
-          constexpr uint64_t kHaloDesc = ((uint64_t)1 << 16) | ((uint64_t)((TC_HALO_W * 128) >> 4) << 32) |
-                                         ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
-          for (int kc = 0; kc < kchunks; ++kc) {
-            const uint32_t hs = warp_uniform((uint32_t)hstage);
-            mbar_wait_warp_a(afull_a + 8 * hs, hphase);
-            tc_fence_after();
-            const uint32_t ha = smem_a + hs * TC_HALO_STAGE;
-            for (int tap = 0; tap < 9; ++tap) {
-              const uint32_t st = warp_uniform((uint32_t)stage);
-              mbar_wait_warp_a(full_a + 8 * st, phase);
-              tc_fence_after();
-              const uint32_t toff = warp_uniform((uint32_t)((tap / 3) * TC_HALO_W + tap % 3) * 128u);
-              const uint64_t a_hi = kHaloDesc | (uint64_t)(((ha + toff) >> 4) & 0x3fffu);
-              const uint64_t a_lo = kHaloDesc | (uint64_t)(((ha + TC_HALO_PLANE + toff) >> 4) & 0x3fffu);
-              const uint32_t sb = ring_a + st * STAGE_BYTES;
-              if (elect_one()) {
-                mma_step(d_tmem, a_hi, a_lo, umma_desc_kmajor_sw128(sb), umma_desc_kmajor_sw128(sb + B_BYTES),
-                         kc == 0 && tap == 0);
-                commit(empty_a + 8 * st);           // frees the weight slot (in both CTAs of a pair) when these MMAs retire
-                if (tap == 8) {
-                  commit(aempty_a + 8 * hs);        // ... the halo slot after its ninth tap
-                  if (kc == kchunks - 1) commit(tfull_a + 8 * as);   // ... and hands the accumulator to the epilogue
-                }
-              }
-              __syncwarp();
-              if (++stage == STAGES) { stage = 0; phase ^= 1; }
-            }
-            if (++hstage == NA) { hstage = 0; hphase ^= 1; }
-          }
-        } else {
-          for (int kit = 0; kit < kiters; ++kit) {
-            const uint32_t st = warp_uniform((uint32_t)stage);
-            mbar_wait_warp_a(full_a + 8 * st, phase);
-            tc_fence_after();
-            const uint32_t sa = smem_a + st * STAGE_BYTES;
-            if (elect_one()) {
-              mma_step(d_tmem, umma_desc_kmajor_sw128(sa), umma_desc_kmajor_sw128(sa + TC_A_BYTES),
-                       umma_desc_kmajor_sw128(sa + 2 * TC_A_BYTES), umma_desc_kmajor_sw128(sa + 2 * TC_A_BYTES + B_BYTES),
-                       kit == 0);
-              commit(empty_a + 8 * st);             // frees the smem slot (in both CTAs of a pair) when these MMAs retire
-              if (kit == kiters - 1) commit(tfull_a + 8 * as);   // accumulator ready for the epilogue
-            }
-            __syncwarp();
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
-          }
-        }
+        wgmma_commit();
+        wgmma_wait<1>();                      // the previous stage's MMAs have retired: release its slot
+        if (prev >= 0) release_w(prev);
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
-    }
-  } else {
-    // ================= epilogue (warps 2..5) =================
-    const int q = warp & 3;                 // TMEM lane quarter this warp may access
-    const int m = q * 32 + lane;            // accumulator row = pixel index inside the patch
-    const int r = m >> a.tw_log2, c = m & (TW - 1);
-    int it = 0;
-    for (int tile = worker; tile < a.total_tiles; tile += n_workers, ++it) {
-      const int as = it & 1;
-      const uint32_t aphase = (it >> 1) & 1;
-      const int nt = tile % a.n_tiles;
-      const int pt = PAIR ? 2 * (tile / a.n_tiles) + (int)rank : tile / a.n_tiles;
-      const int img = pt / tiles_per_img;
-      const int rem = pt - img * tiles_per_img;
-      const int h0 = (rem / a.tiles_w) * (TC_BM >> a.tw_log2);
-      const int w0 = (rem % a.tiles_w) * TW;
-      const int n0 = nt * BN;
-      mbar_wait(&tfull_bar[as], aphase);
-      tc_fence_after();
-      const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16) + as * ACC_COLS;
-      conv_epilogue_tile<BN, kConcat>(a, t_row, img, h0, w0, n0, nt, r, c, TW);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (PAIR && !leader) mbar_arrive_remote(mapa_u32(smem_u32(&tempty_bar[as]), 0));
-        else mbar_arrive(&tempty_bar[as]);
-      }
+      wgmma_wait<0>();
+      acc.fence_operands();
+      if (prev >= 0) release_w(prev);
+      conv_epilogue_tile<BN>(a, acc, stg, img, h0, w0, nt * BN, nt, r, c, TW);
     }
   }
-
-  tc_fence_before();
   __syncthreads();
-  if (PAIR) cluster_sync_all();
-  if (warp == 1) {
-    tc_fence_after();
-    if (PAIR) tmem_dealloc_2sm(tmem_base, TMEM_COLS);
-    else tmem_dealloc(tmem_base, TMEM_COLS);
-  }
+  if (PAIR) cluster_sync_all();     // no CTA leaves while its peer may still multicast into it or arrive on its barriers
 }
 
 // ---- host launcher --------------------------------------------------------------------------
-template <int BN, int STAGES, bool PAIR, bool HALO = false, int NA = 0>
+template <int BN, int STAGES, bool HALO = false, int NA = 0>
 static int launch_tc_variant(const CUtensorMap& xhi, const CUtensorMap& xlo, const CUtensorMap& whi,
-                             const CUtensorMap& wlo, const ConvTcArgs& a, cudaStream_t s) {
-  constexpr int smem = ConvTcSmem<BN, PAIR, HALO, NA>::A_RING + STAGES * ConvTcSmem<BN, PAIR, HALO, NA>::STAGE_BYTES +
-                       1024 /*align slack*/ + 256 /*barriers*/;
+                             const CUtensorMap& wlo, const ConvTcArgs& a, bool pair, cudaStream_t s) {
+  constexpr int smem = ConvTcSmem<BN, STAGES, HALO, NA>::BYTES;
   static_assert(smem <= 232448, "shared-memory budget");
-  static DeviceOnce attr_done;   // the attribute is per device
+  static DeviceOnce attr_done;   // the attributes are per device
   if (!attr_done.done()) {
-    IBL_CUDA_OK(cudaFuncSetAttribute(conv3x3_tc_kernel<BN, STAGES, PAIR, HALO, NA>,
-                                     cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    IBL_CUDA_OK(cudaFuncSetAttribute(conv3x3_tc_kernel<BN, STAGES, HALO, NA, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    IBL_CUDA_OK(cudaFuncSetAttribute(conv3x3_tc_kernel<BN, STAGES, HALO, NA, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     attr_done.mark();
   }
-  int dev = 0, sms = 148;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  if (PAIR) {   // a.total_tiles counts pair work items; one 2-CTA cluster per item, at most sms/2 clusters
-    const int pairs = a.total_tiles < sms / 2 ? a.total_tiles : sms / 2;
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(2 * pairs);
-    cfg.blockDim = dim3(192);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = s;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    IBL_CUDA_OK(cudaLaunchKernelEx(&cfg, conv3x3_tc_kernel<BN, STAGES, PAIR, HALO, NA>, xhi, xlo, whi, wlo, a));
+  const int sms = device_sm_count();
+  if (!pair) {
+    const int grid = a.total_tiles < sms ? a.total_tiles : sms;
+    conv3x3_tc_kernel<BN, STAGES, HALO, NA, false><<<grid, 160, smem, s>>>(xhi, xlo, whi, wlo, a);
+    IBL_CUDA_OK(cudaGetLastError());
     return IBL_OK;
   }
-  int grid = a.total_tiles < sms ? a.total_tiles : sms;
-  conv3x3_tc_kernel<BN, STAGES, PAIR, HALO, NA><<<grid, 192, smem, s>>>(xhi, xlo, whi, wlo, a);
-  IBL_CUDA_OK(cudaGetLastError());
+  // a.total_tiles counts pair work items; one 2-CTA cluster per item, at most sms/2 clusters
+  const int pairs = a.total_tiles < sms / 2 ? a.total_tiles : sms / 2;
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(2 * pairs);
+  cfg.blockDim = dim3(160);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = s;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = 2;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  IBL_CUDA_OK(cudaLaunchKernelEx(&cfg, conv3x3_tc_kernel<BN, STAGES, HALO, NA, true>, xhi, xlo, whi, wlo, a));
   return IBL_OK;
 }
 
-static int g_tc_bn_override = 0;   // test hook: force BN (64/128/256) where it divides Cout
+static int g_tc_bn_override = 0;   // test hook: force BN (64/128) where it divides Cout
 void tc_set_bn_override(int bn) { g_tc_bn_override = bn; }
 
 int launch_conv3x3_tc(const __nv_bfloat16* x_hi, const __nv_bfloat16* x_lo, const ConvParams& p,
                       int N, int H, int W, int cin, int cout, bool relu, bool pool,
                       __nv_bfloat16* y_hi, __nv_bfloat16* y_lo, float* y_f32, cudaStream_t s, float* ssq,
                       int* ssq_parts) {
-  IBL_REQUIRE(cin % 64 == 0 && cout % 64 == 0, "tcgen05 conv needs Cin%64==0 and Cout%64==0");
-  IBL_REQUIRE(p.w_hi && p.w_lo, "tcgen05 conv: weights were not re-laid-out");
+  IBL_REQUIRE(cin % 64 == 0 && cout % 64 == 0, "tensor-core conv needs Cin%64==0 and Cout%64==0");
+  IBL_REQUIRE(p.w_hi && p.w_lo, "tensor-core conv: weights were not re-laid-out");
   IBL_REQUIRE(H >= 1 && W >= 1 && N >= 1, "empty conv input");
   ConvTcArgs a{};
   a.N = N; a.H = H; a.W = W; a.cin = cin; a.cout = cout;
@@ -673,52 +560,39 @@ int launch_conv3x3_tc(const __nv_bfloat16* x_hi, const __nv_bfloat16* x_lo, cons
     return (long long)cdiv(W, tw) * tw * cdiv(H, th) * th;
   };
   a.tw_log2 = (waste(16) <= waste(8)) ? 4 : 3;
-  // halo staging needs 16x8 patches (8-pixel row groups at a uniform stride); IBL_CONV_HALO=0 disables it
-  // (set below once the N tile is known: it pays on the 128-wide tiles only)
-  static const int halo_env = [] { const char* v = getenv("IBL_CONV_HALO"); return v ? atoi(v) : 1; }();
   const int TW = 1 << a.tw_log2, TH = 128 / TW;
   a.tiles_w = cdiv(W, TW);
   a.tiles_h = cdiv(H, TH);
-  // N tile: 256 where Cout allows and there are enough patches to fill the machine (measured
-  // 5-9 % faster than 128 on conv3_x/conv4_x: 96 vs 128 B/clk of shared-memory operand reads per
-  // MMA); 128 otherwise; 64 only for Cout = 64 (profiles/r01_bench_layers_v1.txt).
-  // The choice depends on the IMAGE geometry only (a nominal batch of 32), never on the actual batch: the variants
-  // walk K in different orders (halo: chunk-major, im2col boxes: tap-major), so a batch-dependent choice would make
-  // an image's descriptor depend on the batch it travels in (tests: bit-identical across batch compositions).
+  // N tile: 128 where Cout allows (the accumulator is 128 registers per consumer thread), 64 for Cout = 64.  The
+  // choice depends on Cout only, never on the batch, so an image's descriptor does not depend on the batch it
+  // travels in (tests: bit-identical across batch compositions).
   int bn = cout % 128 == 0 ? 128 : 64;
-  if (cout % 256 == 0 && 32ll * a.tiles_h * a.tiles_w * (cout / 256) >= 4 * 148) bn = 256;
-  if (g_tc_bn_override && cout % g_tc_bn_override == 0) bn = g_tc_bn_override;
-  {
-    static int env_bn = -1;   // experiment hook: IBL_TC_BN=256 forces the N tile where it divides Cout
-    if (env_bn < 0) { const char* v = getenv("IBL_TC_BN"); env_bn = v ? atoi(v) : 0; }
-    if (env_bn > 0 && !g_tc_bn_override && cout % env_bn == 0) bn = env_bn;
-  }
-  // Halo staging: measured -12 % / -6 % on conv2_1 / conv2_2 (BN = 128, where the nine im2col boxes per chunk
-  // saturate the 64 B/clk L2->SM path), but +4..9 % on the 256-wide tiles (the tap views are not 1024-byte
-  // aligned, so the A operand costs extra shared-memory wavefronts that the N = 256 MMAs cannot hide) and
-  // neutral on conv1_2.  IBL_CONV_HALO=0: never, =2: every layer.
+  if (g_tc_bn_override && cout % g_tc_bn_override == 0 && (g_tc_bn_override == 64 || g_tc_bn_override == 128))
+    bn = g_tc_bn_override;
+  // Halo staging (16x8 patches): IBL_CONV_HALO=0 never, =1 (default) on the 128-wide tiles, =2 on every N tile.  The
+  // choice depends on Cout only, never on the batch (the variants walk K in different orders).
+  static const int halo_env = [] { const char* v = getenv("IBL_CONV_HALO"); return v ? atoi(v) : 1; }();
   const bool halo = halo_env == 2 || (halo_env == 1 && bn == 128);
   if (halo) {
     a.tw_log2 = 3;
     a.tiles_w = cdiv(W, 8);
     a.tiles_h = cdiv(H, 16);
   }
-  // SM pairs for the 256-wide tiles (measured 3-7 % faster on conv4_x/conv5_x, neutral on conv3_x; the
-  // 128-wide pair variant is 30 % SLOWER than one SM per tile and is only reachable with IBL_CONV_2SM=2).
-  // IBL_CONV_2SM=0: one-SM kernels everywhere.
-  static const int pair_env = [] { const char* v = getenv("IBL_CONV_2SM"); return v ? atoi(v) : 1; }();
+  // SM pairs (weight taps multicast to two CTAs with adjacent patches): IBL_CONV_2SM=0 (default) never, =1 where the
+  // weights are the larger operand stream (Cin >= 256: conv3_2 .. conv5_3), =2 on every layer.  Measured on an H100 at
+  // batch 32 x 480x640: =1 gave 949 images/s against 1063 without pairs (the cluster-wide slot release costs more
+  // than the halved weight traffic saves), hence off by default.  Each CTA still computes its own patch in the same
+  // order, so the results do not depend on the choice.
+  static const int pair_env = [] { const char* v = getenv("IBL_CONV_2SM"); return v ? atoi(v) : 0; }();
   const long long patches = (long long)N * a.tiles_h * a.tiles_w;
-  const bool pair = pair_env && patches >= 2 && ((bn == 256 && cin >= 256) || pair_env == 2) && bn >= 128 &&
-                    !(halo && bn != 256);
-  // (A conv1_2 variant on SM pairs with resident weights was measured at 3.5 ms against 2.1 ms for the one-SM
-  // kernel -- cta_group::2 MMAs only pay off at N = 256 -- and was removed; see git history, round 1.)
+  const bool pair = patches >= 2 && (pair_env == 2 || (pair_env == 1 && cin >= 256));
   a.n_tiles = cout / bn;
   a.total_tiles = (int)((pair ? (patches + 1) / 2 : patches) * a.n_tiles);
   a.relu = relu; a.pool = pool;
   a.bias = p.bias; a.y_hi = y_hi; a.y_lo = y_lo; a.y_f32 = y_f32;
   a.ssq = pool ? nullptr : ssq;
   a.ssq_stride = (long long)N * H * W;
-  a.acc_scale = tc_acc_scale(cin, bn == 64);
+  a.acc_scale = tc_acc_scale(cin);
   if (ssq_parts) *ssq_parts = a.n_tiles;
 
   CUtensorMap m_xhi, m_xlo, m_whi, m_wlo;
@@ -737,40 +611,28 @@ int launch_conv3x3_tc(const __nv_bfloat16* x_hi, const __nv_bfloat16* x_lo, cons
     IBL_RET(make_tmap(&m_wlo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, p.w_lo, dims, str, box));
   }
   if (halo) {
-    if (bn == 64) return launch_tc_variant<64, 4, false, true, 3>(m_xhi, m_xlo, m_whi, m_wlo, a, s);
-    if (bn == 128) return launch_tc_variant<128, 3, false, true, 2>(m_xhi, m_xlo, m_whi, m_wlo, a, s);
-    if (pair) return launch_tc_variant<256, 4, true, true, 2>(m_xhi, m_xlo, m_whi, m_wlo, a, s);
-    return launch_tc_variant<256, 2, false, true, 2>(m_xhi, m_xlo, m_whi, m_wlo, a, s);
+    if (bn == 64) return launch_tc_variant<64, 4, true, 3>(m_xhi, m_xlo, m_whi, m_wlo, a, pair, s);
+    return launch_tc_variant<128, 3, true, 2>(m_xhi, m_xlo, m_whi, m_wlo, a, pair, s);
   }
-  if (bn == 64) return launch_tc_variant<64, 4, false>(m_xhi, m_xlo, m_whi, m_wlo, a, s);
-  if (bn == 128) {
-    if (pair) return launch_tc_variant<128, 4, true>(m_xhi, m_xlo, m_whi, m_wlo, a, s);
-    return launch_tc_variant<128, 3, false>(m_xhi, m_xlo, m_whi, m_wlo, a, s);
-  }
-  if (pair) return launch_tc_variant<256, 3, true>(m_xhi, m_xlo, m_whi, m_wlo, a, s);
-  return launch_tc_variant<256, 2, false>(m_xhi, m_xlo, m_whi, m_wlo, a, s);
+  if (bn == 64) return launch_tc_variant<64, 4>(m_xhi, m_xlo, m_whi, m_wlo, a, pair, s);
+  return launch_tc_variant<128, 3>(m_xhi, m_xlo, m_whi, m_wlo, a, pair, s);
 }
 
 // =====================================================================================================================
 // conv1_1 + conv1_2 (+ ReLU + 2x2 max-pool) in ONE kernel  (vgg.py:40-42 slots 0 and 2)
 //
 // conv1_1's output -- 64 channels at full resolution, 2.5 GB per batch of 32 as hi/lo planes -- is the largest tensor
-// of the network and was written to HBM by one kernel only to be read back by the next.  Here a CTA owns a 16 x 8
-// patch of conv1_2 outputs and RECOMPUTES the conv1_1 activations it needs, the (16+2) x (8+2) = 180-pixel halo
-// (1.06 GFLOP per image, +41 % on 180 vs 128 pixels), straight into the shared-memory halo tile that conv1_2's nine
-// tap views read (the HALO staging of conv3x3_tc_kernel, one 64-channel chunk):
+// of the network and would be written to HBM by one kernel only to be read back by the next.  Here a CTA owns a 16 x 8
+// patch of conv1_2 outputs and RECOMPUTES the conv1_1 activations it needs, the (16+2) x (8+2) = 180-pixel halo,
+// straight into the shared-memory halo tile that conv1_2's nine tap views read (the HALO staging above):
 //
-//   builders (4 warps)   im2col of the 3-channel input for the 180 halo pixels: K = 27 -> 32, bf16 hi/lo, K-major
-//                        SW128 rows (two 128-row M tiles)                                   [as conv1_1_tc_kernel]
-//   MMA (1 thread)       C1: 2 M tiles x 2 K steps x 3 MMAs (M128 N64)  ->  TMEM acc1 (128 columns)
-//   epilogue 1 (4 warps) acc1 -> + bias, ReLU, ZERO outside the image (conv1_2's padding), hi/lo split -> halo tile
-//   MMA                  C2: 9 taps x 4 K steps x (A_hi.[W_hi;W_lo] N128 + A_lo.W_hi N64) -> acc2 (2 x 192 columns)
-//   epilogue 2 (4 warps) acc2 -> + bias, ReLU, 2x2 max-pool, hi/lo planes -> HBM              [conv_epilogue_tile]
-//   producer (1 thread)  TMA ring of conv1_2's weight taps (16 KiB each)
-//
-// The MMA thread issues C1 of tile i+1 BEFORE C2 of tile i, so builders and epilogue 1 of the next tile run under the
-// nine-tap main loop of the current one.  HBM traffic of the pair of layers: the 3-channel input (118 MB) + the pooled
-// output (629 MB) instead of + 2 x 2.5 GB.
+//   builders (warps 5-8)   im2col of the 3-channel input for the 180 halo pixels: K = 27 -> 32, bf16 hi/lo, K-major
+//                          SW128 rows (two 128-row M tiles)                                    [as conv1_1_tc_kernel]
+//   consumer (warps 0-3)   C1: 2 M tiles x 2 K steps x 3 wgmma (N = 64) -> bias, ReLU, ZERO outside the image
+//                          (conv1_2's padding), hi/lo -> halo tile;  C2: 9 taps x 4 K steps x 3 wgmma -> bias, ReLU,
+//                          2x2 max-pool, hi/lo planes -> HBM                                   [conv_epilogue_tile]
+//   producer (warp 4)      TMA ring of conv1_2's weight taps (16 KiB each)
+// The builders fill the operand of the next tile while the consumer runs C1/C2 of the current one.
 // =====================================================================================================================
 struct Conv1FusedArgs {
   const float* x;       // [N,3,H,W]
@@ -786,12 +648,13 @@ constexpr int F1_W2_STAGE = 2 * 64 * TC_BK * 2;      // one tap of conv1_2: W_hi
 constexpr int F1_W2_STAGES = 3;
 constexpr int F1_OFF_A1 = F1_W1;
 constexpr int F1_OFF_HALO = F1_OFF_A1 + F1_A1;       // 80 KiB, 1024-aligned
-constexpr int F1_OFF_W2 = F1_OFF_HALO + 2 * TC_HALO_STAGE;
-constexpr int F1_OFF_BAR = F1_OFF_W2 + F1_W2_STAGES * F1_W2_STAGE;
+constexpr int F1_OFF_W2 = F1_OFF_HALO + TC_HALO_STAGE;
+constexpr int F1_OFF_STG = F1_OFF_W2 + F1_W2_STAGES * F1_W2_STAGE;
+constexpr int F1_OFF_BAR = F1_OFF_STG + ACC_STG_BYTES;
 constexpr int F1_SMEM = F1_OFF_BAR + 512 + 1024;
 static_assert(F1_SMEM <= 232448, "shared-memory budget of the fused conv1 kernel");
 
-__global__ void __launch_bounds__(448, 1)
+__global__ void __launch_bounds__(288, 1)
 conv1_fused_tc_kernel(const __grid_constant__ CUtensorMap tm_whi, const __grid_constant__ CUtensorMap tm_wlo,
                       const Conv1FusedArgs fa) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -802,24 +665,17 @@ conv1_fused_tc_kernel(const __grid_constant__ CUtensorMap tm_whi, const __grid_c
   uint8_t* a1 = smem + F1_OFF_A1;
   uint8_t* halo = smem + F1_OFF_HALO;
   uint8_t* w2 = smem + F1_OFF_W2;
+  float* stg = reinterpret_cast<float*>(smem + F1_OFF_STG);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + F1_OFF_BAR);
-  uint64_t* w_full = bars;                 // [3]
-  uint64_t* w_empty = bars + 3;            // [3]
+  uint64_t* w_full = bars;                 // [3] producer
+  uint64_t* w_empty = bars + 3;            // [3] 4 consumer warps
   uint64_t* a1_full = bars + 6;            // 4 builder warps
-  uint64_t* a1_empty = bars + 7;           // commit of C1
-  uint64_t* acc1_full = bars + 8;          // commit of C1
-  uint64_t* acc1_empty = bars + 9;         // 4 epilogue-1 warps
-  uint64_t* halo_full = bars + 10;         // [2] 4 epilogue-1 warps
-  uint64_t* halo_empty = bars + 12;        // [2] commit of C2
-  uint64_t* acc2_full = bars + 14;         // [2] commit of C2
-  uint64_t* acc2_empty = bars + 16;        // [2] 4 epilogue-2 warps
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 18);
-  float* bias1_s = reinterpret_cast<float*>(bars + 20);   // [64]
+  uint64_t* a1_empty = bars + 7;           // 4 consumer warps
+  float* bias1_s = reinterpret_cast<float*>(bars + 8);   // [64]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // one-time: zero A1 (the K >= 32 half of every row stays zero), lay out conv1_1's filters, zero the halo padding rows
+  // one-time: zero A1 (the K >= 32 half of every row stays zero), lay out conv1_1's filters
   for (int i = threadIdx.x; i < F1_A1 / 16; i += blockDim.x) reinterpret_cast<uint4*>(a1)[i] = make_uint4(0, 0, 0, 0);
-  for (int i = threadIdx.x; i < (2 * TC_HALO_STAGE) / 16; i += blockDim.x) reinterpret_cast<uint4*>(halo)[i] = make_uint4(0, 0, 0, 0);
   for (int i = threadIdx.x; i < 64 * 8; i += blockDim.x) {   // (row n, chunk j): 8 k-values each, k = tap*3 + c
     const int n = i >> 3, j = i & 7;
     uint32_t hi[4], lo[4];
@@ -845,27 +701,13 @@ conv1_fused_tc_kernel(const __grid_constant__ CUtensorMap tm_whi, const __grid_c
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tm_whi);
     tma_prefetch_desc(&tm_wlo);
-    for (int i = 0; i < F1_W2_STAGES; ++i) { mbar_init(&w_full[i], 1); mbar_init(&w_empty[i], 1); }
-    mbar_init(a1_full, 4); mbar_init(a1_empty, 1);
-    mbar_init(acc1_full, 1); mbar_init(acc1_empty, 4);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&halo_full[i], 4); mbar_init(&halo_empty[i], 1);
-      mbar_init(&acc2_full[i], 1); mbar_init(&acc2_empty[i], 4);
-    }
+    for (int i = 0; i < F1_W2_STAGES; ++i) { mbar_init(&w_full[i], 1); mbar_init(&w_empty[i], 4); }
+    mbar_init(a1_full, 4);
+    mbar_init(a1_empty, 4);
     fence_barrier_init();
   }
-  if (warp == 1) { tmem_alloc(tmem_slot, 512); tmem_relinquish(); }
-  fence_proxy_async();
-  tc_fence_before();
+  fence_proxy_async();        // generic-proxy writes of the filters and the zero fill -> visible to the tensor core
   __syncthreads();
-  tc_fence_after();
-  // All 512 columns are allocated, so the allocation starts at column 0 of lane 0: address 0.  A compile-time constant
-  // keeps every TMEM operand of the MMAs in a uniform register (a value loaded from shared memory is per-thread as far
-  // as the compiler knows, and each MMA then pays an ELECT / R2UR.BROADCAST loop).
-  if (*tmem_slot != 0u) __trap();
-  constexpr uint32_t tmem_base = 0u;
-  const uint32_t t_acc1 = tmem_base + 384;            // M tile 0: columns 384-447, M tile 1: 448-511
-  constexpr uint32_t ACC2_COLS = 192;
   const int tiles_per_img = a.tiles_h * a.tiles_w;
   auto coords = [&](int tile, int& img, int& h0, int& w0) {
     img = tile / tiles_per_img;
@@ -875,140 +717,63 @@ conv1_fused_tc_kernel(const __grid_constant__ CUtensorMap tm_whi, const __grid_c
   };
   const long long HW = (long long)a.H * a.W;
 
-  if (warp == 0) {
+  if (warp == 4) {
     // ================= TMA producer: conv1_2 weight taps (convergent warp, one elected lane issues) =================
-    {
-      int stage = 0; uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < a.total_tiles; tile += gridDim.x) {
-        for (int tap = 0; tap < 9; ++tap) {
-          mbar_wait_warp(&w_empty[stage], phase ^ 1);
-          uint8_t* st = w2 + stage * F1_W2_STAGE;
-          if (elect_one()) {
-            mbar_arrive_expect_tx(&w_full[stage], F1_W2_STAGE);
-            tma_load_3d(st, &tm_whi, &w_full[stage], 0, 0, tap);
-            tma_load_3d(st + F1_W2_STAGE / 2, &tm_wlo, &w_full[stage], 0, 0, tap);
-          }
-          __syncwarp();
-          if (++stage == F1_W2_STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ================= MMA issuer =================
-    // The whole warp walks the schedule in convergent code and ONE ELECTED lane executes the tcgen05 instructions of a
-    // stage (see conv3x3_tc_kernel's issuer): 72 + 12 small MMAs per tile (N = 64 / 128: 32-65 clk of tensor pipe each)
-    // cost ~90 clk of issue apiece behind `if (lane == 0)` -- the kernel ran at 40 % tensor-pipe activity with the
-    // issuing thread busy 75 % of the time.
-    {
-      constexpr uint32_t idesc64 = umma_idesc_bf16_f32(TC_BM, 64);
-      constexpr uint32_t idesc128 = umma_idesc_bf16_f32(TC_BM, 128);
-      constexpr uint64_t kHaloDesc = ((uint64_t)1 << 16) | ((uint64_t)((TC_HALO_W * 128) >> 4) << 32) |
-                                     ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
-      const uint64_t b1h = umma_desc_kmajor_sw128(smem_u32(w1_hi)), b1l = umma_desc_kmajor_sw128(smem_u32(w1_lo));
-      int n_tiles = 0;
-      for (int tile = blockIdx.x; tile < a.total_tiles; tile += gridDim.x) ++n_tiles;
-      auto issue_c1 = [&](int it) {
-        mbar_wait_warp(a1_full, it & 1);
-        mbar_wait_warp(acc1_empty, (it & 1) ^ 1);
-        tc_fence_after();
+    int stage = 0; uint32_t phase = 0;
+    for (int tile = blockIdx.x; tile < a.total_tiles; tile += gridDim.x) {
+      for (int tap = 0; tap < 9; ++tap) {
+        mbar_wait_warp(&w_empty[stage], phase ^ 1);
+        uint8_t* st = w2 + stage * F1_W2_STAGE;
         if (elect_one()) {
-#pragma unroll
-          for (int mt = 0; mt < 2; ++mt) {
-            const uint32_t sa = smem_u32(a1) + mt * 16384;
-            const uint64_t ah = umma_desc_kmajor_sw128(sa), al = umma_desc_kmajor_sw128(sa + F1_A1_PLANE);
-            const uint32_t d = t_acc1 + mt * 64;
-#pragma unroll
-            for (int k = 0; k < 2; ++k) {               // K = 32: two 16-wide steps
-              const uint64_t ko = (uint64_t)(k * 2);
-              umma_bf16(d, al + ko, b1h + ko, idesc64, k > 0 ? 1u : 0u);
-              umma_bf16(d, ah + ko, b1l + ko, idesc64, 1u);
-              umma_bf16(d, ah + ko, b1h + ko, idesc64, 1u);
-            }
-          }
-          umma_commit(a1_empty);
-          umma_commit(acc1_full);
+          mbar_arrive_expect_tx(&w_full[stage], F1_W2_STAGE);
+          tma_load_3d(st, &tm_whi, &w_full[stage], 0, 0, tap);
+          tma_load_3d(st + F1_W2_STAGE / 2, &tm_wlo, &w_full[stage], 0, 0, tap);
         }
         __syncwarp();
-      };
-      int stage = 0; uint32_t phase = 0;
-      if (n_tiles > 0) issue_c1(0);
-      for (int it = 0; it < n_tiles; ++it) {
-        if (it + 1 < n_tiles) issue_c1(it + 1);
-        const int hb = it & 1;
-        const uint32_t hph = (it >> 1) & 1;
-        mbar_wait_warp(&acc2_empty[hb], hph ^ 1);
-        mbar_wait_warp(&halo_full[hb], hph);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + hb * ACC2_COLS;
-        const uint32_t ha = smem_u32(halo + hb * TC_HALO_STAGE);
-        for (int tap = 0; tap < 9; ++tap) {
-          mbar_wait_warp(&w_full[stage], phase);
-          tc_fence_after();
-          const uint32_t toff = (uint32_t)((tap / 3) * TC_HALO_W + tap % 3) * 128u;
-          const uint64_t a_hi = kHaloDesc | (uint64_t)(((ha + toff) >> 4) & 0x3fffu);
-          const uint64_t a_lo = kHaloDesc | (uint64_t)(((ha + TC_HALO_PLANE + toff) >> 4) & 0x3fffu);
-          const uint32_t sb = smem_u32(w2 + stage * F1_W2_STAGE);
-          const uint64_t b_cat = umma_desc_kmajor_sw128(sb);          // 128 rows: W_hi then W_lo
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < TC_BK / 16; ++k) {
-              const uint64_t ko = (uint64_t)(k * 2);
-              const uint32_t first = (tap > 0 || k > 0) ? 1u : 0u;
-              umma_bf16(d_tmem, a_hi + ko, b_cat + ko, idesc128, first);            // [hi.hi | hi.lo]
-              umma_bf16(d_tmem + 128, a_lo + ko, b_cat + ko, idesc64, first);       // lo.hi
-            }
-            umma_commit(&w_empty[stage]);
-            if (tap == 8) {                           // same elected thread as the MMAs these commits cover
-              umma_commit(&halo_empty[hb]);
-              umma_commit(&acc2_full[hb]);
-            }
-          }
-          __syncwarp();
-          if (++stage == F1_W2_STAGES) { stage = 0; phase ^= 1; }
-        }
+        if (++stage == F1_W2_STAGES) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp <= 5) {
-    // ================= epilogue 2: conv1_2 accumulators -> bias, ReLU, pool, hi/lo planes =================
-    const int q = warp & 3;
-    const int m = q * 32 + lane;
-    const int r = m >> 3, c = m & 7;                  // 8-wide, 16-tall patch
+  } else if (warp < 4) {
+    // ================= consumer warpgroup: C1 -> halo tile, C2 -> conv1_2 epilogue =================
+    const int t = threadIdx.x;
+    const int r = t >> 3, c = t & 7;                  // 8-wide, 16-tall patch
+    const uint64_t b1h = gmma_desc_kmajor_sw128(smem_u32(w1_hi)), b1l = gmma_desc_kmajor_sw128(smem_u32(w1_lo));
+    constexpr uint64_t kHaloDesc = ((uint64_t)1 << 16) | ((uint64_t)((TC_HALO_W * 128) >> 4) << 32) | ((uint64_t)1 << 62);
+    constexpr uint64_t kHaloHalf = 8 * TC_HALO_W * 128 / 16;   // pixel rows 64-127 of a tap view: groups 8-15
+    const uint32_t ha = smem_u32(halo);
+    int stage = 0; uint32_t phase = 0;
     int it = 0;
     for (int tile = blockIdx.x; tile < a.total_tiles; tile += gridDim.x, ++it) {
       int img, h0, w0;
       coords(tile, img, h0, w0);
-      const int hb = it & 1;
-      mbar_wait(&acc2_full[hb], (it >> 1) & 1);
-      tc_fence_after();
-      const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16) + hb * ACC2_COLS;
-      conv_epilogue_tile<64, true>(a, t_row, img, h0, w0, 0, 0, r, c, 8);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc2_empty[hb]);
-    }
-  } else if (warp <= 9) {
-    // ================= epilogue 1: conv1_1 accumulators -> bias, ReLU, image mask, hi/lo -> halo tile =================
-    const int q = warp & 3;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < a.total_tiles; tile += gridDim.x, ++it) {
-      int img, h0, w0;
-      coords(tile, img, h0, w0);
-      const int hb = it & 1;
-      mbar_wait(acc1_full, it & 1);
-      mbar_wait(&halo_empty[hb], ((it >> 1) & 1) ^ 1);
-      tc_fence_after();
-      uint8_t* hh = halo + hb * TC_HALO_STAGE;
+      mbar_wait(a1_full, it & 1);
 #pragma unroll 1
       for (int mt = 0; mt < 2; ++mt) {
-        const int p = mt * 128 + q * 32 + lane;          // halo row = TMEM lane of M tile mt
+        const uint32_t sa = smem_u32(a1) + mt * 16384;
+        const uint64_t ah = gmma_desc_kmajor_sw128(sa), al = gmma_desc_kmajor_sw128(sa + F1_A1_PLANE);
+        constexpr uint64_t kHalf = 64 * 128 / 16;
+        Acc128<64> c1;
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {                   // K = 32: two 16-wide steps
+          const uint64_t ko = (uint64_t)(k * 2);
+          c1.mma(al + ko, al + kHalf + ko, b1h + ko, k > 0 ? 1u : 0u);
+          c1.mma(ah + ko, ah + kHalf + ko, b1l + ko, 1u);
+          c1.mma(ah + ko, ah + kHalf + ko, b1h + ko, 1u);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        c1.fence_operands();
+        if (mt == 1 && lane == 0) mbar_arrive(a1_empty);   // the builders may refill A1
+        // epilogue 1: bias, ReLU, image mask, hi/lo -> halo row p (the previous tile's C2 has retired)
+        const int p = mt * 128 + t;
         const int hl = p / TC_HALO_W, wl = p - hl * TC_HALO_W;
         const int ph = h0 - 1 + hl, pw = w0 - 1 + wl;
         const bool inside = p < TC_HALO_W * TC_HALO_H && ph >= 0 && ph < a.H && pw >= 0 && pw < a.W && img < a.N;
-#pragma unroll 1
+#pragma unroll
         for (int ch = 0; ch < 2; ++ch) {
           uint32_t raw[32];
-          tmem_ld_32x32(t_acc1 + ((uint32_t)(q * 32) << 16) + mt * 64 + ch * 32, raw);
-          tmem_ld_wait();
+          c1.rows32(ch, stg, raw);
           if (p < TC_HALO_W * TC_HALO_H) {
             uint32_t hi[16], lo[16];
 #pragma unroll
@@ -1021,7 +786,7 @@ conv1_fused_tc_kernel(const __grid_constant__ CUtensorMap tm_whi, const __grid_c
               hi[j] = *reinterpret_cast<uint32_t*>(&hv);
               lo[j] = pack_bf16x2(x0 - __bfloat162float(h0b), x1 - __bfloat162float(h1b));
             }
-            uint8_t* rh = hh + p * 128;
+            uint8_t* rh = halo + p * 128;
             uint8_t* rl = rh + TC_HALO_PLANE;
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
@@ -1032,14 +797,40 @@ conv1_fused_tc_kernel(const __grid_constant__ CUtensorMap tm_whi, const __grid_c
           }
         }
       }
-      tc_fence_before();
-      fence_proxy_async();                              // generic-proxy writes of the halo -> visible to the tensor core
-      __syncwarp();
-      if (lane == 0) { mbar_arrive(acc1_empty); mbar_arrive(&halo_full[hb]); }
+      fence_proxy_async();                               // generic-proxy writes of the halo -> visible to the tensor core
+      wg_sync();                                         // every halo row is written
+      // C2: conv1_2 over the nine tap views of the halo tile
+      Acc128<64> acc;
+      int prev = -1;
+      for (int tap = 0; tap < 9; ++tap) {
+        mbar_wait(&w_full[stage], phase);
+        const uint32_t toff = (uint32_t)((tap / 3) * TC_HALO_W + tap % 3) * 128u;
+        const uint64_t a_hi = kHaloDesc | (uint64_t)(((ha + toff) >> 4) & 0x3fffu);
+        const uint64_t a_lo = kHaloDesc | (uint64_t)(((ha + TC_HALO_PLANE + toff) >> 4) & 0x3fffu);
+        const uint32_t sb = smem_u32(w2 + stage * F1_W2_STAGE);
+        const uint64_t b_hi = gmma_desc_kmajor_sw128(sb), b_lo = gmma_desc_kmajor_sw128(sb + F1_W2_STAGE / 2);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < TC_BK / 16; ++k) {
+          const uint64_t ko = (uint64_t)(k * 2);
+          acc.mma(a_lo + ko, a_lo + kHaloHalf + ko, b_hi + ko, (tap > 0 || k > 0) ? 1u : 0u);
+          acc.mma(a_hi + ko, a_hi + kHaloHalf + ko, b_lo + ko, 1u);
+          acc.mma(a_hi + ko, a_hi + kHaloHalf + ko, b_hi + ko, 1u);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0 && lane == 0) mbar_arrive(&w_empty[prev]);
+        prev = stage;
+        if (++stage == F1_W2_STAGES) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      acc.fence_operands();
+      if (lane == 0) mbar_arrive(&w_empty[prev]);
+      conv_epilogue_tile<64>(a, acc, stg, img, h0, w0, 0, 0, r, c, 8);
     }
   } else {
     // ================= builders: im2col rows of conv1_1 for the 180 halo pixels =================
-    const int bw = warp - 10;
+    const int bw = warp - 5;
     int it = 0;
     for (int tile = blockIdx.x; tile < a.total_tiles; tile += gridDim.x, ++it) {
       int img, h0, w0;
@@ -1092,9 +883,6 @@ conv1_fused_tc_kernel(const __grid_constant__ CUtensorMap tm_whi, const __grid_c
       if (lane == 0) mbar_arrive(a1_full);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, 512); }
 }
 
 // x [N,3,H,W] fp32 -> conv1_1 -> ReLU -> conv1_2 -> ReLU -> 2x2 max-pool as hi/lo planes [N,H/2,W/2,64]
@@ -1112,7 +900,7 @@ int launch_conv1_fused_tc(const float* x_nchw, const float* w1_oihw, const float
   a.total_tiles = (int)((long long)N * a.tiles_h * a.tiles_w);
   a.relu = 1; a.pool = 1;
   a.bias = p2.bias; a.y_hi = y_hi; a.y_lo = y_lo; a.y_f32 = nullptr; a.ssq = nullptr; a.ssq_stride = 0;
-  a.acc_scale = tc_acc_scale(64, true);
+  a.acc_scale = tc_acc_scale(64);
   CUtensorMap m_whi, m_wlo;
   {
     uint64_t dims[3] = {64, 64, 9};
@@ -1128,7 +916,7 @@ int launch_conv1_fused_tc(const float* x_nchw, const float* w1_oihw, const float
   }
   const int sms = device_sm_count();
   const int grid = a.total_tiles < sms ? a.total_tiles : sms;
-  conv1_fused_tc_kernel<<<grid, 448, F1_SMEM, s>>>(m_whi, m_wlo, fa);
+  conv1_fused_tc_kernel<<<grid, 288, F1_SMEM, s>>>(m_whi, m_wlo, fa);
   IBL_CUDA_OK(cudaGetLastError());
   return IBL_OK;
 }
@@ -1168,7 +956,7 @@ int launch_maxpool2x2_planes(const __nv_bfloat16* hi, const __nv_bfloat16* lo, i
                              int C, __nv_bfloat16* yhi, __nv_bfloat16* ylo, cudaStream_t s) {
   long long total = (long long)N * (H / 2) * (W / 2) * C;
   unsigned blocks = (unsigned)((total + 255) / 256);
-  if (blocks > 148 * 32) blocks = 148 * 32;
+  if (blocks > 132 * 32) blocks = 132 * 32;
   if (!blocks) blocks = 1;
   maxpool2x2_planes_kernel<<<blocks, 256, 0, s>>>(hi, lo, N, H, W, C, yhi, ylo);
   IBL_CUDA_OK(cudaGetLastError());

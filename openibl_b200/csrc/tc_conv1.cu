@@ -1,15 +1,15 @@
-// conv1_1 (Cin = 3, reference ibl/models/vgg.py slot 0) on tcgen05.
+// conv1_1 (Cin = 3, reference ibl/models/vgg.py slot 0) on the Hopper tensor cores (wgmma).
 //
 // K = 27 is too short for a TMA-fed implicit GEMM (a 3-channel NHWC row is 6 bytes), so the A
 // operand is built in shared memory by four "im2col" warps straight from the NCHW fp32 input:
 // one pixel per thread, its 3x3x3 window ordered k = tap*3 + c, split into bf16 hi/lo, zero-padded
 // to K = 32 and written as one K-major 128-byte-swizzled row (the layout TMA would have produced).
 // The 64x27 filter bank is laid out the same way once per CTA.  Two K=16 MMA steps x 3 (bf16x3)
-// per 128-pixel tile; the epilogue is the usual TMEM -> bias -> ReLU -> hi/lo planes with 16-byte
-// stores.  The kernel is bound by the 2.5 GB of NHWC output it writes per batch of 32.
+// per 128-pixel tile; the epilogue is the usual accumulator -> bias -> ReLU -> hi/lo planes with
+// 16-byte stores.  The kernel is bound by the 2.5 GB of NHWC output it writes per batch of 32.
 //
-// Warps: 0 MMA issuer + TMEM owner, 1-4 operand builders, 5-8 epilogue.  A and the TMEM
-// accumulator are double-buffered, persistent grid.
+// Warps: 0-3 consumer warpgroup (wgmma + epilogue), 4-7 operand builders.  A is double-buffered,
+// persistent grid.
 #include "common.cuh"
 #include "tc_common.cuh"
 
@@ -28,22 +28,24 @@ struct Conv1Args {
 };
 
 constexpr int C1_ABYTES = 128 * 128;   // one plane of one A stage: 128 rows x 128 B
+constexpr int C1_OFF_A = 16384;                          // after the filters (hi 8 KiB | lo 8 KiB)
+constexpr int C1_OFF_OUT = C1_OFF_A + 4 * C1_ABYTES;     // output staging: 4 warps x (hi 4 KiB | lo 4 KiB)
+constexpr int C1_OFF_ACC = C1_OFF_OUT + 4 * 8192;        // accumulator transposition
+constexpr int C1_OFF_BAR = C1_OFF_ACC + ACC_STG_BYTES;
+constexpr int C1_SMEM = C1_OFF_BAR + 512 + 1024;
 
-// (Two CTAs per SM were tried and measured the same 1.10 ms: the kernel is not occupancy-bound.)
-__global__ void __launch_bounds__(288, 1) conv1_1_tc_kernel(const Conv1Args a) {
+__global__ void __launch_bounds__(256, 1) conv1_1_tc_kernel(const Conv1Args a) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* b_hi = smem;                       // [64 rows][128 B]
   uint8_t* b_lo = smem + 8192;
-  uint8_t* a_buf = smem + 16384;              // 2 stages x (hi 16 KiB | lo 16 KiB)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(a_buf + 4 * C1_ABYTES);
+  uint8_t* a_buf = smem + C1_OFF_A;           // 2 stages x (hi 16 KiB | lo 16 KiB)
+  uint8_t* stg = smem + C1_OFF_OUT;
+  float* acc_stg = reinterpret_cast<float*>(smem + C1_OFF_ACC);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C1_OFF_BAR);
   uint64_t* a_full = bars;        // [2] count 4 (builder warps)
-  uint64_t* a_empty = bars + 2;   // [2] count 1 (tcgen05.commit)
-  uint64_t* t_full = bars + 4;    // [2]
-  uint64_t* t_empty = bars + 6;   // [2] count 4 (epilogue warps)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 8);
-  float* bias_s = reinterpret_cast<float*>(bars + 9);   // [64]
-  uint8_t* stg = reinterpret_cast<uint8_t*>(bars + 64);     // epilogue staging: 4 warps x (hi 4 KiB | lo 4 KiB), 512-B aligned
+  uint64_t* a_empty = bars + 2;   // [2] count 4 (consumer warps)
+  float* bias_s = reinterpret_cast<float*>(bars + 4);   // [64]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   // zero both A stages once (the K >= 32 half of every row stays zero) and lay out the filters
@@ -75,49 +77,88 @@ __global__ void __launch_bounds__(288, 1) conv1_1_tc_kernel(const Conv1Args a) {
   if (threadIdx.x == 0) {
     for (int i = 0; i < 2; ++i) {
       mbar_init(&a_full[i], 4);
-      mbar_init(&a_empty[i], 1);
-      mbar_init(&t_full[i], 1);
-      mbar_init(&t_empty[i], 4);
+      mbar_init(&a_empty[i], 4);
     }
     fence_barrier_init();
   }
-  if (warp == 0) { tmem_alloc(tmem_slot, 128); tmem_relinquish(); }
   fence_proxy_async();        // generic-proxy writes of B (and the zero fill) -> visible to the tensor core
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   const long long M = (long long)a.N * a.H * a.W;
   const long long HW = (long long)a.H * a.W;
 
-  if (warp == 0) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_bf16_f32(128, 64);
-      const uint64_t bh = umma_desc_kmajor_sw128(smem_u32(b_hi)), bl = umma_desc_kmajor_sw128(smem_u32(b_lo));
-      int it = 0;
-      for (int tile = blockIdx.x; tile < a.total_tiles; tile += gridDim.x, ++it) {
-        const int st = it & 1;
-        const uint32_t ph = (it >> 1) & 1;
-        mbar_wait(&a_full[st], ph);
-        mbar_wait(&t_empty[st], ph ^ 1);
-        tc_fence_after();
-        const uint32_t sa = smem_u32(a_buf + st * 2 * C1_ABYTES);
-        const uint64_t ah = umma_desc_kmajor_sw128(sa), al = umma_desc_kmajor_sw128(sa + C1_ABYTES);
-        const uint32_t d = tmem_base + st * 64;
+  if (warp < 4) {
+    // ---------------- consumer warpgroup: MMA + epilogue ----------------
+    const uint64_t bh = gmma_desc_kmajor_sw128(smem_u32(b_hi)), bl = gmma_desc_kmajor_sw128(smem_u32(b_lo));
+    int it = 0;
+    for (int tile = blockIdx.x; tile < a.total_tiles; tile += gridDim.x, ++it) {
+      const int st = it & 1;
+      const uint32_t ph = (it >> 1) & 1;
+      mbar_wait(&a_full[st], ph);
+      const uint32_t sa = smem_u32(a_buf + st * 2 * C1_ABYTES);
+      const uint64_t ah = gmma_desc_kmajor_sw128(sa), al = gmma_desc_kmajor_sw128(sa + C1_ABYTES);
+      constexpr uint64_t kHalf = 64 * 128 / 16;   // pixel rows 64-127: +8 KiB
+      Acc128<64> acc;
+      wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < 2; ++k) {             // K = 32: two 16-wide steps (columns 32..63 are zero)
-          const uint64_t ko = (uint64_t)(k * 2);
-          umma_bf16(d, al + ko, bh + ko, idesc, k > 0 ? 1u : 0u);
-          umma_bf16(d, ah + ko, bl + ko, idesc, 1u);
-          umma_bf16(d, ah + ko, bh + ko, idesc, 1u);
-        }
-        umma_commit(&a_empty[st]);
-        umma_commit(&t_full[st]);
+      for (int k = 0; k < 2; ++k) {             // K = 32: two 16-wide steps (columns 32..63 are zero)
+        const uint64_t ko = (uint64_t)(k * 2);
+        acc.mma(al + ko, al + kHalf + ko, bh + ko, k > 0 ? 1u : 0u);
+        acc.mma(ah + ko, ah + kHalf + ko, bl + ko, 1u);
+        acc.mma(ah + ko, ah + kHalf + ko, bh + ko, 1u);
       }
+      wgmma_commit();
+      wgmma_wait<0>();
+      acc.fence_operands();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&a_empty[st]);   // the builders may refill this stage
+      // bias + ReLU + hi/lo split into this warp's staging rows (one 128-byte row per pixel and plane,
+      // 16-byte chunks XOR-swizzled by the row index), then the warp writes its 32 pixels as eight fully
+      // coalesced 512-byte stores per plane instead of 32 scattered 16-byte pieces per instruction.
+      uint8_t* sth = stg + warp * 8192 + lane * 128;
+      uint8_t* stl = sth + 4096;
+#pragma unroll
+      for (int ch = 0; ch < 2; ++ch) {
+        uint32_t raw[32];
+        acc.rows32(ch, acc_stg, raw);
+        uint32_t hi[16], lo[16];
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const float x0 = fmaxf(__uint_as_float(raw[2 * j]) + bias_s[ch * 32 + 2 * j], 0.f);
+          const float x1 = fmaxf(__uint_as_float(raw[2 * j + 1]) + bias_s[ch * 32 + 2 * j + 1], 0.f);
+          const __nv_bfloat16 h0 = __float2bfloat16_rn(x0), h1 = __float2bfloat16_rn(x1);
+          __nv_bfloat162 hh(h0, h1);
+          __nv_bfloat162 ll = __floats2bfloat162_rn(x0 - __bfloat162float(h0), x1 - __bfloat162float(h1));
+          hi[j] = *reinterpret_cast<uint32_t*>(&hh);
+          lo[j] = *reinterpret_cast<uint32_t*>(&ll);
+        }
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const int pos = ((ch * 4 + j) ^ (lane & 7)) * 16;
+          *reinterpret_cast<uint4*>(sth + pos) = make_uint4(hi[4 * j], hi[4 * j + 1], hi[4 * j + 2], hi[4 * j + 3]);
+          *reinterpret_cast<uint4*>(stl + pos) = make_uint4(lo[4 * j], lo[4 * j + 1], lo[4 * j + 2], lo[4 * j + 3]);
+        }
+      }
+      __syncwarp();
+      {
+        const uint8_t* wb = stg + warp * 8192;
+        const long long p0 = (long long)tile * 128 + warp * 32;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const int r = i * 4 + (lane >> 3), cchunk = lane & 7;
+          const int pos = r * 128 + ((cchunk ^ (r & 7)) * 16);
+          const uint4 vh = *reinterpret_cast<const uint4*>(wb + pos);
+          const uint4 vl = *reinterpret_cast<const uint4*>(wb + 4096 + pos);
+          if (p0 + r < M) {
+            *reinterpret_cast<uint4*>(a.y_hi + (p0 + r) * 64 + cchunk * 8) = vh;
+            *reinterpret_cast<uint4*>(a.y_lo + (p0 + r) * 64 + cchunk * 8) = vl;
+          }
+        }
+      }
+      __syncwarp();                               // the staging rows are rewritten by the next tile
     }
-  } else if (warp <= 4) {
+  } else {
     // ---------------- operand builders: one pixel (= one A row) per thread ----------------
-    const int row = (warp - 1) * 32 + lane;
+    const int row = (warp - 4) * 32 + lane;
     int it = 0;
     for (int tile = blockIdx.x; tile < a.total_tiles; tile += gridDim.x, ++it) {
       const int st = it & 1;
@@ -164,66 +205,7 @@ __global__ void __launch_bounds__(288, 1) conv1_1_tc_kernel(const Conv1Args a) {
       __syncwarp();
       if (lane == 0) mbar_arrive(&a_full[st]);
     }
-  } else {
-    // ---------------- epilogue ----------------
-    const int q = warp & 3;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < a.total_tiles; tile += gridDim.x, ++it) {
-      const int st = it & 1;
-      const uint32_t ph = (it >> 1) & 1;
-      mbar_wait(&t_full[st], ph);
-      tc_fence_after();
-      // bias + ReLU + hi/lo split into this warp's staging rows (one 128-byte row per pixel and plane,
-      // 16-byte chunks XOR-swizzled by the row index), then the warp writes its 32 pixels as eight fully
-      // coalesced 512-byte stores per plane instead of 32 scattered 16-byte pieces per instruction.
-      uint8_t* sth = stg + (warp - 5) * 8192 + lane * 128;
-      uint8_t* stl = sth + 4096;
-#pragma unroll 1
-      for (int ch = 0; ch < 2; ++ch) {
-        uint32_t raw[32];
-        tmem_ld_32x32(tmem_base + ((uint32_t)(q * 32) << 16) + st * 64 + ch * 32, raw);
-        tmem_ld_wait();
-        uint32_t hi[16], lo[16];
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const float x0 = fmaxf(__uint_as_float(raw[2 * j]) + bias_s[ch * 32 + 2 * j], 0.f);
-          const float x1 = fmaxf(__uint_as_float(raw[2 * j + 1]) + bias_s[ch * 32 + 2 * j + 1], 0.f);
-          const __nv_bfloat16 h0 = __float2bfloat16_rn(x0), h1 = __float2bfloat16_rn(x1);
-          __nv_bfloat162 hh(h0, h1);
-          __nv_bfloat162 ll = __floats2bfloat162_rn(x0 - __bfloat162float(h0), x1 - __bfloat162float(h1));
-          hi[j] = *reinterpret_cast<uint32_t*>(&hh);
-          lo[j] = *reinterpret_cast<uint32_t*>(&ll);
-        }
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int pos = ((ch * 4 + j) ^ (lane & 7)) * 16;
-          *reinterpret_cast<uint4*>(sth + pos) = make_uint4(hi[4 * j], hi[4 * j + 1], hi[4 * j + 2], hi[4 * j + 3]);
-          *reinterpret_cast<uint4*>(stl + pos) = make_uint4(lo[4 * j], lo[4 * j + 1], lo[4 * j + 2], lo[4 * j + 3]);
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&t_empty[st]);      // TMEM buffer is free; the copy-out only touches smem
-      {
-        const uint8_t* wb = stg + (warp - 5) * 8192;
-        const long long p0 = (long long)tile * 128 + q * 32;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int r = i * 4 + (lane >> 3), cchunk = lane & 7;
-          const int pos = r * 128 + ((cchunk ^ (r & 7)) * 16);
-          const uint4 vh = *reinterpret_cast<const uint4*>(wb + pos);
-          const uint4 vl = *reinterpret_cast<const uint4*>(wb + 4096 + pos);
-          if (p0 + r < M) {
-            *reinterpret_cast<uint4*>(a.y_hi + (p0 + r) * 64 + cchunk * 8) = vh;
-            *reinterpret_cast<uint4*>(a.y_lo + (p0 + r) * 64 + cchunk * 8) = vl;
-          }
-        }
-      }
-    }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) { tc_fence_after(); tmem_dealloc(tmem_base, 128); }
 }
 
 int launch_conv1_1_tc(const float* x_nchw, const float* w_oihw, const float* bias, int N, int H, int W,
@@ -233,17 +215,14 @@ int launch_conv1_1_tc(const float* x_nchw, const float* w_oihw, const float* bia
   a.N = N; a.H = H; a.W = W;
   const long long M = (long long)N * H * W;
   a.total_tiles = (int)((M + 127) / 128);
-  const int smem = 16384 + 4 * C1_ABYTES + 1024 + 512 + 4 * 8192;
   static DeviceOnce attr_done;   // the attribute is per device
   if (!attr_done.done()) {
-    IBL_CUDA_OK(cudaFuncSetAttribute(conv1_1_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    IBL_CUDA_OK(cudaFuncSetAttribute(conv1_1_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, C1_SMEM));
     attr_done.mark();
   }
-  int sms = 148, dev = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int sms = device_sm_count();
   const int grid = a.total_tiles < sms ? a.total_tiles : sms;
-  conv1_1_tc_kernel<<<grid, 288, smem, s>>>(a);
+  conv1_1_tc_kernel<<<grid, 256, C1_SMEM, s>>>(a);
   IBL_CUDA_OK(cudaGetLastError());
   return IBL_OK;
 }

@@ -2,7 +2,7 @@
 // conv5_1..conv5_3 under the SFRS loss; reference: autograd through ibl/models/vgg.py:61-62, cuDNN dgrad/wgrad).
 //
 //   dgrad   dX[n,h,w,ci] = sum_{tap,co} dY[n,h-(kh-1),w-(kw-1),co] W[co,ci,kh,kw]
-//           = the SAME tcgen05 implicit-GEMM forward kernel (tc_conv.cu) applied to dY with the filter bank
+//           = the SAME tensor-core implicit-GEMM forward kernel (tc_conv.cu) applied to dY with the filter bank
 //             rotated by 180 degrees and its channel roles swapped (repack_weights_dgrad_kernel).
 //   wgrad   dW[co,ci,kh,kw] = sum_{n,h,w} dY[n,h,w,co] X[n,h+kh-1,w+kw-1,ci]
 //           = per tap a GEMM whose reduction index is the PIXEL: both operands are "MN-major" in shared memory
@@ -10,7 +10,7 @@
 //             hi/lo planes delivers -- the layout the second NetVLAD contraction already uses (tc_netvlad.cu).
 //             conv_wgrad_tc_kernel: one CTA per (tap, 128 output channels, 128 input channels, pixel split);
 //             64-pixel K steps (boxes of 16 x 4 pixels; the X box is shifted by the tap, TMA zero-fills the
-//             padding), bf16x3, one 128 x 128 fp32 accumulator in TMEM, partial sums per split reduced by
+//             padding), bf16x3, one 128 x 128 fp32 wgmma accumulator, partial sums per split reduced by
 //             wgrad_reduce_kernel into the OIHW gradient.
 //   db, ReLU mask, 2x2 max-pool backward: small CUDA-core kernels.
 #include <stdlib.h>
@@ -21,20 +21,6 @@
 namespace ibl {
 
 using namespace tc;
-
-// same MN-major descriptor / instruction-descriptor helpers as tc_netvlad.cu
-__device__ __forceinline__ uint64_t bwd_desc_mnmajor_sw128(uint32_t smem_addr, uint32_t lbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3fffu);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3fffu) << 16;
-  d |= (uint64_t)(1024u >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-__host__ __device__ constexpr uint32_t bwd_idesc_mn(int M, int N) {
-  return umma_idesc_bf16_f32(M, N) | (1u << 15) | (1u << 16);   // A and B both MN-major
-}
 
 // ---- filter bank for dgrad: planes [tap'][Cin][Cout] with tap' = 8 - tap (the forward kernel's [tap][N][K] layout with
 // N = Cin, K = Cout), from the engine's fp32 copy w_tck [tap][Cin][Cout] ------------------------------------------
@@ -76,7 +62,7 @@ __global__ void relu_mask_planes_kernel(const float* __restrict__ g, const float
 int launch_relu_mask_planes(const float* g, const float* y, size_t n, bool relu, __nv_bfloat16* hi, __nv_bfloat16* lo,
                             cudaStream_t s) {
   unsigned blocks = (unsigned)((n + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   if (!blocks) blocks = 1;
   relu_mask_planes_kernel<<<blocks, 256, 0, s>>>(g, y, n, relu ? 1 : 0, hi, lo);
   IBL_CUDA_OK(cudaGetLastError());
@@ -133,14 +119,14 @@ __global__ void maxpool2x2_bwd_kernel(const float* __restrict__ x, const float* 
 int launch_maxpool2x2_bwd(const float* x, const float* gy, int N, int H, int W, int C, float* gx, cudaStream_t s) {
   const long long total = (long long)N * H * W * C;
   unsigned blocks = (unsigned)((total + 255) / 256);
-  if (blocks > 148 * 32) blocks = 148 * 32;
+  if (blocks > 132 * 32) blocks = 132 * 32;
   if (!blocks) blocks = 1;
   maxpool2x2_bwd_kernel<<<blocks, 256, 0, s>>>(x, gy, N, H, W, C, gx);
   IBL_CUDA_OK(cudaGetLastError());
   return IBL_OK;
 }
 
-// ---- wgrad on tcgen05 ----------------------------------------------------------------------------------------
+// ---- wgrad on the tensor cores ----------------------------------------------------------------------------------------
 struct WgradArgs {
   int N, H, W, cin, cout;
   int tiles_w, tiles_h;        // 16 x 4-pixel boxes per image
@@ -154,17 +140,16 @@ constexpr int WG_BOX = 8192;                    // [64 px][64 ch] bf16
 constexpr int WG_STAGE = 8 * WG_BOX;            // dY hi c0,c1 | dY lo c0,c1 | X hi c0,c1 | X lo c0,c1 = 64 KiB
 constexpr int WG_STAGES = 3;
 
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(160, 1)
 conv_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tm_ghi, const __grid_constant__ CUtensorMap tm_glo,
                      const __grid_constant__ CUtensorMap tm_xhi, const __grid_constant__ CUtensorMap tm_xlo,
                      const WgradArgs a) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + WG_STAGES * WG_STAGE);
+  float* stg = reinterpret_cast<float*>(smem + WG_STAGES * WG_STAGE);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + WG_STAGES * WG_STAGE + ACC_STG_BYTES);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + WG_STAGES;
-  uint64_t* d_full = bars + 2 * WG_STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * WG_STAGES + 1);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   // item = ((split * 9 + tap) * m_tiles + mt) * n_tiles + nt
@@ -177,25 +162,19 @@ conv_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tm_ghi, const __grid_co
   const long long per = (a.boxes + a.splits - 1) / a.splits;
   const long long b0 = (long long)split * per, b1 = (b0 + per < a.boxes) ? b0 + per : a.boxes;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 4 && lane == 0) {
     tma_prefetch_desc(&tm_ghi); tma_prefetch_desc(&tm_glo); tma_prefetch_desc(&tm_xhi); tma_prefetch_desc(&tm_xlo);
-    for (int i = 0; i < WG_STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-    mbar_init(d_full, 1);
+    for (int i = 0; i < WG_STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 4); }
     fence_barrier_init();
     fence_proxy_async();
   }
-  if (warp == 1) { tmem_alloc(tmem_slot, 128); tmem_relinquish(); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  // Producer and MMA issuer: the whole warp walks the loop in convergent code and ONE ELECTED lane (elect.sync) issues a
-  // stage's TMA / tcgen05 instructions, with ring position and addresses made warp-uniform -- see the MMA issuer of
-  // conv3x3_tc_kernel (tc_conv.cu) for what `if (lane == 0)` costs per instruction.
-  if (warp == 0) {
+  if (warp == 4) {
+    // producer: the whole warp walks the loop in convergent code and ONE ELECTED lane (elect.sync) issues a stage's
+    // TMA instructions, with ring position and addresses made warp-uniform
     const uint32_t smem_a = warp_uniform(smem_u32(smem));
-    const uint32_t full_a = smem_a + WG_STAGES * WG_STAGE, empty_a = full_a + 8 * WG_STAGES;
+    const uint32_t full_a = smem_a + WG_STAGES * WG_STAGE + ACC_STG_BYTES, empty_a = full_a + 8 * WG_STAGES;
     int stage = 0; uint32_t phase = 0;
     const int per_img = a.tiles_h * a.tiles_w;
     const int co0 = mt * 128, ci0 = nt * 128;
@@ -221,46 +200,46 @@ conv_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tm_ghi, const __grid_co
       __syncwarp();
       if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
     }
-  } else if (warp == 1) {
-    constexpr uint32_t idesc = bwd_idesc_mn(128, 128);
-    const uint32_t tmem_u = warp_uniform(tmem_base);
-    const uint32_t smem_a = warp_uniform(smem_u32(smem));
-    const uint32_t full_a = smem_a + WG_STAGES * WG_STAGE, empty_a = full_a + 8 * WG_STAGES, dfull_a = full_a + 16 * WG_STAGES;
-    int stage = 0; uint32_t phase = 0;
-    for (long long b = b0; b < b1; ++b) {
-      const uint32_t sg = warp_uniform((uint32_t)stage);
-      mbar_wait_warp_a(full_a + 8 * sg, phase);
-      tc_fence_after();
-      const uint32_t sa = smem_a + sg * WG_STAGE;
-      if (elect_one()) {
+  } else {
+    // consumer warpgroup: D[co][ci] over the pixel range, both operands MN-major; then thread = output channel row
+    const int co = mt * 128 + threadIdx.x;
+    float* po = a.part + (((long long)split * 9 + tap) * a.cout + co) * a.cin + nt * 128;
+    if (b1 > b0) {
+      const uint32_t smem_a = smem_u32(smem);
+      Acc128<128> acc;
+      int stage = 0; uint32_t phase = 0;
+      int prev = -1;
+      for (long long b = b0; b < b1; ++b) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = smem_a + stage * WG_STAGE;
+        wgmma_fence();
 #pragma unroll
         for (int ks = 0; ks < 4; ++ks) {          // 16 pixel rows (2048 B) per MMA
           const uint32_t off = ks * 2048;
-          const uint64_t gh = bwd_desc_mnmajor_sw128(sa + off, WG_BOX);
-          const uint64_t gl = bwd_desc_mnmajor_sw128(sa + 2 * WG_BOX + off, WG_BOX);
-          const uint64_t xh = bwd_desc_mnmajor_sw128(sa + 4 * WG_BOX + off, WG_BOX);
-          const uint64_t xl = bwd_desc_mnmajor_sw128(sa + 6 * WG_BOX + off, WG_BOX);
-          umma_bf16(tmem_u, gl, xh, idesc, (b == b0 && ks == 0) ? 0u : 1u);
-          umma_bf16(tmem_u, gh, xl, idesc, 1u);
-          umma_bf16(tmem_u, gh, xh, idesc, 1u);
+          // A = dY: output channels 0-63 / 64-127 of the tile are the two 64-channel boxes (one MN atom each)
+          const uint64_t gh0 = gmma_desc_mnmajor_sw128(sa + off, WG_BOX);
+          const uint64_t gh1 = gmma_desc_mnmajor_sw128(sa + WG_BOX + off, WG_BOX);
+          const uint64_t gl0 = gmma_desc_mnmajor_sw128(sa + 2 * WG_BOX + off, WG_BOX);
+          const uint64_t gl1 = gmma_desc_mnmajor_sw128(sa + 3 * WG_BOX + off, WG_BOX);
+          // B = X: 128 input channels = two MN atoms WG_BOX apart
+          const uint64_t xh = gmma_desc_mnmajor_sw128(sa + 4 * WG_BOX + off, WG_BOX);
+          const uint64_t xl = gmma_desc_mnmajor_sw128(sa + 6 * WG_BOX + off, WG_BOX);
+          acc.mma<false, 1, 1>(gl0, gl1, xh, (b == b0 && ks == 0) ? 0u : 1u);
+          acc.mma<false, 1, 1>(gh0, gh1, xl, 1u);
+          acc.mma<false, 1, 1>(gh0, gh1, xh, 1u);
         }
-        umma_commit_a(empty_a + 8 * sg);
-        if (b == b1 - 1) umma_commit_a(dfull_a);   // same elected thread as the MMAs it covers
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
       }
-      __syncwarp();
-      if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
-    }
-  } else {
-    const int q = warp & 3;
-    const int co = mt * 128 + q * 32 + lane;            // TMEM lane == output channel inside the tile
-    float* po = a.part + (((long long)split * 9 + tap) * a.cout + co) * a.cin + nt * 128;
-    if (b1 > b0) {
-      mbar_wait(d_full, 0);
-      tc_fence_after();
+      wgmma_wait<0>();
+      acc.fence_operands();
+#pragma unroll
       for (int ch = 0; ch < 4; ++ch) {
         uint32_t r[32];
-        tmem_ld_32x32(tmem_base + ((uint32_t)(q * 32) << 16) + ch * 32, r);
-        tmem_ld_wait();
+        acc.rows32(ch, stg, r);
         if (co < a.cout) {
 #pragma unroll
           for (int j = 0; j < 32; ++j) {
@@ -274,9 +253,6 @@ conv_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tm_ghi, const __grid_co
         if (nt * 128 + j < a.cin) po[j] = 0.f;
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, 128); }
 }
 
 // dW[co][ci][kh][kw] = sum_s part[s][tap][co][ci]
@@ -310,7 +286,7 @@ int wgrad_tc_splits(int N, int H, int W, int cin, int cout) {
 int launch_conv_wgrad_tc(const __nv_bfloat16* g_hi, const __nv_bfloat16* g_lo, const __nv_bfloat16* x_hi,
                          const __nv_bfloat16* x_lo, int N, int H, int W, int cin, int cout, float* part, int splits,
                          float* bpart, float* dw_oihw, float* db, cudaStream_t s) {
-  IBL_REQUIRE(cin % 64 == 0 && cout % 64 == 0, "tcgen05 wgrad needs Cin%64==0 and Cout%64==0");
+  IBL_REQUIRE(cin % 64 == 0 && cout % 64 == 0, "tensor-core wgrad needs Cin%64==0 and Cout%64==0");
   CUtensorMap m_ghi, m_glo, m_xhi, m_xlo;
   {
     uint64_t dims[4] = {(uint64_t)cout, (uint64_t)W, (uint64_t)H, (uint64_t)N};
@@ -333,14 +309,14 @@ int launch_conv_wgrad_tc(const __nv_bfloat16* g_hi, const __nv_bfloat16* g_lo, c
   a.splits = splits;
   a.boxes = (long long)N * a.tiles_h * a.tiles_w;
   a.part = part;
-  const int smem = WG_STAGES * WG_STAGE + 1024 + 128;
+  const int smem = WG_STAGES * WG_STAGE + ACC_STG_BYTES + 1024 + 128;
   static DeviceOnce attr_done;
   if (!attr_done.done()) {
     IBL_CUDA_OK(cudaFuncSetAttribute(conv_wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     attr_done.mark();
   }
   const int grid = splits * 9 * a.m_tiles * a.n_tiles;
-  conv_wgrad_tc_kernel<<<grid, 192, smem, s>>>(m_ghi, m_glo, m_xhi, m_xlo, a);
+  conv_wgrad_tc_kernel<<<grid, 160, smem, s>>>(m_ghi, m_glo, m_xhi, m_xlo, a);
   IBL_CUDA_OK(cudaGetLastError());
   const long long total = (long long)cout * cin * 9;
   int blocks = (int)((total + 255) / 256);

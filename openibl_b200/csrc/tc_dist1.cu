@@ -7,9 +7,9 @@
 //                             [0.5,1): no overflow, 11 significant bits), exact fp32 |x|^2 (same summation order as
 //                             planes_sqnorm_kernel, so the exact distances below are unchanged), the 4-norm and
 //                             the max of each row (error model of the guard);
-//   2. gemm2_f16_top16_kernel tcgen05.mma.cta_group::2 kind::f16 (fp16 x fp16 -> fp32 in TMEM), ONE MMA per
-//                             K step, 256 queries x 256 database rows per SM pair, 6-stage TMA ring, running
-//                             top-16 per query in registers across the pair's database range;
+//   2. gemm_f16_top16_kernel  wgmma f16 (fp16 x fp16 -> fp32 in registers), ONE MMA per K step and 64-row
+//                             half, 128 queries x 128 database rows per tile, 5-stage TMA ring, running
+//                             top-16 per query in registers across the CTA's database range;
 //   3. dist_finish_kernel     per query: merge of the per-range candidate lists, exact fp32 re-scoring of the 16
 //                             survivors (|q|^2 + |d|^2 - 2 q.d, bit-identical to round 1's rescore_sort_kernel),
 //                             final (dist, idx) sort, and the GUARD: a database row that was NOT kept has a
@@ -95,20 +95,16 @@ __global__ void dist_colmax_kernel(const float4* __restrict__ aux, int n, float*
   }
 }
 
-// ---- 2. screening GEMM on SM pairs ----------------------------------------------------------------
+// ---- 2. screening GEMM (fp16 wgmma) ----------------------------------------------------------------
 struct Dist1Args {
   int M, N, K;
-  int n_tiles, nt_per_item, items_per_mpair, total_items, n_valid;
+  int n_tiles, nt_per_item, items_per_mtile, total_items, n_valid;
   const float4* a_aux;  // per query  {|q|^2, 2^eq, ...}
   const float4* b_aux;  // per db row {|d|^2, 2^ed, ...}
-  float* cand_d;        // [items_per_mpair][M][16] screened distances
-  int* cand_i;          // [items_per_mpair][M][16] local database rows (-1: none)
+  float* cand_d;        // [items_per_mtile][M][16] screened distances
+  int* cand_i;          // [items_per_mtile][M][16] local database rows (-1: none)
   unsigned* gate;       // [M] orderable bits of the smallest 16th-best distance any work item of this query has reached
 };
-
-__host__ __device__ constexpr uint32_t umma_idesc_f16_f32(int M, int N) {   // kind::f16, fp16 A/B, fp32 accumulator
-  return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
 
 __device__ __forceinline__ uint32_t d1_ord(float f) {
   uint32_t u = __float_as_uint(f);
@@ -127,178 +123,93 @@ __device__ __forceinline__ float2 d1_lds64(uint32_t addr) {
   return v;
 }
 
-constexpr int D1_BN = 256, D1_BK = 64;
+constexpr int D1_BN = 128, D1_BK = 64;
 constexpr int D1_PEND = 32;                            // pending candidates per row between two merges (see the epilogue)
 constexpr int D1_A_BYTES = 128 * D1_BK * 2;            // 16 KiB: this CTA's 128 query rows
-constexpr int D1_BH_BYTES = (D1_BN / 2) * D1_BK * 2;   // 16 KiB: this CTA's half of one 256-row database sub-tile
+constexpr int D1_B_BYTES = D1_BN * D1_BK * 2;          // 16 KiB: one 128-row database tile
+constexpr int D1_STAGES = 5;
+constexpr int D1_STAGE = D1_A_BYTES + D1_B_BYTES;
+constexpr int D1_BARS = 256;                           // mbarriers
+constexpr int D1_BSTAGE = 4 * 32 * 8;                  // per consumer warp: {|d|^2, 2^e} of the 32 columns of a chunk
+constexpr int D1_PENDB = 128 * D1_PEND * 8;            // per query row: D1_PEND pending (distance, column) pairs
+constexpr int D1_SMEM = D1_STAGES * D1_STAGE + ACC_STG_BYTES + D1_BARS + D1_BSTAGE + D1_PENDB + 1024;
+static_assert(D1_SMEM <= 232448, "shared-memory budget of the screening kernel");
 
-// SUB = 256-row database sub-tiles per work tile.  SUB = 1 (default): 256 x 256 tiles, two 256-column accumulators, the
-// epilogue of tile i runs under the main loop of tile i+1.  SUB = 2 (IBL_DIST_BN=512): a 256 x 512 tile reuses every
-// staged query block for two MMAs (48 KiB per stage instead of 2 x 32: 25 % less L2->SM traffic) but has ONE 512-column
-// accumulator, so epilogue and main loop alternate.  Measured (profiles/r02_dist_variants_s8.jsonl, whole call,
-// 6.8k x {10k, 31k, 250k} x 4096): SUB = 1 0.70 / 1.62 / 11.9 ms, SUB = 2 0.79 / 1.80 / 12.4 ms.
-template <int SUB> struct D1Cfg {
-  static constexpr int STAGES = SUB == 1 ? 6 : 4;
-  static constexpr int STAGE = D1_A_BYTES + SUB * D1_BH_BYTES;
-  static constexpr int TILE_N = D1_BN * SUB;
-  static constexpr int ACC_BUFS = SUB == 1 ? 2 : 1;
-  static constexpr int BARS = 256;                      // mbarriers + the TMEM slot
-  static constexpr int BSTAGE = 4 * 32 * 8;             // per epilogue warp: {|d|^2, 2^e} of the 32 columns of a chunk
-  static constexpr int PEND = 128 * D1_PEND * 8;        // per query row: D1_PEND pending (distance, column) pairs
-  static constexpr int SMEM = STAGES * STAGE + BARS + BSTAGE + PEND + 1024;
-};
-
-// SM pairs: the peer CTA's producer does NOT arrive on the leader's full barrier.  The leader's single
-// arrive.expect_tx names the bytes of BOTH CTAs; the peer's TMA completions decrement the same transaction count
-// (complete_tx may land before the expect_tx: the phase still cannot complete before the leader's arrival).  Round 1
-// had the peer do an `mbarrier.arrive.release.cluster` per stage; removing it was worth ~2 %.  The peer cannot lap the
-// ring: it waits on its local empty barrier, which the leader's multicast commit signals.
-//
-// What actually bounded this kernel (ncu source view, profiles/r02_dist_f16_v{2,3,4}*.md): the EPILOGUE.  At 10 k
-// database rows per query the sorted insertion ran for half of all columns (any of a warp's 32 rows inserting) at
-// ~110 instructions a time, one warp per scheduler: 968 us with the tensor pipe 27 % active.  The pending-list epilogue
-// below brought the kernel to the MMA/L2 bound (whole call 1.24 -> 0.70 ms).
-template <int SUB>
-__global__ void __launch_bounds__(192, 1)
-gemm2_f16_top16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
-                       const Dist1Args g) {
-  using C = D1Cfg<SUB>;
-  constexpr int STAGES = C::STAGES, STAGE = C::STAGE, TILE_N = C::TILE_N;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int unit0 = blockIdx.x >> 1, unit_stride = gridDim.x >> 1;
+// What bounded this kernel (profiled on the previous generation's tensor cores): the EPILOGUE.  At 10 k database rows
+// per query a sorted insertion per column ran for half of all columns (any of a warp's 32 rows inserting) at ~110
+// instructions a time.  The pending-list epilogue below brings it to the MMA/L2 bound.
+__global__ void __launch_bounds__(160, 1)
+gemm_f16_top16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
+                      const Dist1Args g) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE);
-  uint64_t* full_bar = bars;                    // leader's are used: count 1 (the leader's arrive.expect_tx for both CTAs)
-  uint64_t* empty_bar = bars + STAGES;          // local, count 1 (multicast commit)
-  uint64_t* tfull_bar = bars + 2 * STAGES;      // local, count 1 (multicast commit)
-  uint64_t* tempty_bar = bars + 2 * STAGES + 2; // leader's are used: count 8 (4 epilogue warps x 2 CTAs)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
+  float* stg = reinterpret_cast<float*>(smem + D1_STAGES * D1_STAGE);
+  uint8_t* tail = smem + D1_STAGES * D1_STAGE + ACC_STG_BYTES;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(tail);
+  uint64_t* full_bar = bars;
+  uint64_t* empty_bar = bars + D1_STAGES;       // one arrival per consumer warp
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 4 && lane == 0) {
     tma_prefetch_desc(&tm_a); tma_prefetch_desc(&tm_b);
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-    mbar_init(&tfull_bar[0], 1); mbar_init(&tfull_bar[1], 1);
-    mbar_init(&tempty_bar[0], 8); mbar_init(&tempty_bar[1], 8);
+    for (int i = 0; i < D1_STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 4); }
     fence_barrier_init();
     fence_proxy_async();
   }
-  if (warp == 1) tmem_alloc_2sm(tmem_slot, 512);   // both CTAs, same warp id: one allocation spanning the pair
-  tc_fence_before();
   __syncthreads();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  auto decode = [&](int item, int& mp, int& nt0, int& ntn) {
-    mp = item / g.items_per_mpair;
-    const int sub = item - mp * g.items_per_mpair;
+  auto decode = [&](int item, int& mt, int& nt0, int& ntn) {
+    mt = item / g.items_per_mtile;
+    const int sub = item - mt * g.items_per_mtile;
     nt0 = sub * g.nt_per_item;
     ntn = (nt0 + g.nt_per_item <= g.n_tiles) ? g.nt_per_item : (g.n_tiles - nt0);
   };
   const int kiters = g.K / D1_BK;
 
-  if (warp == 0) {
-    // TMA producer (both CTAs): convergent warp, one elected lane issues, warp-uniform operands (tc_conv.cu)
-    {
-      const uint32_t smem_a = warp_uniform(smem_u32(smem));
-      const uint32_t bars_a = smem_a + STAGES * STAGE;
-      const uint32_t full_a = bars_a, empty_a = bars_a + 8 * STAGES;
-      const uint32_t full_c = warp_uniform(mapa_u32(full_a, 0));   // the leader's barriers, shared::cluster addresses
-      const int rank_u = (int)warp_uniform(rank);
-      int stage = 0; uint32_t phase = 0;
-      for (int item = unit0; item < g.total_items; item += unit_stride) {
-        int mp, nt0, ntn;
-        decode(item, mp, nt0, ntn);
-        const int row0 = (int)warp_uniform((uint32_t)((mp * 2 + rank_u) * 128));
-        for (int nt = nt0; nt < nt0 + ntn; ++nt) {
-          const int col0 = (int)warp_uniform((uint32_t)(nt * TILE_N + rank_u * (D1_BN / 2)));
-          for (int kit = 0; kit < kiters; ++kit) {
-            const uint32_t sg = warp_uniform((uint32_t)stage);
-            mbar_wait_warp_a(empty_a + 8 * sg, phase ^ 1);
-            const uint32_t st = smem_a + sg * STAGE;
-            const int k0 = (int)warp_uniform((uint32_t)(kit * D1_BK));
-            if (elect_one()) {
-              if (leader) mbar_arrive_expect_tx_a(full_a + 8 * sg, 2 * STAGE);   // bytes of BOTH CTAs; the peer only loads
-              tma_load_2d_2sm_a(st, &tm_a, full_c + 8 * sg, k0, row0);
-#pragma unroll
-              for (int j = 0; j < SUB; ++j)     // rows beyond the matrix are zero-filled by the TMA unit
-                tma_load_2d_2sm_a(st + D1_A_BYTES + j * D1_BH_BYTES, &tm_b, full_c + 8 * sg, k0, col0 + j * D1_BN);
-            }
-            __syncwarp();
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
+  if (warp == 4) {
+    // TMA producer: convergent warp, one elected lane issues, warp-uniform operands
+    const uint32_t smem_a = warp_uniform(smem_u32(smem));
+    const uint32_t bars_a = smem_a + D1_STAGES * D1_STAGE + ACC_STG_BYTES;
+    const uint32_t full_a = bars_a, empty_a = bars_a + 8 * D1_STAGES;
+    int stage = 0; uint32_t phase = 0;
+    for (int item = blockIdx.x; item < g.total_items; item += gridDim.x) {
+      int mt, nt0, ntn;
+      decode(item, mt, nt0, ntn);
+      const int row0 = (int)warp_uniform((uint32_t)(mt * 128));
+      for (int nt = nt0; nt < nt0 + ntn; ++nt) {
+        const int col0 = (int)warp_uniform((uint32_t)(nt * D1_BN));
+        for (int kit = 0; kit < kiters; ++kit) {
+          const uint32_t sg = warp_uniform((uint32_t)stage);
+          mbar_wait_warp_a(empty_a + 8 * sg, phase ^ 1);
+          const uint32_t st = smem_a + sg * D1_STAGE, fb = full_a + 8 * sg;
+          const int k0 = (int)warp_uniform((uint32_t)(kit * D1_BK));
+          if (elect_one()) {
+            mbar_arrive_expect_tx_a(fb, D1_STAGE);
+            tma_load_2d_a(st, &tm_a, fb, k0, row0);
+            tma_load_2d_a(st + D1_A_BYTES, &tm_b, fb, k0, col0);   // rows beyond the matrix are zero-filled
           }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // whole warp in convergent code, one elected lane issues, ring position / bases warp-uniform: every tcgen05 operand lives in a
-    // uniform register (tc_conv.cu, MMA issuer)
-    if (warp_uniform(leader ? 1u : 0u)) {
-      constexpr uint32_t idesc = umma_idesc_f16_f32(256, D1_BN);
-      const uint32_t tmem_u = warp_uniform(tmem_base);
-      const uint32_t smem_a = warp_uniform(smem_u32(smem));
-      const uint32_t bars_a = smem_a + STAGES * STAGE;
-      const uint32_t full_a = bars_a, empty_a = bars_a + 8 * STAGES;
-      const uint32_t tfull_a = bars_a + 16 * STAGES, tempty_a = tfull_a + 16;
-      int stage = 0; uint32_t phase = 0;
-      int it = 0;
-      for (int item = unit0; item < g.total_items; item += unit_stride) {
-        int mp, nt0, ntn;
-        decode(item, mp, nt0, ntn);
-        for (int nt = nt0; nt < nt0 + ntn; ++nt, ++it) {
-          const uint32_t as = warp_uniform((uint32_t)(C::ACC_BUFS == 2 ? (it & 1) : 0));
-          const uint32_t aphase = C::ACC_BUFS == 2 ? ((it >> 1) & 1) : (it & 1);
-          mbar_wait_warp_a(tempty_a + 8 * as, aphase ^ 1);
-          tc_fence_after();
-          const uint32_t d_tmem = tmem_u + as * D1_BN;
-          for (int kit = 0; kit < kiters; ++kit) {
-            const uint32_t st = warp_uniform((uint32_t)stage);
-            mbar_wait_warp_a(full_a + 8 * st, phase);
-            tc_fence_after();
-            const uint32_t sa = smem_a + st * STAGE;
-            if (elect_one()) {
-              const uint64_t a = umma_desc_kmajor_sw128(sa);
-#pragma unroll
-              for (int k = 0; k < D1_BK / 16; ++k) {
-#pragma unroll
-                for (int j = 0; j < SUB; ++j) {
-                  const uint64_t b = umma_desc_kmajor_sw128(sa + D1_A_BYTES + j * D1_BH_BYTES);
-                  umma_bf16_2sm(d_tmem + j * D1_BN, a + (uint64_t)(k * 2), b + (uint64_t)(k * 2), idesc,
-                                (kit > 0 || k > 0) ? 1u : 0u);
-                }
-              }
-              umma_commit_2sm_mc_a(empty_a + 8 * st, 0x3);
-              if (kit == kiters - 1) umma_commit_2sm_mc_a(tfull_a + 8 * as, 0x3);   // same elected thread as the MMAs
-            }
-            __syncwarp();
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
-          }
+          __syncwarp();
+          if (++stage == D1_STAGES) { stage = 0; phase ^= 1; }
         }
       }
     }
   } else {
-    // Epilogue: one warp per scheduler, one thread per query row, 256+ accumulator columns per tile.  With a single
-    // warp per scheduler every instruction counts (no other warp hides a dependent issue), and ncu's source view of the
-    // first version -- a sorted 16-entry insertion behind `if (d < td[15])` for every column -- showed ~85 executed
-    // warp instructions per column: whenever ANY of the 32 rows of the warp inserts (half of all columns at 10 k
-    // database rows per query) the whole warp walks the ~110-instruction insertion.  Here the per-column work is
-    // scale + compare + a predicated 8-byte shared-memory append to a per-row pending list; the lists are merged into
-    // the sorted top-16 in a compact loop (trip count = the longest list of the warp) when one could overflow within
-    // the next 16 columns, and at the end of every tile.  All 32 rows insert side by side in that loop, so the walk runs
-    // once per ~16 appended candidates of the fullest row instead of once per column with a candidate anywhere.
-    const int q = warp & 3;
-    const int rloc = q * 32 + lane;
+    // Consumer warpgroup: fp16 wgmma main loop, then one thread per query row.  The per-column work is scale + compare
+    // + a predicated 8-byte shared-memory append to a per-row pending list; the lists are merged into the sorted top-16
+    // in a compact loop (trip count = the longest list of the warp) when one could overflow within the next 16 columns,
+    // and at the end of every tile.  All 32 rows of a warp insert side by side in that loop, so the walk runs once per
+    // ~16 appended candidates of the fullest row instead of once per column with a candidate anywhere.
+    const int q = warp;
+    const int rloc = threadIdx.x;
+    const uint32_t smem_a = smem_u32(smem);
     // shared-state-space addresses (the generic pointer arithmetic above makes the compiler emit generic LD/ST)
-    const uint32_t bst = smem_u32(smem + STAGES * STAGE + C::BARS) + q * 256;
-    const uint32_t pend = smem_u32(smem + STAGES * STAGE + C::BARS + C::BSTAGE) + rloc * 8;   // [slot][128 rows] x 8 B
-    int it = 0;
-    for (int item = unit0; item < g.total_items; item += unit_stride) {
-      int mp, nt0, ntn;
-      decode(item, mp, nt0, ntn);
-      const int row = (mp * 2 + (int)rank) * 128 + rloc;
+    const uint32_t bst = smem_u32(tail + D1_BARS) + q * 256;
+    const uint32_t pend = smem_u32(tail + D1_BARS + D1_BSTAGE) + rloc * 8;   // [slot][128 rows] x 8 B
+    int stage = 0; uint32_t phase = 0;
+    for (int item = blockIdx.x; item < g.total_items; item += gridDim.x) {
+      int mt, nt0, ntn;
+      decode(item, mt, nt0, ntn);
+      const int row = mt * 128 + rloc;
       const bool row_ok = row < g.M;
       float an = 0.f, m2sa = 0.f;
       if (row_ok) { const float4 t = __ldg(g.a_aux + row); an = t.x; m2sa = -2.f * t.y; }
@@ -336,9 +247,7 @@ gemm2_f16_top16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_co
         }
         paddr = pend;
       };
-      for (int nt = nt0; nt < nt0 + ntn; ++nt, ++it) {
-        const int as = C::ACC_BUFS == 2 ? (it & 1) : 0;
-        const uint32_t aphase = C::ACC_BUFS == 2 ? ((it >> 1) & 1) : (it & 1);
+      for (int nt = nt0; nt < nt0 + ntn; ++nt) {
         // Shared gate: the work items of one query block scan different database ranges concurrently, each keeping its
         // own top-16.  An element that is not below the 16th-best distance ANY of them has already reached cannot be in
         // the merged top-16, so every item publishes its 16th-best (atomicMin) after each tile and reads the common
@@ -348,24 +257,40 @@ gemm2_f16_top16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_co
           const unsigned gv = *reinterpret_cast<volatile unsigned*>(g.gate + row);
           if (gv != 0xFFFFFFFFu) thr = fminf(thr, d1_unord(gv));       // 0xFFFFFFFF = "no gate yet" (the memset pattern)
         }
-        mbar_wait(&tfull_bar[as], aphase);
-        tc_fence_after();
-        const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16) + as * D1_BN;
-#pragma unroll 1
-        for (int ch = 0; ch < TILE_N / 32; ++ch) {
-          const int col0 = nt * TILE_N + ch * 32;
-          if (col0 >= g.n_valid) break;                    // warp-uniform: the rest of the tile is padding
+        Acc128<D1_BN> acc;
+        int prev = -1;
+        for (int kit = 0; kit < kiters; ++kit) {
+          mbar_wait(&full_bar[stage], phase);
+          const uint32_t sa = smem_a + stage * D1_STAGE;
+          const uint64_t da = gmma_desc_kmajor_sw128(sa), db = gmma_desc_kmajor_sw128(sa + D1_A_BYTES);
+          constexpr uint64_t kHalf = 64 * 128 / 16;   // query rows 64-127: +8 KiB
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < D1_BK / 16; ++k)
+            acc.mma<true>(da + (uint64_t)(k * 2), da + kHalf + (uint64_t)(k * 2), db + (uint64_t)(k * 2),
+                          (kit > 0 || k > 0) ? 1u : 0u);
+          wgmma_commit();
+          wgmma_wait<1>();
+          if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+          prev = stage;
+          if (++stage == D1_STAGES) { stage = 0; phase ^= 1; }
+        }
+        wgmma_wait<0>();
+        acc.fence_operands();
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+#pragma unroll
+        for (int ch = 0; ch < D1_BN / 32; ++ch) {     // unrolled: the accumulator is indexed with constants only
+          const int col0 = nt * D1_BN + ch * 32;
+          if (col0 >= g.n_valid) break;                    // block-uniform: the rest of the tile is padding
           // The per-column terms {|d|^2, 2^e} of this chunk: ONE coalesced load (lane j fetches column col0 + j) staged
-          // in shared memory and read back as warp-wide broadcasts.  A `__ldg(b_aux + col)` per column, as round 1's
-          // kernels did, is a chain of 256 dependent L2-latency loads per tile.
+          // in shared memory and read back as warp-wide broadcasts, instead of a chain of dependent per-column loads.
           float2 mine = make_float2(INFINITY, 0.f);        // padding columns: +inf, never below the threshold
           if (col0 + lane < g.n_valid) { const float4 t = __ldg(g.b_aux + col0 + lane); mine = make_float2(t.x, t.y); }
           uint32_t raw[32];
-          tmem_ld_32x32(t_row + ch * 32, raw);
+          acc.rows32(ch, stg, raw);
           __syncwarp();                                    // the previous chunk's broadcast reads are done
           d1_sts64(bst + lane * 8, mine.x, mine.y);
           __syncwarp();
-          tmem_ld_wait();
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             if (__any_sync(0xffffffffu, paddr > pend + (D1_PEND - 16) * 1024)) {   // could overflow within 16 columns: merge first
@@ -383,20 +308,14 @@ gemm2_f16_top16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_co
             }
           }
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) {
-          if (leader) mbar_arrive(&tempty_bar[as]);
-          else mbar_arrive_remote(mapa_u32(smem_u32(&tempty_bar[as]), 0));
-        }
-        merge_pending();                                   // after the accumulator is released: overlaps the next main loop
+        merge_pending();
         if (row_ok && td[15] < thr) {
           thr = td[15];
           atomicMin(g.gate + row, d1_ord(thr));
         }
       }
       if (row_ok) {
-        const int sub = item % g.items_per_mpair;
+        const int sub = item % g.items_per_mtile;
         float4* od = reinterpret_cast<float4*>(g.cand_d + ((long long)sub * g.M + row) * 16);
         int4* oi = reinterpret_cast<int4*>(g.cand_i + ((long long)sub * g.M + row) * 16);
 #pragma unroll
@@ -406,13 +325,6 @@ gemm2_f16_top16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_co
         }
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc_2sm(tmem_base, 512);
   }
 }
 
@@ -643,14 +555,14 @@ dist_exact_merge_kernel(const ExactArgs g) {
 }
 
 // ---- host -----------------------------------------------------------------------------------------
-static int pick_runs1(int m_pairs, int n_tiles) {
-  const int G = device_sm_count() / 2;
+static int pick_runs1(int m_tiles, int n_tiles) {
+  const int G = device_sm_count();
   int best = 1;
   double best_eff = -1.0;
   for (int r = 1; r <= n_tiles && r <= 8; ++r) {          // dist_finish_kernel merges up to 8 x 16 candidates
     const int per = cdiv(n_tiles, r), runs = cdiv(n_tiles, per);
-    const long long total = (long long)m_pairs * runs, waves = (total + G - 1) / G;
-    const double eff = (double)m_pairs * n_tiles / ((double)waves * G * per);
+    const long long total = (long long)m_tiles * runs, waves = (total + G - 1) / G;
+    const double eff = (double)m_tiles * n_tiles / ((double)waves * G * per);
     if (eff > best_eff + 1e-9) { best_eff = eff; best = runs; }
   }
   return best;
@@ -707,47 +619,30 @@ int launch_dist_topk_1pass(const float* q, int m, const float* db, int n, int n_
     IBL_RET(make_tmap(&ma, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, qp, dims_a, str, box));
     IBL_RET(make_tmap(&mb, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, dp, dims_b, str, box));
   }
-  // default: 256 x 256 tiles with two overlapped accumulators; IBL_DIST_BN=512 selects the 256 x 512 tile (variant tests)
-  static const int tile_env = [] { const char* v = getenv("IBL_DIST_BN"); return v ? atoi(v) : 256; }();
-  const int SUBn = tile_env == 256 ? 1 : 2;
   Dist1Args g{};
   g.M = m; g.N = n; g.K = d;
-  g.n_tiles = cdiv(n_valid, D1_BN * SUBn);
-  const int m_pairs = cdiv(cdiv(m, 128), 2);
-  const int runs = pick_runs1(m_pairs, g.n_tiles);
+  g.n_tiles = cdiv(n_valid, D1_BN);
+  const int m_tiles = cdiv(m, 128);
+  const int runs = pick_runs1(m_tiles, g.n_tiles);
   g.nt_per_item = cdiv(g.n_tiles, runs);
-  g.items_per_mpair = cdiv(g.n_tiles, g.nt_per_item);
-  g.total_items = m_pairs * g.items_per_mpair;
+  g.items_per_mtile = cdiv(g.n_tiles, g.nt_per_item);
+  g.total_items = m_tiles * g.items_per_mtile;
   g.n_valid = n_valid;
   g.a_aux = qa; g.b_aux = da; g.cand_d = cd; g.cand_i = ci; g.gate = gate;
   static DeviceOnce attr_done;   // the attributes are per device
   if (!attr_done.done()) {
-    IBL_CUDA_OK(cudaFuncSetAttribute(gemm2_f16_top16_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, D1Cfg<1>::SMEM));
-    IBL_CUDA_OK(cudaFuncSetAttribute(gemm2_f16_top16_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, D1Cfg<2>::SMEM));
+    IBL_CUDA_OK(cudaFuncSetAttribute(gemm_f16_top16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, D1_SMEM));
     IBL_CUDA_OK(cudaFuncSetAttribute(dist_finish_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
     IBL_CUDA_OK(cudaFuncSetAttribute(dist_exact_chunk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
     attr_done.mark();
   }
-  const int pairs = device_sm_count() / 2;
-  const int units = g.total_items < pairs ? g.total_items : pairs;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(2 * units);
-  cfg.blockDim = dim3(192);
-  cfg.dynamicSmemBytes = SUBn == 1 ? D1Cfg<1>::SMEM : D1Cfg<2>::SMEM;
-  cfg.stream = s;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  if (SUBn == 1) IBL_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm2_f16_top16_kernel<1>, ma, mb, g));
-  else IBL_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm2_f16_top16_kernel<2>, ma, mb, g));
+  const int sms = device_sm_count();
+  gemm_f16_top16_kernel<<<g.total_items < sms ? g.total_items : sms, 160, D1_SMEM, s>>>(ma, mb, g);
+  IBL_CUDA_OK(cudaGetLastError());
 
   FinishArgs f{};
   f.q = q; f.db = db; f.q_aux = qa; f.db_aux = da; f.db_max2 = dmax2; f.cand_d = cd; f.cand_i = ci;
-  f.m = m; f.d = d; f.runs = g.items_per_mpair; f.k_out = k; f.n_valid = n_valid; f.idx_base = idx_base;
+  f.m = m; f.d = d; f.runs = g.items_per_mtile; f.k_out = k; f.n_valid = n_valid; f.idx_base = idx_base;
   f.out_dist = out_dist; f.out_idx = out_idx; f.flag_count = fcount; f.flag_list = flist;
   const size_t qsm = d <= 16384 ? (size_t)d * sizeof(float) : 16;
   dist_finish_kernel<<<m, 128, qsm, s>>>(f);

@@ -1,6 +1,6 @@
-// tcgen05 "NT" GEMM with fp32-grade operands:  acc[i,j] = sum_k A[i,k] * B[j,k]
+// Hopper "NT" GEMM with fp32-grade operands:  acc[i,j] = sum_k A[i,k] * B[j,k]
 // A [M,K] and B [N,K] are row-major fp32 matrices carried as bf16 hi/lo planes; every K-chunk
-// issues A_lo.B_hi + A_hi.B_lo + A_hi.B_hi into an fp32 TMEM accumulator (see tc_conv.cu).
+// issues A_lo.B_hi + A_hi.B_lo + A_hi.B_hi into an fp32 wgmma accumulator (see tc_conv.cu).
 //
 // Used for
 //   * stage (iii-b) query x database L2 distance (reference ibl/evaluators.py:127-129), with
@@ -40,66 +40,48 @@ struct GemmTcArgs {
 };
 
 constexpr int GT_BM = 128;
+constexpr int GT_BK = 64;
 
-// MC = true: the grid is launched as clusters of two CTAs that walk the same column tiles with adjacent
-// row tiles.  Each CTA fetches only half of every B tile and TMA-multicasts it into both CTAs' shared
-// memory, so the per-SM L2->SM operand traffic drops from A+B to A+B/2 per K chunk (the kernel is bound by
-// the L2 latency x bandwidth product against the ~190 KiB of stages that fit, profiles/r01_dist_tc.md).
-// A stage may be refilled only when BOTH CTAs' MMAs have released it: the MMA warp's tcgen05.commit is
-// multicast to the empty barrier of both CTAs (arrival count 2).
-template <int BN, int STAGES, int EPI, bool MC, int BK = 64>
-__global__ void __launch_bounds__(192, 1)
+// MC = true: the grid is launched as clusters of two CTAs ("SM pairs") that walk the same column tiles with adjacent
+// row tiles.  Each CTA fetches only half of every B tile and TMA-multicasts it into both CTAs' shared memory, so the
+// per-SM L2->SM operand traffic drops from A+B to A+B/2 per K chunk.  A stage may be refilled only when BOTH CTAs'
+// consumers have released it: every consumer warp arrives on the empty barrier of both CTAs (arrival count 8).
+template <int BN, int STAGES, int EPI, bool MC>
+__global__ void __launch_bounds__(160, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tm_ahi, const __grid_constant__ CUtensorMap tm_alo,
                const __grid_constant__ CUtensorMap tm_bhi, const __grid_constant__ CUtensorMap tm_blo,
                const GemmTcArgs g) {
   constexpr int CL = MC ? 2 : 1;
-  uint32_t cta_rank = 0;
-  if (MC) asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(cta_rank));
+  const uint32_t cta_rank = MC ? cluster_ctarank() : 0u;
   const int unit0 = blockIdx.x / CL, unit_stride = gridDim.x / CL;   // a unit = one CTA or one CTA pair
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  // BK = 64: 128-byte rows, 128B swizzle.  BK = 32: 64-byte rows, 64B swizzle -- half-size stages, so a
-  // 256-column tile still gets a 4-deep pipeline.
-  constexpr int A_BYTES = GT_BM * BK * 2;
-  constexpr int B_BYTES = BN * BK * 2;
+  constexpr int A_BYTES = GT_BM * GT_BK * 2;
+  constexpr int B_BYTES = BN * GT_BK * 2;
   constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
+  float* stg = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + ACC_STG_BYTES);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + STAGES;
-  uint64_t* tfull_bar = bars + 2 * STAGES;
-  uint64_t* tempty_bar = bars + 2 * STAGES + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
-  constexpr uint32_t TMEM_COLS = (2 * BN < 32) ? 32 : 2 * BN;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 0 && lane == 0) {
+  if (warp == 4 && lane == 0) {
     tma_prefetch_desc(&tm_ahi);
     tma_prefetch_desc(&tm_alo);
     tma_prefetch_desc(&tm_bhi);
     tma_prefetch_desc(&tm_blo);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], CL);
+      mbar_init(&empty_bar[i], 4 * CL);   // one arrival per consumer warp (of both CTAs of a pair)
     }
-    mbar_init(&tfull_bar[0], 1);
-    mbar_init(&tfull_bar[1], 1);
-    mbar_init(&tempty_bar[0], 4);
-    mbar_init(&tempty_bar[1], 4);
     fence_barrier_init();
     fence_proxy_async();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
   if (MC) cluster_sync_all();     // the peer's barriers exist before anything is multicast into this CTA
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  // item -> (row tile, first column tile, #column tiles, first K chunk, #K chunks); with MC an item is a
-  // pair of adjacent row tiles and this CTA takes the one matching its rank in the cluster
+  // item -> (row tile, first column tile, #column tiles, first K chunk, #K chunks); with MC an item is a pair of
+  // adjacent row tiles and this CTA takes the one matching its rank in the cluster
   auto decode = [&](int item, int& mt, int& nt0, int& ntn, int& k0, int& kn) {
     mt = item / g.items_per_mtile;
     const int sub = item - mt * g.items_per_mtile;
@@ -107,106 +89,65 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tm_ahi, const __grid_constant
     if (EPI == EPI_PARTIAL) {
       nt0 = 0; ntn = g.n_tiles;
       k0 = sub * g.kit_per_item;
-      const int ktot = g.K / BK;
+      const int ktot = g.K / GT_BK;
       kn = (k0 + g.kit_per_item <= ktot) ? g.kit_per_item : (ktot - k0);
     } else {
       nt0 = sub * g.nt_per_item;
       ntn = (nt0 + g.nt_per_item <= g.n_tiles) ? g.nt_per_item : (g.n_tiles - nt0);
-      k0 = 0; kn = g.K / BK;
+      k0 = 0; kn = g.K / GT_BK;
     }
   };
 
-  if (warp == 0) {
-    // TMA producer: convergent warp, one elected lane issues, warp-uniform operands (tc_conv.cu explains why)
-    {
-      const uint32_t smem_a = warp_uniform(smem_u32(smem));
-      const uint32_t bars_a = smem_a + STAGES * STAGE_BYTES;
-      const uint32_t full_a = bars_a, empty_a = bars_a + 8 * STAGES;
-      const int rank_u = (int)warp_uniform(cta_rank);
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int item = unit0; item < g.total_items; item += unit_stride) {
-        int mt, nt0, ntn, k0, kn;
-        decode(item, mt, nt0, ntn, k0, kn);
-        const int row0 = (int)warp_uniform((uint32_t)(mt * GT_BM));
-        for (int nt = nt0; nt < nt0 + ntn; ++nt) {
-          const int col0 = (int)warp_uniform((uint32_t)(nt * BN));
-          for (int kit = k0; kit < k0 + kn; ++kit) {
-            const uint32_t sg = warp_uniform((uint32_t)stage);
-            mbar_wait_warp_a(empty_a + 8 * sg, phase ^ 1);
-            const uint32_t st = smem_a + sg * STAGE_BYTES, fb = full_a + 8 * sg;
-            const int kc = (int)warp_uniform((uint32_t)(kit * BK));
-            if (elect_one()) {
-              mbar_arrive_expect_tx_a(fb, STAGE_BYTES);
-              tma_load_2d_a(st, &tm_ahi, fb, kc, row0);
-              tma_load_2d_a(st + A_BYTES, &tm_alo, fb, kc, row0);
-              if (MC) {   // this CTA's half of the B tile, delivered to both CTAs of the pair
-                constexpr int HB = B_BYTES / 2;
-                tma_load_2d_mc_a(st + 2 * A_BYTES + rank_u * HB, &tm_bhi, fb, kc, col0 + rank_u * (BN / 2), 0x3);
-                tma_load_2d_mc_a(st + 2 * A_BYTES + B_BYTES + rank_u * HB, &tm_blo, fb, kc, col0 + rank_u * (BN / 2), 0x3);
-              } else {
-                tma_load_2d_a(st + 2 * A_BYTES, &tm_bhi, fb, kc, col0);
-                tma_load_2d_a(st + 2 * A_BYTES + B_BYTES, &tm_blo, fb, kc, col0);
-              }
+  if (warp == 4) {
+    // TMA producer: convergent warp, one elected lane issues, warp-uniform operands
+    const uint32_t smem_a = warp_uniform(smem_u32(smem));
+    const uint32_t bars_a = smem_a + STAGES * STAGE_BYTES + ACC_STG_BYTES;
+    const uint32_t full_a = bars_a, empty_a = bars_a + 8 * STAGES;
+    const int rank_u = (int)warp_uniform(cta_rank);
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int item = unit0; item < g.total_items; item += unit_stride) {
+      int mt, nt0, ntn, k0, kn;
+      decode(item, mt, nt0, ntn, k0, kn);
+      const int row0 = (int)warp_uniform((uint32_t)(mt * GT_BM));
+      for (int nt = nt0; nt < nt0 + ntn; ++nt) {
+        const int col0 = (int)warp_uniform((uint32_t)(nt * BN));
+        for (int kit = k0; kit < k0 + kn; ++kit) {
+          const uint32_t sg = warp_uniform((uint32_t)stage);
+          mbar_wait_warp_a(empty_a + 8 * sg, phase ^ 1);
+          const uint32_t st = smem_a + sg * STAGE_BYTES, fb = full_a + 8 * sg;
+          const int kc = (int)warp_uniform((uint32_t)(kit * GT_BK));
+          if (elect_one()) {
+            mbar_arrive_expect_tx_a(fb, STAGE_BYTES);
+            tma_load_2d_a(st, &tm_ahi, fb, kc, row0);
+            tma_load_2d_a(st + A_BYTES, &tm_alo, fb, kc, row0);
+            if (MC) {   // this CTA's half of the B tile, delivered to both CTAs of the pair
+              constexpr int HB = B_BYTES / 2;
+              tma_load_2d_mc_a(st + 2 * A_BYTES + rank_u * HB, &tm_bhi, fb, kc, col0 + rank_u * (BN / 2), 0x3);
+              tma_load_2d_mc_a(st + 2 * A_BYTES + B_BYTES + rank_u * HB, &tm_blo, fb, kc, col0 + rank_u * (BN / 2), 0x3);
+            } else {
+              tma_load_2d_a(st + 2 * A_BYTES, &tm_bhi, fb, kc, col0);
+              tma_load_2d_a(st + 2 * A_BYTES + B_BYTES, &tm_blo, fb, kc, col0);
             }
-            __syncwarp();
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
           }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // MMA issuer: convergent warp, one elected lane issues, ring position and bases warp-uniform (tc_conv.cu explains why)
-    {
-      constexpr uint32_t idesc = umma_idesc_bf16_f32(GT_BM, BN);
-      const uint32_t tmem_u = warp_uniform(tmem_base);
-      const uint32_t smem_a = warp_uniform(smem_u32(smem));
-      const uint32_t bars_a = smem_a + STAGES * STAGE_BYTES;
-      const uint32_t full_a = bars_a, empty_a = bars_a + 8 * STAGES;
-      const uint32_t tfull_a = bars_a + 16 * STAGES, tempty_a = tfull_a + 16;
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int item = unit0; item < g.total_items; item += unit_stride) {
-        int mt, nt0, ntn, k0, kn;
-        decode(item, mt, nt0, ntn, k0, kn);
-        for (int nt = nt0; nt < nt0 + ntn; ++nt, ++it) {
-          const uint32_t as = warp_uniform((uint32_t)(it & 1));
-          const uint32_t aphase = (it >> 1) & 1;
-          mbar_wait_warp_a(tempty_a + 8 * as, aphase ^ 1);
-          tc_fence_after();
-          const uint32_t d_tmem = tmem_u + as * BN;
-          for (int kit = 0; kit < kn; ++kit) {
-            const uint32_t sg = warp_uniform((uint32_t)stage);
-            mbar_wait_warp_a(full_a + 8 * sg, phase);
-            tc_fence_after();
-            const uint32_t sa = smem_a + sg * STAGE_BYTES;
-            if (elect_one()) {
-              const uint64_t a_hi = umma_desc_kmajor<BK>(sa);
-              const uint64_t a_lo = umma_desc_kmajor<BK>(sa + A_BYTES);
-              const uint64_t b_hi = umma_desc_kmajor<BK>(sa + 2 * A_BYTES);
-              const uint64_t b_lo = umma_desc_kmajor<BK>(sa + 2 * A_BYTES + B_BYTES);
-#pragma unroll
-              for (int k = 0; k < BK / 16; ++k) {
-                const uint64_t ko = (uint64_t)(k * 2);
-                umma_bf16(d_tmem, a_lo + ko, b_hi + ko, idesc, (kit > 0 || k > 0) ? 1u : 0u);
-                umma_bf16(d_tmem, a_hi + ko, b_lo + ko, idesc, 1u);
-                umma_bf16(d_tmem, a_hi + ko, b_hi + ko, idesc, 1u);
-              }
-              if (MC) umma_commit_mc_a(empty_a + 8 * sg, 0x3);   // frees the slot in both CTAs of the pair
-              else umma_commit_a(empty_a + 8 * sg);
-              if (kit == kn - 1) umma_commit_a(tfull_a + 8 * as);   // same elected thread as the MMAs it covers
-            }
-            __syncwarp();
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
-          }
+          __syncwarp();
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
     }
   } else {
-    const int q = warp & 3;
-    const int rloc = q * 32 + lane;
-    int it = 0;
+    // consumer warpgroup: wgmma main loop (one group in flight while the next stage is issued), then the epilogue on
+    // row-per-thread views of the accumulator (thread = row of the 128-row tile)
+    const int rloc = threadIdx.x;
+    const uint32_t smem_a = smem_u32(smem);
+    auto release = [&](int st) {          // this warp is done reading stage st (in both CTAs' rings with MC)
+      if (lane == 0) {
+        mbar_arrive(&empty_bar[st]);
+        if (MC) mbar_arrive_remote(mapa_u32(smem_u32(&empty_bar[st]), cta_rank ^ 1u));
+      }
+    };
+    int stage = 0;
+    uint32_t phase = 0;
     for (int item = unit0; item < g.total_items; item += unit_stride) {
       int mt, nt0, ntn, k0, kn;
       decode(item, mt, nt0, ntn, k0, kn);
@@ -220,17 +161,37 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tm_ahi, const __grid_constant
 #pragma unroll
         for (int j = 0; j < 16; ++j) { td[j] = INFINITY; ti[j] = -1; }
       }
-      for (int nt = nt0; nt < nt0 + ntn; ++nt, ++it) {
-        const int as = it & 1;
-        const uint32_t aphase = (it >> 1) & 1;
-        mbar_wait(&tfull_bar[as], aphase);
-        tc_fence_after();
-        const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16) + as * BN;
-#pragma unroll 1
-        for (int ch = 0; ch < BN / 32; ++ch) {
+      for (int nt = nt0; nt < nt0 + ntn; ++nt) {
+        Acc128<BN> acc;
+        int prev = -1;
+        for (int kit = 0; kit < kn; ++kit) {
+          mbar_wait(&full_bar[stage], phase);
+          const uint32_t sa = smem_a + stage * STAGE_BYTES;
+          const uint64_t a_hi = gmma_desc_kmajor_sw128(sa), a_lo = gmma_desc_kmajor_sw128(sa + A_BYTES);
+          const uint64_t b_hi = gmma_desc_kmajor_sw128(sa + 2 * A_BYTES);
+          const uint64_t b_lo = gmma_desc_kmajor_sw128(sa + 2 * A_BYTES + B_BYTES);
+          constexpr uint64_t kHalf = (GT_BM / 2) * 128 / 16;   // rows 64-127 of A: +8 KiB
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < GT_BK / 16; ++k) {
+            const uint64_t ko = (uint64_t)(k * 2);
+            acc.mma(a_lo + ko, a_lo + kHalf + ko, b_hi + ko, (kit > 0 || k > 0) ? 1u : 0u);
+            acc.mma(a_hi + ko, a_hi + kHalf + ko, b_lo + ko, 1u);
+            acc.mma(a_hi + ko, a_hi + kHalf + ko, b_hi + ko, 1u);
+          }
+          wgmma_commit();
+          wgmma_wait<1>();
+          if (prev >= 0) release(prev);
+          prev = stage;
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+        wgmma_wait<0>();
+        acc.fence_operands();
+        if (prev >= 0) release(prev);
+#pragma unroll
+        for (int ch = 0; ch < BN / 32; ++ch) {     // unrolled: the accumulator is indexed with constants only
           uint32_t raw[32];
-          tmem_ld_32x32(t_row + ch * 32, raw);
-          tmem_ld_wait();
+          acc.rows32(ch, stg, raw);
           const int col0 = nt * BN + ch * 32;
           if (EPI == EPI_PARTIAL) {
             const int split = item % g.items_per_mtile;
@@ -263,7 +224,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tm_ahi, const __grid_constant
             }
           } else {  // EPI_TOP16
             // one coalesced load of the chunk's |d|^2 terms + shuffles, chain-free sorted insert (see tc_dist1.cu)
-            const float bmine = (col0 + (int)(threadIdx.x & 31) < g.n_valid) ? __ldg(g.bn + col0 + (threadIdx.x & 31)) : INFINITY;
+            const float bmine = (col0 + lane < g.n_valid) ? __ldg(g.bn + col0 + lane) : INFINITY;
 #pragma unroll
             for (int j = 0; j < 32; ++j) {
               const int col = col0 + j;
@@ -283,9 +244,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tm_ahi, const __grid_constant
             }
           }
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tempty_bar[as]);
       }
       if (EPI == EPI_TOP16 && row_ok) {
         const int sub = item % g.items_per_mtile;
@@ -296,31 +254,25 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tm_ahi, const __grid_constant
       }
     }
   }
-
-  tc_fence_before();
   __syncthreads();
   if (MC) cluster_sync_all();     // no CTA leaves while its peer may still multicast into it or arrive on its barriers
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
-  }
 }
 
 // ---- host ------------------------------------------------------------------------------------
 static int sm_count() { return device_sm_count(); }   // per device: one process may drive several GPUs
 
-template <int BN, int STAGES, int EPI, bool MC = false, int BK = 64>
+template <int BN, int STAGES, int EPI, bool MC = false>
 static int launch_gemm_variant(const CUtensorMap* maps, const GemmTcArgs& g, cudaStream_t s) {
-  constexpr int smem = STAGES * (2 * GT_BM * BK * 2 + 2 * BN * BK * 2) + 1024 + 256;
+  constexpr int smem = STAGES * (2 * GT_BM * GT_BK * 2 + 2 * BN * GT_BK * 2) + ACC_STG_BYTES + 1024 + 256;
+  static_assert(smem <= 232448, "shared-memory budget");
   static DeviceOnce attr_done;   // the attribute is per device
   if (!attr_done.done()) {
-    IBL_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<BN, STAGES, EPI, MC, BK>,
-                                     cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    IBL_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<BN, STAGES, EPI, MC>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     attr_done.mark();
   }
   if (!MC) {
     const int grid = g.total_items < sm_count() ? g.total_items : sm_count();
-    gemm_tc_kernel<BN, STAGES, EPI, false, BK><<<grid, 192, smem, s>>>(maps[0], maps[1], maps[2], maps[3], g);
+    gemm_tc_kernel<BN, STAGES, EPI, false><<<grid, 160, smem, s>>>(maps[0], maps[1], maps[2], maps[3], g);
     IBL_CUDA_OK(cudaGetLastError());
     return IBL_OK;
   }
@@ -329,7 +281,7 @@ static int launch_gemm_variant(const CUtensorMap* maps, const GemmTcArgs& g, cud
   const int units = g.total_items < pairs ? g.total_items : pairs;
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(2 * units);
-  cfg.blockDim = dim3(192);
+  cfg.blockDim = dim3(160);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = s;
   cudaLaunchAttribute attr[1];
@@ -339,20 +291,19 @@ static int launch_gemm_variant(const CUtensorMap* maps, const GemmTcArgs& g, cud
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  IBL_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BN, STAGES, EPI, true, BK>, maps[0], maps[1], maps[2], maps[3], g));
+  IBL_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BN, STAGES, EPI, true>, maps[0], maps[1], maps[2], maps[3], g));
   return IBL_OK;
 }
 
 static int make_plane_maps(CUtensorMap* maps, const __nv_bfloat16* a_hi, const __nv_bfloat16* a_lo, int M,
-                           const __nv_bfloat16* b_hi, const __nv_bfloat16* b_lo, int N, int K, int bn, int bk = 64) {
+                           const __nv_bfloat16* b_hi, const __nv_bfloat16* b_lo, int N, int K, int bn) {
   uint64_t dims_a[2] = {(uint64_t)K, (uint64_t)M}, dims_b[2] = {(uint64_t)K, (uint64_t)N};
   uint64_t str[1] = {(uint64_t)K * 2};
-  uint32_t box_a[2] = {(uint32_t)bk, 128}, box_b[2] = {(uint32_t)bk, (uint32_t)bn};
-  const int sw = bk == 64 ? 128 : 64;
-  IBL_RET(make_tmap(&maps[0], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, a_hi, dims_a, str, box_a, sw));
-  IBL_RET(make_tmap(&maps[1], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, a_lo, dims_a, str, box_a, sw));
-  IBL_RET(make_tmap(&maps[2], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, b_hi, dims_b, str, box_b, sw));
-  IBL_RET(make_tmap(&maps[3], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, b_lo, dims_b, str, box_b, sw));
+  uint32_t box_a[2] = {(uint32_t)GT_BK, 128}, box_b[2] = {(uint32_t)GT_BK, (uint32_t)bn};
+  IBL_RET(make_tmap(&maps[0], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, a_hi, dims_a, str, box_a));
+  IBL_RET(make_tmap(&maps[1], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, a_lo, dims_a, str, box_a));
+  IBL_RET(make_tmap(&maps[2], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, b_hi, dims_b, str, box_b));
+  IBL_RET(make_tmap(&maps[3], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, b_lo, dims_b, str, box_b));
   return IBL_OK;
 }
 
@@ -375,71 +326,58 @@ static int pick_runs(int m_tiles, int n_tiles, int min_tiles_per_run, int units 
 }
 
 // Distance + running top-16 per (query, column run): cand_* [runs][M][16]; returns runs.
-// Tile shape of the distance kernel (measured on 6.8k x 10k x 4096, whole retrieval call, same process):
-//   BN=128, BK=64 (128B swizzle), 3 stages                      1.945 ms
-//   BN=128, BK=64, 3 stages, CTA pairs + TMA multicast of B     1.890 ms   (IBL_DIST_BN=128 IBL_GEMM_MC=1)
-//   BN=256, BK=32 (64B swizzle), 4 stages                       1.846 ms   (default)
-// A 256-column tile needs 96 instead of 128 B/clk of shared-memory operand reads per MMA, and the half-size
-// K chunk keeps a 4-deep pipeline inside 192 KiB.  All three land near 1.3 ms for the GEMM itself
-// (~1285 TF/s of issued bf16 MMA, ~0.89 of the power-capped cuBLAS rate).
-// clusters of two CTAs with TMA multicast of the database tile (only with BN=128; IBL_GEMM_MC=0 disables)
-static bool gemm_mc() {
-  static int mc = -1;
-  if (mc < 0) { const char* v = getenv("IBL_GEMM_MC"); mc = (v && atoi(v) == 0) ? 0 : 1; }
-  return mc != 0;
-}
+// 128 x 128 tiles: the accumulator of one tile is 128 registers per consumer thread.
+constexpr int DIST_BN = 128;
 
-static int dist_bn() {
-  static int bn = 0;
-  if (!bn) { const char* v = getenv("IBL_DIST_BN"); bn = (v && atoi(v) == 128) ? 128 : 256; }
-  return bn;
+// SM pairs (clusters of two CTAs sharing each database tile by TMA multicast) for the distance GEMMs.
+// IBL_GEMM_MC=1 forces them, =0 forbids them; unset, the dense GEMM uses them and the top-16 GEMM follows the caller
+// (`pairs`, IBL_DIST_2SM in the engine).  A single row tile always runs on one SM.
+static bool gemm_pairs(int m_tiles, bool pairs) {
+  static const int env = [] { const char* v = getenv("IBL_GEMM_MC"); return v ? (atoi(v) != 0 ? 1 : 0) : -1; }();
+  return m_tiles >= 2 && (env == 1 || (env == -1 && pairs));
 }
 
 int launch_dist_top16_tc(const __nv_bfloat16* q_hi, const __nv_bfloat16* q_lo, const float* qn, int m,
                          const __nv_bfloat16* d_hi, const __nv_bfloat16* d_lo, const float* dn, int n,
                          int n_valid, int K, float* cand_d, long long* cand_i, int max_runs, int* runs_out,
-                         cudaStream_t s) {
-  IBL_REQUIRE(K % 64 == 0, "tcgen05 distance needs dim % 64 == 0");
-  const int BN = dist_bn();
+                         bool pairs, cudaStream_t s) {
+  IBL_REQUIRE(K % 64 == 0, "tensor-core distance needs dim % 64 == 0");
   const int m_tiles = cdiv(m, GT_BM);
-  const bool mc = gemm_mc() && BN == 128 && m_tiles >= 2;
-  const int bk = BN == 256 ? 32 : 64;
+  const bool mc = gemm_pairs(m_tiles, pairs);
   CUtensorMap maps[4];
-  IBL_RET(make_plane_maps(maps, q_hi, q_lo, m, d_hi, d_lo, n, K, mc ? BN / 2 : BN, bk));
+  IBL_RET(make_plane_maps(maps, q_hi, q_lo, m, d_hi, d_lo, n, K, mc ? DIST_BN / 2 : DIST_BN));
   GemmTcArgs g{};
   g.M = m; g.N = n; g.K = K;
-  g.n_tiles = cdiv(n_valid > 0 ? n_valid : 1, BN);
+  g.n_tiles = cdiv(n_valid > 0 ? n_valid : 1, DIST_BN);
   const int m_units = mc ? cdiv(m_tiles, 2) : m_tiles;
-  int runs = pick_runs(m_units, g.n_tiles, BN == 256 ? 1 : 2, mc ? sm_count() / 2 : 0);
+  int runs = pick_runs(m_units, g.n_tiles, 2, mc ? sm_count() / 2 : 0);
   if (runs > max_runs) runs = max_runs;
   g.nt_per_item = cdiv(g.n_tiles, runs);
   g.items_per_mtile = cdiv(g.n_tiles, g.nt_per_item);
-  g.kit_per_item = K / bk;
+  g.kit_per_item = K / GT_BK;
   g.total_items = m_units * g.items_per_mtile;
   g.n_valid = n_valid;
   g.an = qn; g.bn = dn;
   g.cand_d = cand_d; g.cand_i = cand_i;
   *runs_out = g.items_per_mtile;
-  if (mc) return launch_gemm_variant<128, 3, EPI_TOP16, true>(maps, g, s);
-  if (BN == 256) return launch_gemm_variant<256, 4, EPI_TOP16, false, 32>(maps, g, s);
-  return launch_gemm_variant<128, 3, EPI_TOP16>(maps, g, s);
+  if (mc) return launch_gemm_variant<DIST_BN, 3, EPI_TOP16, true>(maps, g, s);
+  return launch_gemm_variant<DIST_BN, 3, EPI_TOP16>(maps, g, s);
 }
 
-int dist_top16_max_runs(int m, int n_valid) {
-  const int BN = dist_bn();
+int dist_top16_max_runs(int m, int n_valid, bool pairs) {
   const int m_tiles = cdiv(m, GT_BM);
-  const bool mc = gemm_mc() && BN == 128 && m_tiles >= 2;
-  return pick_runs(mc ? cdiv(m_tiles, 2) : m_tiles, cdiv(n_valid > 0 ? n_valid : 1, BN), BN == 256 ? 1 : 2,
+  const bool mc = gemm_pairs(m_tiles, pairs);
+  return pick_runs(mc ? cdiv(m_tiles, 2) : m_tiles, cdiv(n_valid > 0 ? n_valid : 1, DIST_BN), 2,
                    mc ? sm_count() / 2 : 0);
 }
 
 int launch_dist_dense_tc(const __nv_bfloat16* q_hi, const __nv_bfloat16* q_lo, const float* qn, int m,
                          const __nv_bfloat16* d_hi, const __nv_bfloat16* d_lo, const float* dn, int n, int K,
                          float* out, long long ld_out, cudaStream_t s) {
-  IBL_REQUIRE(K % 64 == 0, "tcgen05 distance needs dim % 64 == 0");
+  IBL_REQUIRE(K % 64 == 0, "tensor-core distance needs dim % 64 == 0");
   constexpr int BN = 128;
   const int m_tiles = cdiv(m, GT_BM);
-  const bool mc = gemm_mc() && m_tiles >= 2;
+  const bool mc = gemm_pairs(m_tiles, true);
   CUtensorMap maps[4];
   IBL_RET(make_plane_maps(maps, q_hi, q_lo, m, d_hi, d_lo, n, K, mc ? BN / 2 : BN));
   GemmTcArgs g{};
@@ -449,7 +387,7 @@ int launch_dist_dense_tc(const __nv_bfloat16* q_hi, const __nv_bfloat16* q_lo, c
   const int runs = pick_runs(m_units, g.n_tiles, 1, mc ? sm_count() / 2 : 0);
   g.nt_per_item = cdiv(g.n_tiles, runs);
   g.items_per_mtile = cdiv(g.n_tiles, g.nt_per_item);
-  g.kit_per_item = K / 64;
+  g.kit_per_item = K / GT_BK;
   g.total_items = m_units * g.items_per_mtile;
   g.n_valid = n;
   g.an = qn; g.bn = dn;
@@ -462,8 +400,8 @@ int launch_dist_dense_tc(const __nv_bfloat16* q_hi, const __nv_bfloat16* q_lo, c
 int launch_pca_partial_tc(const __nv_bfloat16* w_hi, const __nv_bfloat16* w_lo, int P,
                           const __nv_bfloat16* v_hi, const __nv_bfloat16* v_lo, int N, int D,
                           float* partial, int* splits_out, cudaStream_t s) {
-  IBL_REQUIRE(D % 64 == 0, "tcgen05 PCA needs D % 64 == 0");
-  IBL_REQUIRE(N >= 1 && N <= 32, "tcgen05 PCA handles up to 32 rows per call");
+  IBL_REQUIRE(D % 64 == 0, "tensor-core PCA needs D % 64 == 0");
+  IBL_REQUIRE(N >= 1 && N <= 32, "tensor-core PCA handles up to 32 rows per call");
   constexpr int BN = 32;
   CUtensorMap maps[4];
   IBL_RET(make_plane_maps(maps, w_hi, w_lo, P, v_hi, v_lo, N, D, BN));

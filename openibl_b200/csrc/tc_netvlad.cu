@@ -1,8 +1,9 @@
-// tcgen05 building block for the fused NetVLAD kernel: a "TN" product  C[m,n] = sum_k A[k,m] B[k,n]
-// whose operands are MN-major in shared memory (the reduction index is the row index), i.e. the layout
-// a TMA box [rows = k][64 contiguous elements] produces.  This is what the second NetVLAD contraction
-// needs: vlad[c,k] = sum_s x^[s,c] a[s,k] reads the same [pixel][channel] tile the first contraction
-// (logits = x^ W^T, K-major) already staged, so the feature map is read from HBM once.
+// Fused NetVLAD on the Hopper tensor cores (wgmma), plus a micro-test of its "TN" building block:
+// C[m,n] = sum_k A[k,m] B[k,n] with operands MN-major in shared memory (the reduction index is the
+// row index), i.e. the layout a TMA box [rows = k][64 contiguous elements] produces.  This is what the
+// second NetVLAD contraction needs: vlad[c,k] = sum_s x^[s,c] a[s,k] reads the same [pixel][channel]
+// tile the first contraction (logits = x^ W^T, K-major) already staged, so the feature map is read
+// from HBM once.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -11,22 +12,6 @@
 namespace ibl {
 
 using namespace tc;
-
-// MN-major operand, 128-byte swizzle: rows (K index) of 64 bf16 = 128 B, 8-row atoms 1024 B apart
-// (SBO); further 64-element blocks along M/N are `lbo_bytes` apart (cute::UMMA canonical layout
-// ((8,n),(8,k)):((1,LBO),(8,SBO)) in 16-byte units).
-__device__ __forceinline__ uint64_t umma_desc_mnmajor_sw128(uint32_t smem_addr, uint32_t lbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3fffu);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3fffu) << 16;
-  d |= (uint64_t)(1024u >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-__host__ __device__ constexpr uint32_t umma_idesc_bf16_f32_mn(int M, int N, int a_mn, int b_mn) {
-  return umma_idesc_bf16_f32(M, N) | ((uint32_t)a_mn << 15) | ((uint32_t)b_mn << 16);
-}
 
 // ---- micro-test: one CTA, M = 128, N = 64, K = 128, bf16x3 -----------------------------------------
 __global__ void __launch_bounds__(128, 1)
@@ -40,23 +25,14 @@ tn_gemm_test_kernel(const __grid_constant__ CUtensorMap tm_ahi, const __grid_con
   uint8_t* a_lo = smem + 32768;
   uint8_t* b_hi = smem + 65536;
   uint8_t* b_lo = smem + 81920;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 98304);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  float* stg = reinterpret_cast<float*>(smem + 98304);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 98304 + ACC_STG_BYTES);
   if (threadIdx.x == 0) {
     mbar_init(&bars[0], 1);
-    mbar_init(&bars[1], 1);
     fence_barrier_init();
     fence_proxy_async();
   }
-  if (warp == 0) {
-    tmem_alloc(tmem_slot, 64);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   if (threadIdx.x == 0) {
     mbar_arrive_expect_tx(&bars[0], 98304);
     tma_load_2d(a_hi, &tm_ahi, &bars[0], 0, 0);
@@ -65,37 +41,32 @@ tn_gemm_test_kernel(const __grid_constant__ CUtensorMap tm_ahi, const __grid_con
     tma_load_2d(a_lo + 16384, &tm_alo, &bars[0], 64, 0);
     tma_load_2d(b_hi, &tm_bhi, &bars[0], 0, 0);
     tma_load_2d(b_lo, &tm_blo, &bars[0], 0, 0);
-    mbar_wait(&bars[0], 0);
-    tc_fence_after();
-    constexpr uint32_t idesc = umma_idesc_bf16_f32_mn(128, 64, 1, 1);
-    for (int ks = 0; ks < 8; ++ks) {   // 16 k-rows (2048 B) per MMA
-      const uint32_t off = ks * 2048;
-      const uint64_t dah = umma_desc_mnmajor_sw128(smem_u32(a_hi) + off, 16384);
-      const uint64_t dal = umma_desc_mnmajor_sw128(smem_u32(a_lo) + off, 16384);
-      const uint64_t dbh = umma_desc_mnmajor_sw128(smem_u32(b_hi) + off, 0);
-      const uint64_t dbl = umma_desc_mnmajor_sw128(smem_u32(b_lo) + off, 0);
-      umma_bf16(tmem_base, dal, dbh, idesc, ks > 0 ? 1u : 0u);
-      umma_bf16(tmem_base, dah, dbl, idesc, 1u);
-      umma_bf16(tmem_base, dah, dbh, idesc, 1u);
-    }
-    umma_commit(&bars[1]);
   }
-  __syncwarp();
-  mbar_wait(&bars[1], 0);
-  tc_fence_after();
-  const int m = warp * 32 + lane;
+  mbar_wait(&bars[0], 0);
+  Acc128<64> acc;
+  wgmma_fence();
+  for (int ks = 0; ks < 8; ++ks) {   // 16 k-rows (2048 B) per MMA
+    const uint32_t off = ks * 2048;
+    const uint64_t dah0 = gmma_desc_mnmajor_sw128(smem_u32(a_hi) + off, 16384);
+    const uint64_t dah1 = gmma_desc_mnmajor_sw128(smem_u32(a_hi) + 16384 + off, 16384);
+    const uint64_t dal0 = gmma_desc_mnmajor_sw128(smem_u32(a_lo) + off, 16384);
+    const uint64_t dal1 = gmma_desc_mnmajor_sw128(smem_u32(a_lo) + 16384 + off, 16384);
+    const uint64_t dbh = gmma_desc_mnmajor_sw128(smem_u32(b_hi) + off, 0);
+    const uint64_t dbl = gmma_desc_mnmajor_sw128(smem_u32(b_lo) + off, 0);
+    acc.mma<false, 1, 1>(dal0, dal1, dbh, ks > 0 ? 1u : 0u);
+    acc.mma<false, 1, 1>(dah0, dah1, dbl, 1u);
+    acc.mma<false, 1, 1>(dah0, dah1, dbh, 1u);
+  }
+  wgmma_commit();
+  wgmma_wait<0>();
+  acc.fence_operands();
+  const int m = threadIdx.x;
+#pragma unroll
   for (int ch = 0; ch < 2; ++ch) {
     uint32_t raw[32];
-    tmem_ld_32x32(tmem_base + ((uint32_t)(warp * 32) << 16) + ch * 32, raw);
-    tmem_ld_wait();
+    acc.rows32(ch, stg, raw);
 #pragma unroll
     for (int j = 0; j < 32; ++j) C[m * 64 + ch * 32 + j] = __uint_as_float(raw[j]);
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 64);
   }
 }
 
@@ -114,7 +85,7 @@ int debug_gemm_tn(const float* A, const float* B, float* C, cudaStream_t s) {
   if (rc == IBL_OK) rc = make_tmap(&maps[2], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, pb, db, sb, box);
   if (rc == IBL_OK) rc = make_tmap(&maps[3], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, pb + 128 * 64, db, sb, box);
   if (rc == IBL_OK) {
-    const int smem = 98304 + 1024 + 64;
+    const int smem = 98304 + ACC_STG_BYTES + 1024 + 64;
     cudaFuncSetAttribute(tn_gemm_test_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     tn_gemm_test_kernel<<<1, 128, smem, s>>>(maps[0], maps[1], maps[2], maps[3], C);
     if (cudaGetLastError() != cudaSuccess) rc = IBL_ERR_CUDA;
@@ -130,25 +101,25 @@ int debug_gemm_tn(const float* A, const float* B, float* C, cudaStream_t s) {
 // Fused NetVLAD (reference ibl/models/netvlad.py:44-61 + the intra-normalisation / L2 of :78-80)
 //
 //   x^[s,:] = x[s,:] / max(|x[s,:]|, eps)                       |x[s,:]|^2 comes from the conv5_3 epilogue
-//   z[s,k]  = W[k,:] . x^[s,:]          GEMM 1 (tcgen05, K-major operands: pixel tile x channel chunk)
-//   a[s,:]  = softmax_k z[s,:]          epilogue warps, one pixel per thread, fp32, max-subtracted
-//   V[c,k]  = sum_s x^[s,c] a[s,k]      GEMM 2 (tcgen05, MN-major operands: the SAME [pixel][channel]
+//   z[s,k]  = W[k,:] . x^[s,:]          GEMM 1 (wgmma, K-major operands: pixel tile x channel chunk)
+//   a[s,:]  = softmax_k z[s,:]          one pixel per thread, fp32, max-subtracted
+//   V[c,k]  = sum_s x^[s,c] a[s,k]      GEMM 2 (wgmma, MN-major operands: the SAME [pixel][channel]
 //                                       tiles, and a' = a/|x| written to shared memory by the softmax)
 //   vlad[k,c] = V[c,k] - cent[k,c] * sum_s a[s,k]
 //
-// One work unit = (image, every G-th 128-pixel tile); a unit keeps V (512 x 64 fp32 = 256 TMEM columns)
-// resident across its tiles and writes one partial.  ONE LAUNCH: the unit that arrives last for an image
+// One work unit = (image, every G-th 128-pixel tile); a unit accumulates V (512 x 64 fp32, too large for the
+// registers of one warpgroup) in its own partial slice in global memory, which stays in L2: every element is
+// read-modified-written by the same thread, tile after tile, in tile order.  ONE LAUNCH: the unit that arrives last for an image
 // (atomic ticket in global memory) adds the G partials in index order (L2 hits), subtracts the centroid term
 // and applies the intra-normalisation and the global L2 (netvlad.py:78-80) before the kernel ends -- there is
 // no finalize kernel.  G depends on S only, never on the batch, so an image's descriptor is bit-identical
 // whatever batch it travels in.  The feature map is read from HBM once (the second pass over a tile's
 // channel chunks hits L2).  Both contractions are bf16x3.
-// The logits are double buffered in TMEM (128 + 128 columns) and GEMM 1 of the next tile is issued before
-// GEMM 2 of the current one, so the softmax runs under tensor-core work (44 -> 35 us at B = 32).
 //
-// Warp roles: warp 0 TMA producer, warp 1 MMA issuer + TMEM owner, warps 2-5 softmax / epilogue.
+// Warp roles: warps 0-3 consumer warpgroup (GEMM 1, softmax, GEMM 2, unit epilogue), warp 4 TMA producer.
 // Shared memory: 3 stages of 64 KiB (GEMM 1 stage: X_hi | X_lo | W_hi,W_lo of one 64-channel chunk;
-// GEMM 2 stage: X_hi c0 | X_hi c1 | X_lo c0 | X_lo c1 of one 128-channel block) + a' hi/lo (32 KiB).
+// GEMM 2 stage: X_hi c0 | X_hi c1 | X_lo c0 | X_lo c1 of one 128-channel block) + a' hi/lo (32 KiB)
+// + the accumulator transposition buffer.
 // =====================================================================================================
 struct NvTcArgs {
   int B, S, G, T;                 // images, pixels per image, units per image, 128-pixel tiles per image
@@ -192,7 +163,7 @@ struct NvIter {
   }
 };
 
-// Finalisation of image b by the four epilogue warps (128 threads) of the unit that arrived last:
+// Finalisation of image b by the consumer warpgroup (128 threads) of the unit that arrived last:
 //   vlad[k,c] = sum_g part[b,g,k,c] - cent[k,c] * sum_g asum[b,g,k]   (partials added in index order: deterministic)
 //   intra-normalise every cluster row (netvlad.py:78), flatten k-major, global L2 (:79-80).
 // Warp q owns rows q*16 .. q*16+15, lane L the channels L, L+32, ...; every thread rescales exactly the elements it
@@ -281,13 +252,7 @@ __device__ __forceinline__ void nv_finalize_image(const NvTcArgs& a, int b, int 
   }
 }
 
-// Software pipeline over the CTA's tile list: GEMM 1 of tile i+1 is issued BEFORE GEMM 2 of tile i, so the
-// tensor core computes the next logits while the epilogue warps run the softmax of tile i (logits are double
-// buffered in TMEM: Z0 | Z1 | V = 128 + 128 + 256 columns).  The TMA producer and the MMA issuer walk the same
-// schedule, so the single shared-memory ring stays in order:  G1(0) G1(1) G2(0) G1(2) G2(1) ... G2(n-1).
-// GEMM 1 uses the concatenated operand [W_hi ; W_lo] (adjacent in the stage): x_hi . [W_hi;W_lo]^T is one
-// N = 128 MMA, x_lo . W_hi^T a second N = 64 one into the first 64 columns -- 2 MMAs per K step instead of 3.
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(160, 1)
 netvlad_tc_kernel(const __grid_constant__ CUtensorMap tm_xhi, const __grid_constant__ CUtensorMap tm_xlo,
                   const __grid_constant__ CUtensorMap tm_whi, const __grid_constant__ CUtensorMap tm_wlo,
                   const NvTcArgs a) {
@@ -295,200 +260,84 @@ netvlad_tc_kernel(const __grid_constant__ CUtensorMap tm_xhi, const __grid_const
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* asm_hi = smem + NV_NSTAGE * NV_STAGE;
   uint8_t* asm_lo = asm_hi + NV_SLOT;
+  // the accumulator transposition of the logits runs while a' is free (GEMM 2 of the previous tile has retired, the
+  // softmax has not written yet): it borrows the a' buffers
+  float* stg = reinterpret_cast<float*>(asm_hi);
+  static_assert(ACC_STG_BYTES <= 2 * NV_SLOT, "transposition buffer inside a' hi | lo");
   uint64_t* bars = reinterpret_cast<uint64_t*>(asm_lo + NV_SLOT);
   uint64_t* full_bar = bars;                 // [3]
-  uint64_t* empty_bar = bars + 3;            // [3]
-  uint64_t* z_full = bars + 6;               // [2] GEMM 1 commit
-  uint64_t* z_empty = bars + 8;              // [2] 4 epilogue warps have read the logits
-  uint64_t* a_full = bars + 10;              // 4 epilogue warps have written a'
-  uint64_t* a_empty = bars + 11;             // GEMM 2 commit: a' may be overwritten
-  uint64_t* d_full = bars + 12;
-  uint64_t* d_empty = bars + 13;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 14);
+  uint64_t* empty_bar = bars + 3;            // [3] one arrival per consumer warp
   float* asum_sm = reinterpret_cast<float*>(bars + 16);   // [4 warps][64]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 0 && lane == 0) {
+  if (warp == 4 && lane == 0) {
     tma_prefetch_desc(&tm_xhi); tma_prefetch_desc(&tm_xlo); tma_prefetch_desc(&tm_whi); tma_prefetch_desc(&tm_wlo);
-    for (int i = 0; i < 3; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&z_full[i], 1); mbar_init(&z_empty[i], 4); }
-    mbar_init(a_full, 4);
-    mbar_init(a_empty, 1);
-    mbar_init(d_full, 1);
-    mbar_init(d_empty, 4);
+    for (int i = 0; i < 3; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 4); }
     fence_barrier_init();
     fence_proxy_async();
   }
-  if (warp == 1) { tmem_alloc(tmem_slot, 512); tmem_relinquish(); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t t_d = tmem_base + 256;
   const int n_units = a.B * a.G;
 
-  if (warp == 0) {
-    // TMA producer: same discipline as the MMA issuer below (convergent warp, one elected lane issues, warp-uniform operands)
-    {
-      const uint32_t smem_a = warp_uniform(smem_u32(smem));
-      const uint32_t bars_a = smem_a + NV_NSTAGE * NV_STAGE + 2 * NV_SLOT;
-      const uint32_t full_a = bars_a, empty_a = bars_a + 24;
-      int stage = 0; uint32_t phase = 0;
-      NvIter c1, c2;
-      c1.init(blockIdx.x, gridDim.x, a.G, a.T, n_units);
-      c2.init(blockIdx.x, gridDim.x, a.G, a.T, n_units);
-      int n1 = 0, n2 = 0;
-      while (c2.valid()) {
-        if (c1.valid()) {                         // GEMM 1 stages: one 64-channel chunk + its W chunk
-          const int b = (int)warp_uniform((uint32_t)(c1.u / a.G)), p0 = (int)warp_uniform((uint32_t)(c1.t * 128));
-          for (int c = 0; c < 8; ++c) {           // (a per-CTA rotated chunk order was tried against the slow first
-                                                  // tile: no gain, and it makes the fp32 summation order depend on
-                                                  // the batch composition)
-            const uint32_t sg = warp_uniform((uint32_t)stage);
-            mbar_wait_warp_a(empty_a + 8 * sg, phase ^ 1);
-            const uint32_t st = smem_a + sg * NV_STAGE, fb = full_a + 8 * sg;
-            if (elect_one()) {
-              mbar_arrive_expect_tx_a(fb, 3 * NV_SLOT);
-              tma_load_3d_a(st, &tm_xhi, fb, c * 64, p0, b);
-              tma_load_3d_a(st + NV_SLOT, &tm_xlo, fb, c * 64, p0, b);
-              tma_load_2d_a(st + 2 * NV_SLOT, &tm_whi, fb, c * 64, 0);
-              tma_load_2d_a(st + 2 * NV_SLOT + 8192, &tm_wlo, fb, c * 64, 0);
-            }
-            __syncwarp();
-            if (++stage == NV_NSTAGE) { stage = 0; phase ^= 1; }
-          }
-          c1.next();
-          ++n1;
-          if (c1.valid()) {                       // rolling L2 prefetch: the NEXT tile's boxes, behind this tile's
-            const int bn = (int)warp_uniform((uint32_t)(c1.u / a.G));   // loads (prefetching the whole unit up front
-            const int pn = (int)warp_uniform((uint32_t)(c1.t * 128));   // delayed the first logits of every CTA to 10 us)
-            if (elect_one()) {
-              for (int c2i = 0; c2i < 8; ++c2i) {
-                tma_prefetch_3d(&tm_xhi, c2i * 64, pn, bn);
-                tma_prefetch_3d(&tm_xlo, c2i * 64, pn, bn);
-              }
-            }
-            __syncwarp();
-          }
+  if (warp == 4) {
+    // TMA producer: convergent warp, one elected lane issues, warp-uniform operands.  Per tile: the 8 GEMM 1 stages,
+    // then the 4 GEMM 2 stages (L2 hits), in the order the consumer walks them.
+    const uint32_t smem_a = warp_uniform(smem_u32(smem));
+    const uint32_t bars_a = smem_a + NV_NSTAGE * NV_STAGE + 2 * NV_SLOT;
+    const uint32_t full_a = bars_a, empty_a = bars_a + 24;
+    int stage = 0; uint32_t phase = 0;
+    NvIter c1;
+    c1.init(blockIdx.x, gridDim.x, a.G, a.T, n_units);
+    while (c1.valid()) {
+      const int b = (int)warp_uniform((uint32_t)(c1.u / a.G)), p0 = (int)warp_uniform((uint32_t)(c1.t * 128));
+      for (int c = 0; c < 8; ++c) {           // GEMM 1 stages: one 64-channel chunk + its W chunk
+        const uint32_t sg = warp_uniform((uint32_t)stage);
+        mbar_wait_warp_a(empty_a + 8 * sg, phase ^ 1);
+        const uint32_t st = smem_a + sg * NV_STAGE, fb = full_a + 8 * sg;
+        if (elect_one()) {
+          mbar_arrive_expect_tx_a(fb, 3 * NV_SLOT);
+          tma_load_3d_a(st, &tm_xhi, fb, c * 64, p0, b);
+          tma_load_3d_a(st + NV_SLOT, &tm_xlo, fb, c * 64, p0, b);
+          tma_load_2d_a(st + 2 * NV_SLOT, &tm_whi, fb, c * 64, 0);
+          tma_load_2d_a(st + 2 * NV_SLOT + 8192, &tm_wlo, fb, c * 64, 0);
         }
-        if (n2 < n1 - 1 || !c1.valid()) {         // GEMM 2 stages: one 128-channel block (L2 hits)
-          const int b = (int)warp_uniform((uint32_t)(c2.u / a.G)), p0 = (int)warp_uniform((uint32_t)(c2.t * 128));
-          for (int cb = 0; cb < 4; ++cb) {
-            const uint32_t sg = warp_uniform((uint32_t)stage);
-            mbar_wait_warp_a(empty_a + 8 * sg, phase ^ 1);
-            const uint32_t st = smem_a + sg * NV_STAGE, fb = full_a + 8 * sg;
-            if (elect_one()) {
-              mbar_arrive_expect_tx_a(fb, 4 * NV_SLOT);
-              tma_load_3d_a(st, &tm_xhi, fb, cb * 128, p0, b);
-              tma_load_3d_a(st + NV_SLOT, &tm_xhi, fb, cb * 128 + 64, p0, b);
-              tma_load_3d_a(st + 2 * NV_SLOT, &tm_xlo, fb, cb * 128, p0, b);
-              tma_load_3d_a(st + 3 * NV_SLOT, &tm_xlo, fb, cb * 128 + 64, p0, b);
-            }
-            __syncwarp();
-            if (++stage == NV_NSTAGE) { stage = 0; phase ^= 1; }
-          }
-          c2.next();
-          ++n2;
-        }
+        __syncwarp();
+        if (++stage == NV_NSTAGE) { stage = 0; phase ^= 1; }
       }
-    }
-  } else if (warp == 1) {
-    // MMA issuer: the whole warp walks the schedule in convergent code, ONE ELECTED lane issues; ring position and bases pass
-    // through warp_uniform() so that every tcgen05 operand lives in a uniform register.  Inside an `if (lane == 0)`
-    // region each of the 160 small MMAs of a tile (N = 64 / 128: 32-65 clk of tensor pipe) was wrapped in an ELECT +
-    // R2UR.BROADCAST loop of ~90-100 clk -- a good part of round 1's "3.5 us + 4.7 us per tile" was ISSUE time, not
-    // shared-memory bandwidth (66.6 -> 62.2 us for the kernel with elected-lane issue).
-    {
-      constexpr uint32_t idesc_n128 = umma_idesc_bf16_f32(128, 128);
-      constexpr uint32_t idesc_n64 = umma_idesc_bf16_f32(128, 64);
-      constexpr uint32_t idesc2 = umma_idesc_bf16_f32_mn(128, 64, 1, 1);
-      const uint32_t tmem_u = warp_uniform(tmem_base);
-      const uint32_t smem_a = warp_uniform(smem_u32(smem));
-      const uint32_t ah = smem_a + NV_NSTAGE * NV_STAGE, al = ah + NV_SLOT;
-      const uint32_t bars_a = al + NV_SLOT;
-      const uint32_t full_a = bars_a, empty_a = bars_a + 24, zfull_a = bars_a + 48, zempty_a = bars_a + 64;
-      const uint32_t afull_a = bars_a + 80, aempty_a = bars_a + 88, dfull_a = bars_a + 96, dempty_a = bars_a + 104;
-      const uint32_t t_du = tmem_u + 256;
-      int stage = 0; uint32_t phase = 0;
-      NvIter c1, c2;
-      c1.init(blockIdx.x, gridDim.x, a.G, a.T, n_units);
-      c2.init(blockIdx.x, gridDim.x, a.G, a.T, n_units);
-      int n1 = 0, n2 = 0;
-      while (c2.valid()) {
-        if (c1.valid()) {
-          // ---- GEMM 1 of tile n1: Z[128 px, (x.W_hi) | (x_hi.W_lo)] ----
-          const uint32_t zb = warp_uniform((uint32_t)(n1 & 1));
-          mbar_wait_warp_a(zempty_a + 8 * zb, ((n1 >> 1) & 1) ^ 1);
-          tc_fence_after();
-          const uint32_t t_z = tmem_u + zb * 128;
-          for (int c = 0; c < 8; ++c) {
-            const uint32_t st = warp_uniform((uint32_t)stage);
-            mbar_wait_warp_a(full_a + 8 * st, phase);
-            tc_fence_after();
-            const uint32_t sa = smem_a + st * NV_STAGE;
-            if (elect_one()) {
-              const uint64_t xh = umma_desc_kmajor_sw128(sa), xl = umma_desc_kmajor_sw128(sa + NV_SLOT);
-              const uint64_t wcat = umma_desc_kmajor_sw128(sa + 2 * NV_SLOT);   // 128 rows: W_hi then W_lo
-#pragma unroll
-              for (int k = 0; k < 4; ++k) {
-                const uint64_t ko = (uint64_t)(k * 2);
-                umma_bf16(t_z, xh + ko, wcat + ko, idesc_n128, (c > 0 || k > 0) ? 1u : 0u);
-                umma_bf16(t_z, xl + ko, wcat + ko, idesc_n64, 1u);               // x_lo . W_hi into columns 0-63
-              }
-              umma_commit_a(empty_a + 8 * st);
-              if (c == 7) umma_commit_a(zfull_a + 8 * zb);   // same elected thread as the MMAs it covers
-            }
-            __syncwarp();
-            if (++stage == NV_NSTAGE) { stage = 0; phase ^= 1; }
-          }
-          c1.next();
-          ++n1;
+      for (int cb = 0; cb < 4; ++cb) {        // GEMM 2 stages: one 128-channel block
+        const uint32_t sg = warp_uniform((uint32_t)stage);
+        mbar_wait_warp_a(empty_a + 8 * sg, phase ^ 1);
+        const uint32_t st = smem_a + sg * NV_STAGE, fb = full_a + 8 * sg;
+        if (elect_one()) {
+          mbar_arrive_expect_tx_a(fb, 4 * NV_SLOT);
+          tma_load_3d_a(st, &tm_xhi, fb, cb * 128, p0, b);
+          tma_load_3d_a(st + NV_SLOT, &tm_xhi, fb, cb * 128 + 64, p0, b);
+          tma_load_3d_a(st + 2 * NV_SLOT, &tm_xlo, fb, cb * 128, p0, b);
+          tma_load_3d_a(st + 3 * NV_SLOT, &tm_xlo, fb, cb * 128 + 64, p0, b);
         }
-        if (n2 < n1 - 1 || !c1.valid()) {
-          // ---- GEMM 2 of tile n2: V[128 c, 64 k] (4 channel blocks) += X^T a' ----
-          const bool fresh = c2.first(), unit_done = c2.last();
-          if (fresh) {
-            mbar_wait_warp_a(dempty_a, (c2.useq & 1) ^ 1);   // the previous unit's partial has been read out of TMEM
-            tc_fence_after();
+        __syncwarp();
+        if (++stage == NV_NSTAGE) { stage = 0; phase ^= 1; }
+      }
+      c1.next();
+      if (c1.valid()) {                       // rolling L2 prefetch: the NEXT tile's boxes, behind this tile's loads
+        const int bn = (int)warp_uniform((uint32_t)(c1.u / a.G));
+        const int pn = (int)warp_uniform((uint32_t)(c1.t * 128));
+        if (elect_one()) {
+          for (int c2i = 0; c2i < 8; ++c2i) {
+            tma_prefetch_3d(&tm_xhi, c2i * 64, pn, bn);
+            tma_prefetch_3d(&tm_xlo, c2i * 64, pn, bn);
           }
-          mbar_wait_warp_a(afull_a, n2 & 1);
-          tc_fence_after();
-          for (int cb = 0; cb < 4; ++cb) {
-            const uint32_t st = warp_uniform((uint32_t)stage);
-            mbar_wait_warp_a(full_a + 8 * st, phase);
-            tc_fence_after();
-            const uint32_t sa = smem_a + st * NV_STAGE;
-            const uint32_t d = t_du + warp_uniform((uint32_t)cb) * 64;
-            if (elect_one()) {
-#pragma unroll
-              for (int ks = 0; ks < 8; ++ks) {     // 16 pixel rows (2048 B) per MMA
-                const uint32_t off = ks * 2048;
-                const uint64_t xh = umma_desc_mnmajor_sw128(sa + off, NV_SLOT);
-                const uint64_t xl = umma_desc_mnmajor_sw128(sa + 2 * NV_SLOT + off, NV_SLOT);
-                const uint64_t bh = umma_desc_mnmajor_sw128(ah + off, 0);
-                const uint64_t bl = umma_desc_mnmajor_sw128(al + off, 0);
-                umma_bf16(d, xl, bh, idesc2, (fresh && ks == 0) ? 0u : 1u);
-                umma_bf16(d, xh, bl, idesc2, 1u);
-                umma_bf16(d, xh, bh, idesc2, 1u);
-              }
-              umma_commit_a(empty_a + 8 * st);
-              if (cb == 3) {
-                umma_commit_a(aempty_a);             // a' may be overwritten
-                if (unit_done) umma_commit_a(dfull_a);
-              }
-            }
-            __syncwarp();
-            if (++stage == NV_NSTAGE) { stage = 0; phase ^= 1; }
-          }
-          c2.next();
-          ++n2;
         }
+        __syncwarp();
       }
     }
   } else {
-    const int q = warp & 3;
-    const int s_loc = q * 32 + lane;             // pixel row inside the tile == TMEM lane
-    const uint32_t lane_base = (uint32_t)(q * 32) << 16;
+    const int q = warp;
+    const int s_loc = threadIdx.x;               // pixel row inside the tile
+    const uint32_t smem_a = smem_u32(smem);
+    const uint32_t ah = smem_u32(asm_hi), al = smem_u32(asm_lo);
+    int stage = 0; uint32_t phase = 0;
+    auto release = [&](int st) { if (lane == 0) mbar_arrive(&empty_bar[st]); };
     float as0 = 0.f, as1 = 0.f;                  // sum_s a[s,k] for k = 2*lane, 2*lane+1 (this warp's rows)
     int dslot = 1;
     NvIter cur;
@@ -496,7 +345,7 @@ netvlad_tc_kernel(const __grid_constant__ CUtensorMap tm_xhi, const __grid_const
     NV_STAMP(0);
     for (int it = 0; cur.valid(); cur.next(), ++it) {
       const int unit = cur.u, b = unit / a.G;
-      const int u = cur.useq;
+      float* po = a.part + (long long)unit * 64 * 512;
       {
         const int s = cur.t * 128 + s_loc;
         const bool valid = s < a.S;
@@ -506,26 +355,45 @@ netvlad_tc_kernel(const __grid_constant__ CUtensorMap tm_xhi, const __grid_const
           for (int p = 0; p < a.ssq_parts; ++p) ss += __ldg(a.ssq + (long long)p * a.B * a.S + (long long)b * a.S + s);
           inv = 1.f / fmaxf(sqrtf(ss), 1e-12f);
         }
-        const int zb = it & 1;
-        mbar_wait(&z_full[zb], (it >> 1) & 1);
-        NV_STAMP(dslot); ++dslot;                  // logits of this tile are ready
-        tc_fence_after();
+        // ---- GEMM 1: Z[128 px, 64 clusters] = x . W^T (bf16x3) ----
         float z[64];
         {
-          const uint32_t t_z = tmem_base + zb * 128 + lane_base;
+          Acc128<64> zacc;
+          int prev = -1;
+          for (int c = 0; c < 8; ++c) {
+            mbar_wait(&full_bar[stage], phase);
+            const uint32_t sa = smem_a + stage * NV_STAGE;
+            const uint64_t xh = gmma_desc_kmajor_sw128(sa), xl = gmma_desc_kmajor_sw128(sa + NV_SLOT);
+            const uint64_t wh = gmma_desc_kmajor_sw128(sa + 2 * NV_SLOT);
+            const uint64_t wl = gmma_desc_kmajor_sw128(sa + 2 * NV_SLOT + 8192);
+            constexpr uint64_t kHalf = 64 * 128 / 16;   // pixel rows 64-127: +8 KiB
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+              const uint64_t ko = (uint64_t)(k * 2);
+              zacc.mma(xl + ko, xl + kHalf + ko, wh + ko, (c > 0 || k > 0) ? 1u : 0u);
+              zacc.mma(xh + ko, xh + kHalf + ko, wl + ko, 1u);
+              zacc.mma(xh + ko, xh + kHalf + ko, wh + ko, 1u);
+            }
+            wgmma_commit();
+            wgmma_wait<1>();
+            if (prev >= 0) release(prev);
+            prev = stage;
+            if (++stage == NV_NSTAGE) { stage = 0; phase ^= 1; }
+          }
+          wgmma_wait<0>();
+          zacc.fence_operands();
+          release(prev);
+          NV_STAMP(dslot); ++dslot;                  // logits of this tile are ready
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
-            uint32_t r0[32], r1[32];
-            tmem_ld_32x32(t_z + h * 32, r0);        // x.W_hi (hi and lo planes of x)
-            tmem_ld_32x32(t_z + 64 + h * 32, r1);   // x_hi.W_lo
-            tmem_ld_wait();
+            uint32_t r0[32];
+            zacc.rows32(h, stg, r0);
 #pragma unroll
-            for (int j = 0; j < 32; ++j) z[h * 32 + j] = (__uint_as_float(r1[j]) + __uint_as_float(r0[j])) * inv;
+            for (int j = 0; j < 32; ++j) z[h * 32 + j] = __uint_as_float(r0[j]) * inv;
           }
+          wg_sync();                                 // every row has read its logits before a' overwrites them
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&z_empty[zb]);  // GEMM 1 of tile it+2 may overwrite this buffer
         float m = z[0];
 #pragma unroll
         for (int j = 1; j < 64; ++j) m = fmaxf(m, z[j]);
@@ -536,7 +404,6 @@ netvlad_tc_kernel(const __grid_constant__ CUtensorMap tm_xhi, const __grid_const
 #pragma unroll
         for (int j = 0; j < 64; ++j) z[j] *= rs;   // a[s,:] (0 for rows past the image)
         // a' = a * inv as bf16 hi/lo, MN-major SW128 row s_loc: 8 chunks of 8 values, chunk j at j^(s&7)
-        mbar_wait(a_empty, (it & 1) ^ 1);          // GEMM 2 of the previous tile has consumed the buffer
         {
           uint8_t* rh = asm_hi + s_loc * 128;
           uint8_t* rl = asm_lo + s_loc * 128;
@@ -558,9 +425,7 @@ netvlad_tc_kernel(const __grid_constant__ CUtensorMap tm_xhi, const __grid_const
           }
         }
         fence_proxy_async();                       // generic-proxy smem writes -> visible to the tensor core
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(a_full);
+        wg_sync();                                 // every row of a' is written
         NV_STAMP(dslot); ++dslot;                  // a' published
         // column sums of a over this warp's 32 rows: butterfly, lane L ends with columns 2L, 2L+1
         {
@@ -600,61 +465,79 @@ netvlad_tc_kernel(const __grid_constant__ CUtensorMap tm_xhi, const __grid_const
             if (i == 0) as0 += v; else as1 += v;
           }
         }
+        // ---- GEMM 2: V[128 c, 64 k] (4 channel blocks) += X^T a', added into the unit's partial ----
+        const bool fresh = cur.first();
+        const int fw = q, fl = lane;
+        for (int cb = 0; cb < 4; ++cb) {
+          mbar_wait(&full_bar[stage], phase);
+          const uint32_t sa = smem_a + stage * NV_STAGE;
+          Acc128<64> v;
+          wgmma_fence();
+#pragma unroll
+          for (int ks = 0; ks < 8; ++ks) {     // 16 pixel rows (2048 B) per MMA
+            const uint32_t off = ks * 2048;
+            const uint64_t xh0 = gmma_desc_mnmajor_sw128(sa + off, NV_SLOT);
+            const uint64_t xh1 = gmma_desc_mnmajor_sw128(sa + NV_SLOT + off, NV_SLOT);
+            const uint64_t xl0 = gmma_desc_mnmajor_sw128(sa + 2 * NV_SLOT + off, NV_SLOT);
+            const uint64_t xl1 = gmma_desc_mnmajor_sw128(sa + 3 * NV_SLOT + off, NV_SLOT);
+            const uint64_t bh = gmma_desc_mnmajor_sw128(ah + off, 0);
+            const uint64_t bl = gmma_desc_mnmajor_sw128(al + off, 0);
+            v.mma<false, 1, 1>(xl0, xl1, bh, ks > 0 ? 1u : 0u);
+            v.mma<false, 1, 1>(xh0, xh1, bl, 1u);
+            v.mma<false, 1, 1>(xh0, xh1, bh, 1u);
+          }
+          wgmma_commit();
+          wgmma_wait<0>();
+          v.fence_operands();
+          release(stage);
+          if (++stage == NV_NSTAGE) { stage = 0; phase ^= 1; }
+          // fragment element (channel row r, cluster column k) -> part[k][cb*128 + r]
+#pragma unroll
+          for (int j = 0; j < 2; ++j)
+#pragma unroll
+            for (int i = 0; i < 8; ++i)
+#pragma unroll
+              for (int e = 0; e < 4; ++e) {
+                const int r = 64 * j + 16 * fw + (fl >> 2) + ((e & 2) ? 8 : 0);
+                const int k = 8 * i + 2 * (fl & 3) + (e & 1);
+                float* dst = po + (long long)k * 512 + cb * 128 + r;
+                *dst = fresh ? v.h[j][4 * i + e] : *dst + v.h[j][4 * i + e];
+              }
+        }
       }
       if (cur.last()) {
-        // ---- unit epilogue: partial V^T and partial sum_s a ----
+        // ---- unit epilogue: partial sum_s a, then the last unit of the image finalises it ----
         asum_sm[q * 64 + 2 * lane] = as0;
         asum_sm[q * 64 + 2 * lane + 1] = as1;
-        mbar_wait(d_full, u & 1);
+        wg_sync();
         NV_STAMP(dslot); ++dslot;                    // all MMAs of the unit retired
-        tc_fence_after();
-        float* po = a.part + (long long)unit * 64 * 512;
-        for (int cb = 0; cb < 4; ++cb) {
-          uint32_t r0[32], r1[32];
-          tmem_ld_32x32(t_d + cb * 64 + lane_base, r0);
-          tmem_ld_32x32(t_d + cb * 64 + lane_base + 32, r1);
-          tmem_ld_wait();
-          const int c = cb * 128 + s_loc;            // TMEM lane == channel inside the block
-  #pragma unroll
-          for (int k = 0; k < 32; ++k) {
-            po[(long long)k * 512 + c] = __uint_as_float(r0[k]);
-            po[(long long)(k + 32) * 512 + c] = __uint_as_float(r1[k]);
-          }
-        }
-        tc_fence_before();
-        // the four epilogue warps meet (named barrier 1) before their asum partials are combined
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        if (lane == 0) mbar_arrive(d_empty);         // V has been read out of TMEM: the next unit's GEMM 2 may start
-        if (threadIdx.x - 64 < 64) {
-          const int k = threadIdx.x - 64;
+        if (threadIdx.x < 64) {
+          const int k = threadIdx.x;
           a.asum_part[(long long)unit * 64 + k] = asum_sm[k] + asum_sm[64 + k] + asum_sm[128 + k] + asum_sm[192 + k];
         }
         // ---- last unit of the image finalises it (threadfence-reduction pattern) ----
         __threadfence();                             // this thread's partial is visible device-wide
-        asm volatile("bar.sync 1, 128;" ::: "memory");
+        wg_sync();
         int* flag_sm = reinterpret_cast<int*>(asum_sm + 256);
-        if (threadIdx.x == 64) {
+        if (threadIdx.x == 0) {
           const int tk = atomicAdd(a.ticket + b, 1);
           const int lastu = (tk == a.G - 1) ? 1 : 0;
           if (lastu) a.ticket[b] = 0;                // self-cleaning: the next launch finds zeros again
           *flag_sm = lastu;
         }
-        asm volatile("bar.sync 1, 128;" ::: "memory");
+        wg_sync();
         NV_STAMP(dslot); ++dslot;                    // partial written
         if (*flag_sm) {
           __threadfence();
           nv_finalize_image(a, b, q, lane, asum_sm);
           NV_STAMP(dslot); ++dslot;                  // image finalised
         }
-        asm volatile("bar.sync 1, 128;" ::: "memory");   // flag_sm / asum_sm are reused by the next unit
+        wg_sync();                                   // flag_sm / asum_sm are reused by the next unit
         as0 = 0.f; as1 = 0.f;
         dslot = 1;
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, 512); }
 }
 
 // (A 4-CTA-cluster variant that reads every feature byte once -- channels split over the cluster, partial logits
@@ -697,8 +580,8 @@ int launch_netvlad_tc(const __nv_bfloat16* x_hi, const __nv_bfloat16* x_lo, int 
   static unsigned long long* dbg_dev = nullptr;
   static int dbg_on = -1;
   if (dbg_on < 0) { const char* v = getenv("IBL_NV_DEBUG"); dbg_on = (v && atoi(v)) ? 1 : 0; }
-  if (dbg_on && !dbg_dev) { cudaMalloc(&dbg_dev, 148 * 32 * 8); }
-  if (dbg_on) cudaMemsetAsync(dbg_dev, 0, 148 * 32 * 8, s);
+  if (dbg_on && !dbg_dev) { cudaMalloc(&dbg_dev, 256 * 32 * 8); }
+  if (dbg_on) cudaMemsetAsync(dbg_dev, 0, 256 * 32 * 8, s);
   a.dbg = dbg_on ? dbg_dev : nullptr;
   const int smem = NV_NSTAGE * NV_STAGE + 2 * NV_SLOT + 1024 + 128 + 4 * 64 * 4 + 16;
   static DeviceOnce attr_done;   // the attribute is per device
@@ -706,18 +589,16 @@ int launch_netvlad_tc(const __nv_bfloat16* x_hi, const __nv_bfloat16* x_lo, int 
     IBL_CUDA_OK(cudaFuncSetAttribute(netvlad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     attr_done.mark();
   }
-  int sms = 148, dev = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int sms = device_sm_count();
   const int units = B * a.G;
-  netvlad_tc_kernel<<<units < sms ? units : sms, 192, smem, s>>>(mx_hi, mx_lo, mw_hi, mw_lo, a);
+  netvlad_tc_kernel<<<units < sms ? units : sms, 160, smem, s>>>(mx_hi, mx_lo, mw_hi, mw_lo, a);
   IBL_CUDA_OK(cudaGetLastError());
   if (dbg_on) {   // print phase stamps of a few CTAs (ns relative to the earliest stamp)
     cudaStreamSynchronize(s);
-    static unsigned long long h[148 * 32];
+    static unsigned long long h[256 * 32];
     cudaMemcpy(h, dbg_dev, sizeof(h), cudaMemcpyDeviceToHost);
     unsigned long long t0 = ~0ull;
-    for (int i = 0; i < 148 * 32; ++i) if (h[i] && h[i] < t0) t0 = h[i];
+    for (int i = 0; i < 256 * 32; ++i) if (h[i] && h[i] < t0) t0 = h[i];
     for (int c : {0, 1, 60, 127}) {
       fprintf(stderr, "[nv-debug] cta %3d:", c);
       for (int j = 0; j < 12; ++j) fprintf(stderr, " %6lld", h[c * 32 + j] ? (long long)(h[c * 32 + j] - t0) : -1ll);

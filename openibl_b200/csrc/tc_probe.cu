@@ -1,4 +1,4 @@
-// Hardware probe: does a K-major SWIZZLE_128B UMMA operand tolerate (a) a start address that is 128-byte
+// Hardware probe: does a K-major SWIZZLE_128B wgmma operand tolerate (a) a start address that is 128-byte
 // but not 1024-byte aligned and (b) a stride between 8-row groups (SBO) that is not a multiple of 1024?
 // That is what a convolution needs to read all nine taps out of ONE halo tile staged by a single TMA box
 // ([rows of (TW+2) pixels][64 channels]): tap (kh,kw) starts (kh*(TW+2)+kw) rows into the tile and 8-pixel
@@ -16,65 +16,64 @@ namespace ibl {
 
 using namespace tc;
 
+// K-major SW128 descriptor of the view starting at a_addr with 8-row groups sbo bytes apart; base_mode 1 sets the
+// descriptor's base_offset field to the start row's swizzle phase
+__device__ __forceinline__ uint64_t probe_desc(uint32_t a_addr, uint32_t sbo, int base_mode) {
+  uint64_t d = 0;
+  d |= (uint64_t)((a_addr >> 4) & 0x3fffu);
+  d |= (uint64_t)1 << 16;
+  d |= (uint64_t)((sbo >> 4) & 0x3fffu) << 32;
+  if (base_mode == 1) d |= (uint64_t)((a_addr >> 7) & 7u) << 49;
+  d |= (uint64_t)1 << 62;
+  return d;
+}
+
 __global__ void __launch_bounds__(128, 1)
-umma_strided_probe_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
+gmma_strided_probe_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
                           int rows, int s0, int group_rows, int base_mode, float* __restrict__ D) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* a_sm = smem;                       // rows * 128 B (<= 32 KiB)
   uint8_t* b_sm = smem + 32768;               // 64 rows * 128 B
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 32768 + 8192);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  float* stg = reinterpret_cast<float*>(smem + 32768 + 8192);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 32768 + 8192 + ACC_STG_BYTES);
   if (threadIdx.x == 0) {
     mbar_init(&bars[0], 1);
-    mbar_init(&bars[1], 1);
     fence_barrier_init();
     fence_proxy_async();
   }
-  if (warp == 0) { tmem_alloc(tmem_slot, 64); tmem_relinquish(); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   if (threadIdx.x == 0) {
     mbar_arrive_expect_tx(&bars[0], rows * 128 + 8192);
     tma_load_2d(a_sm, &tm_a, &bars[0], 0, 0);
     tma_load_2d(b_sm, &tm_b, &bars[0], 0, 0);
-    mbar_wait(&bars[0], 0);
-    tc_fence_after();
-    const uint32_t a_addr = smem_u32(a_sm) + (uint32_t)s0 * 128u;
-    uint64_t da = 0;
-    da |= (uint64_t)((a_addr >> 4) & 0x3fffu);
-    da |= (uint64_t)1 << 16;
-    da |= (uint64_t)(((uint32_t)group_rows * 128u) >> 4) << 32;       // SBO = group_rows * 128 B
-    da |= (uint64_t)1 << 46;
-    if (base_mode == 1) da |= (uint64_t)((a_addr >> 7) & 7u) << 49;   // base_offset = start phase
-    da |= (uint64_t)2 << 61;
-    const uint64_t db = umma_desc_kmajor_sw128(smem_u32(b_sm));
-    constexpr uint32_t idesc = umma_idesc_bf16_f32(128, 64);
-    for (int k = 0; k < 4; ++k) umma_bf16(tmem_base, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), idesc, k > 0);
-    umma_commit(&bars[1]);
   }
-  __syncwarp();
-  mbar_wait(&bars[1], 0);
-  tc_fence_after();
-  {
-    uint32_t r0[32], r1[32];
-    const uint32_t t = tmem_base + ((uint32_t)(warp * 32) << 16);
-    tmem_ld_32x32(t, r0);
-    tmem_ld_32x32(t + 32, r1);
-    tmem_ld_wait();
-    float* o = D + (size_t)(warp * 32 + lane) * 64;
-    for (int j = 0; j < 32; ++j) { o[j] = __uint_as_float(r0[j]); o[32 + j] = __uint_as_float(r1[j]); }
+  mbar_wait(&bars[0], 0);
+  const uint32_t sbo = (uint32_t)group_rows * 128u;
+  const uint32_t a0 = smem_u32(a_sm) + (uint32_t)s0 * 128u;
+  const uint32_t a1 = a0 + 8u * sbo;          // rows 64-127 of the view: groups 8-15
+  const uint64_t da0 = probe_desc(a0, sbo, base_mode), da1 = probe_desc(a1, sbo, base_mode);
+  const uint64_t db = gmma_desc_kmajor_sw128(smem_u32(b_sm));
+  Acc128<64> acc;
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < 4; ++k)
+    acc.mma(da0 + (uint64_t)(k * 2), da1 + (uint64_t)(k * 2), db + (uint64_t)(k * 2), k > 0 ? 1u : 0u);
+  wgmma_commit();
+  wgmma_wait<0>();
+  acc.fence_operands();
+  float* o = D + (size_t)threadIdx.x * 64;
+#pragma unroll
+  for (int ch = 0; ch < 2; ++ch) {
+    uint32_t r[32];
+    acc.rows32(ch, stg, r);
+#pragma unroll
+    for (int j = 0; j < 32; ++j) o[ch * 32 + j] = __uint_as_float(r[j]);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) { tc_fence_after(); tmem_dealloc(tmem_base, 64); }
 }
 
 // A: [rows][64] bf16 bits, B: [64][64] bf16 bits (device), D: [128][64] fp32
-int debug_umma_strided(const void* A, int rows, const void* B, int s0, int group_rows, int base_mode, float* D,
+int debug_gmma_strided(const void* A, int rows, const void* B, int s0, int group_rows, int base_mode, float* D,
                        cudaStream_t s) {
   IBL_REQUIRE(rows >= 8 && rows <= 256 && s0 >= 0 && group_rows >= 8 && s0 + 15 * group_rows + 8 <= rows,
               "probe view does not fit the halo tile");
@@ -91,13 +90,13 @@ int debug_umma_strided(const void* A, int rows, const void* B, int s0, int group
     uint32_t box[2] = {64, 64};
     IBL_RET(make_tmap(&mb, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, B, dims, str, box));
   }
-  const int smem = 32768 + 8192 + 1024 + 64;
+  const int smem = 32768 + 8192 + ACC_STG_BYTES + 1024 + 64;
   static DeviceOnce attr_done;   // the attribute is per device
   if (!attr_done.done()) {
-    IBL_CUDA_OK(cudaFuncSetAttribute(umma_strided_probe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    IBL_CUDA_OK(cudaFuncSetAttribute(gmma_strided_probe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     attr_done.mark();
   }
-  umma_strided_probe_kernel<<<1, 128, smem, s>>>(ma, mb, rows, s0, group_rows, base_mode, D);
+  gmma_strided_probe_kernel<<<1, 128, smem, s>>>(ma, mb, rows, s0, group_rows, base_mode, D);
   IBL_CUDA_OK(cudaGetLastError());
   return IBL_OK;
 }

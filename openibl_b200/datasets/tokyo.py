@@ -17,6 +17,6 @@ class Tokyo(PlaceDataset):
                 raise RuntimeError("Dataset not found.")
             raise NotImplementedError(
                 "Tokyo 24/7: meta.json / splits.json are missing under %r; arranging them from the raw .mat files "
-                "is host-side dataset preparation outside the B200 hot path -- produce them once with the "
+                "is host-side dataset preparation outside the GPU hot path -- produce them once with the "
                 "reference's ibl.datasets.create('tokyo', root)" % root)
         self.load(verbose)

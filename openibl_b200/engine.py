@@ -31,7 +31,7 @@ def _require_cuda(t: torch.Tensor, name: str, dtype=torch.float32) -> torch.Tens
         raise TypeError(f"{name} must be a torch.Tensor")
     if not t.is_cuda:
         raise RuntimeError(
-            f"{name} is on '{t.device}': the OpenIBL-B200 hot path runs only on an sm_100 GPU "
+            f"{name} is on '{t.device}': the OpenIBL hot path runs only on an sm_90 (H100) GPU "
             "(there is no CPU fallback); move the tensor/model to CUDA")
     if t.dtype != dtype:
         raise TypeError(f"{name} must be {dtype}, got {t.dtype}")
@@ -51,7 +51,7 @@ class Engine:
 
     def __init__(self, device: int):
         if not torch.cuda.is_available():
-            raise RuntimeError("no CUDA device: the OpenIBL-B200 engine has no CPU fallback")
+            raise RuntimeError("no CUDA device: the OpenIBL engine has no CPU fallback")
         self.lib = _cabi.load()
         self.device = int(device)
         h = c_void_p()
@@ -65,10 +65,10 @@ class Engine:
     def get(device=None) -> "Engine":
         if isinstance(device, torch.device) and device.type != "cuda":
             raise RuntimeError(
-                f"tensor/model is on '{device}': the OpenIBL-B200 hot path runs only on an sm_100 GPU "
+                f"tensor/model is on '{device}': the OpenIBL hot path runs only on an sm_90 (H100) GPU "
                 "(there is no CPU fallback); move it to CUDA")
         if not torch.cuda.is_available():
-            raise RuntimeError("no CUDA device: the OpenIBL-B200 engine has no CPU fallback")
+            raise RuntimeError("no CUDA device: the OpenIBL engine has no CPU fallback")
         if device is None:
             device = torch.cuda.current_device()
         if isinstance(device, torch.device):

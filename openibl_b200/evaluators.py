@@ -301,7 +301,7 @@ class Evaluator(object):
         if not rerank:
             return recalls
         # evaluators.py:194-201: k-reciprocal re-ranking needs the dense q-g, q-q and g-g matrices; they are
-        # built on the GPU (tcgen05 dense distance tiles) and re-ranked there (utils/rerank.py), rank 0 only,
+        # built on the GPU (tensor-core dense distance tiles) and re-ranked there (utils/rerank.py), rank 0 only,
         # as in the reference (the other ranks score the original matrix).  The database rows are gathered
         # over NVLink (device memory), never through the host.
         eng = Engine.get(dev)

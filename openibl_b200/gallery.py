@@ -6,7 +6,7 @@ Every image is generated on the device from a seed that depends only on its GLOB
 and therefore every descriptor, every distance and the final ranking -- is the same whatever the world
 size.  Query j is a noisy copy of database image pos[j] (so Recall@N is a real number); images are smooth random
 fields, not white noise.  A random-init trunk still maps all of them to almost the same descriptor (pairwise distances
-~1e-5: measured, profiles/r02_diag_gallery.jsonl -- every query then trips the screening guard and even fp32 "exact"
+~1e-5 (tools/diag_gallery.py shows it) -- every query then trips the screening guard and even fp32 "exact"
 distances are rounding noise), so callers that want a meaningful ranking first centre the PCA layer on a database sample
 (center_pca below: what a PCA fit does); distances are then ~0.8 and Recall@1 goes from 0.999 (query noise 0.1 sigma) to
 ~0 (0.5 sigma) on 30k images, and 0.2 sigma gives 0.0096 on 250k; the default noise is 0.1 sigma.
@@ -15,7 +15,7 @@ Flow (SURVEY 5 / 8e; reference: ibl/evaluators.py:76-101,105-130,142-167 is what
   1. rank r extracts its DistributedSliceSampler slice of the database and of the queries
      (ceil(n/W) images, VGG16 + NetVLAD + PCA) -- descriptors stay in that GPU's HBM;
   2. the queries are all-gathered (n_q x 16 KiB);
-  3. every rank ranks all queries against its slice (tcgen05 distance + top-k + exact re-scoring);
+  3. every rank ranks all queries against its slice (tensor-core distance + top-k + exact re-scoring);
   4. ONE all-gather of the [n_q, k] candidates (8 B each) + a merge kernel.
 `emulate_world=W` plays all W ranks on one GPU, one after the other, with the very same slicing and
 batching (merge through ibl_topk_merge instead of NCCL): it is how a 1-GPU box checks that the W-GPU

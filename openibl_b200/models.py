@@ -39,7 +39,7 @@ def _layer_table():
 class _VGGTrunkFunction(torch.autograd.Function):
     """VGG.forward with a trainable suffix (layers first..12): frozen prefix on the inference kernels, then one
     conv(+ReLU) at a time keeping (input, post-ReLU output) for the backward; pools are separate so that the pre-pool
-    activation is available.  Backward: ReLU mask + tcgen05 dgrad/wgrad per layer (ibl_vgg16_layer_backward),
+    activation is available.  Backward: ReLU mask + tensor-core dgrad/wgrad per layer (ibl_vgg16_layer_backward),
     first-maximum 2x2 pool backward.  Gradients come back in the parameters' own layouts (OIHW, [Cout])."""
 
     @staticmethod
@@ -83,7 +83,7 @@ def _no_train(module: nn.Module, what: str) -> None:
     if module.training and torch.is_grad_enabled():
         raise NotImplementedError(
             f"{what}: only the inference path (model.eval() / torch.no_grad()) is implemented in the "
-            "B200 engine; the training/backward kernels are scheduled next (SURVEY 8f)")
+            "H100 engine; the training/backward kernels are scheduled next (SURVEY 8f)")
 
 
 class VGG(nn.Module):

@@ -1,4 +1,4 @@
-"""SURVEY 8 row f1 / BASELINE configs[4]: the training surface -- conv dgrad / wgrad on tcgen05, pool backward, the
+"""SURVEY 8 row f1 / BASELINE configs[4]: the training surface -- conv dgrad / wgrad on the tensor cores, pool backward, the
 VGG trunk autograd Function, and one SFRS step (trainers.py:235-259) against the UNMODIFIED reference run on CPU
 (tests/golden/sfrs_step.npz, oracle/gen_golden_sfrs.py).  Tolerances are stated next to each check."""
 import numpy as np
@@ -39,7 +39,7 @@ LAYER_CASES = [
 
 @pytest.mark.parametrize("case", LAYER_CASES)
 def test_conv_layer_forward_backward_vs_fp64_autograd(eng, case):
-    """y = [ReLU](conv(x)+b), dL/dx (tcgen05 dgrad = forward kernel on rotated filters), dL/dW (tcgen05 wgrad with
+    """y = [ReLU](conv(x)+b), dL/dx (tensor-core dgrad = forward kernel on rotated filters), dL/dW (tensor-core wgrad with
     pixel-major operands), dL/db against torch autograd in fp64.  rel-L2 <= 1e-4 (north-star tolerance; bf16x3
     measures ~2e-5)."""
     layer, N, H, W = case

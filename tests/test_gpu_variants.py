@@ -1,6 +1,8 @@
 """Kernel variants that are selected by environment variables (read once per process) are exercised in child
-processes, each running the relevant subset of the parity tests: every staging / pairing mode of the tcgen05
-conv and the one-SM distance kernel must give the same answers as the defaults.  Also pins the hardware property the halo-staged conv relies on."""
+processes, each running the relevant subset of the parity tests: both staging modes and the SM pairs of the tensor-core
+conv, the separate conv1_1 / conv1_2 kernels (tensor-core or CUDA-core conv1_1) and the bf16x3 distance screening kernel
+on one SM or on SM pairs must give the same answers as the defaults.  Also pins the hardware property halo-staged
+convolution relies on."""
 import os
 import subprocess
 import sys
@@ -14,11 +16,10 @@ VARIANTS = [
     # env, -k expression
     ({"IBL_CONV_HALO": "2"}, "conv3x3 or small or odd"),                    # halo staging on every N tile
     ({"IBL_CONV_HALO": "0", "IBL_CONV_2SM": "0"}, "conv3x3 or small or odd"),   # im2col boxes, one SM per tile
-    ({"IBL_CONV_2SM": "2", "IBL_CONV_HALO": "0"}, "conv3x3 or odd"),        # SM pairs on the 128-wide tiles too
+    ({"IBL_CONV_2SM": "2", "IBL_CONV_HALO": "0"}, "conv3x3 or odd"),        # SM pairs on every layer
     ({"IBL_CONV1_FUSED": "0"}, "small or odd or hub or tokyo"),             # separate conv1_1 / conv1_2 kernels
     ({"IBL_CONV1_FUSED": "0", "IBL_CONV1_SIMT": "1"}, "small or odd"),      # ... with the CUDA-core conv1_1
-    ({"IBL_DIST_BN": "512"}, "retrieval or topk or single_pass"),            # 256 x 512 screening tiles, one accumulator
-    ({"IBL_DIST_SCREEN": "3"}, "retrieval or topk"),                         # round-1 bf16x3 screening on SM pairs
+    ({"IBL_DIST_SCREEN": "3"}, "retrieval or topk"),                         # bf16x3 screening (tc_gemm.cu) on SM pairs
     ({"IBL_DIST_SCREEN": "3", "IBL_DIST_2SM": "0"}, "retrieval_vs_reference or topk"),   # ... on one SM
     ({"IBL_DIST_SCREEN": "3", "IBL_DIST_2SM": "0", "IBL_DIST_BN": "128", "IBL_GEMM_MC": "1"}, "retrieval_vs_reference or topk"),
 ]
@@ -39,8 +40,8 @@ def test_variant_matches_references(env, expr):
 
 @pytest.mark.gpu
 def test_umma_sw128_operand_accepts_unaligned_start_and_odd_group_stride():
-    """tc_conv.cu's halo staging reads nine tap views out of one TMA-written tile: starts that are 128-byte but
-    not 1024-byte aligned, 8-row groups 10 rows apart, descriptor base_offset = 0."""
+    """Halo staging reads nine tap views out of one TMA-written tile: starts that are 128-byte but not 1024-byte
+    aligned, 8-row groups 10 rows apart, descriptor base_offset = 0 (tensor-core MMA, here wgmma)."""
     from openibl_b200.engine import Engine, _ptr, _stream
     from openibl_b200._cabi import check
     eng = Engine.get(0)

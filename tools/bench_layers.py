@@ -1,5 +1,5 @@
 """Per-layer device times of the VGG16 backbone at batch 32, 480x640 (same process, CUDA events):
-conv1_1 on the CUDA cores, conv1_2..conv5_3 on tcgen05 with each admissible N tile."""
+conv1_1 on the CUDA cores, conv1_2..conv5_3 on the tensor cores (wgmma) with each admissible N tile."""
 import ctypes, json, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -25,10 +25,10 @@ print(f"{'layer':8s} {'HxW':>9s} {'Cin':>4s} {'Cout':>4s} {'BN':>4s} {'ms':>8s} 
 for li, (hh, ww, cin, cout) in enumerate(shapes):
     if li == 0:
         x = torch.randn(B, 3, hh, ww, device="cuda")
-        bns = [0, 1]   # 0 = tcgen05 conv1_1, 1 = CUDA-core conv1_1
+        bns = [0, 1]   # 0 = tensor-core conv1_1, 1 = CUDA-core conv1_1
     else:
         x = torch.randn(B, hh, ww, cin, device="cuda").relu_()
-        bns = [b for b in (64, 128, 256) if cout % b == 0]
+        bns = [b for b in (64, 128) if cout % b == 0]
     gf = 2.0 * B * hh * ww * 9 * cin * cout / 1e9
     for bn in bns:
         ms = ctypes.c_float()

@@ -221,9 +221,12 @@ int ibl_gemm_nt(ibl_engine* e, const float* A, int m, const float* B, int n, int
                 void* stream);
 
 /* ---- self-tests (GPU) ------------------------------------------------------ */
-/* Queries that the guard of the single-pass distance path re-ranked by exact brute force in the last
- * ibl_l2dist_topk call (-1: that path was not taken).  Synchronises. */
+/* Queries that the screening guard re-ranked by exact brute force in the last ibl_l2dist_topk call
+ * (-1: that call took the exact fp32 path, which has no guard).  Synchronises. */
 int ibl_debug_dist_flagged(ibl_engine* e, int* count, void* stream);
+/* Ranking path of the last ibl_l2dist_topk call: 0 exact fp32 CUDA cores, 1 single-pass fp16 screening,
+ * 2 bf16x3 screening with a running top-16, 3 bf16x3 dense tiles + row select (-1: no call yet). */
+int ibl_debug_dist_path(ibl_engine* e, int* path);
 /* Runs the wgmma/TMA building blocks against CUDA-core results on the device;
  * returns IBL_OK when all agree. max_rel_err (may be NULL) receives the worst error. */
 int ibl_selftest_tc(ibl_engine* e, float* max_rel_err);

@@ -59,6 +59,7 @@ SIGNATURES = {
     "ibl_l2dist_topk_host": (c_int, [_P, _P, c_int, _P, c_int, c_int, c_int, _P, _P, _P]),
     "ibl_gemm_nt": (c_int, [_P, _P, c_int, _P, c_int, c_int, c_float, _P, c_int, _P]),
     "ibl_debug_dist_flagged": (c_int, [_P, POINTER(c_int), _P]),
+    "ibl_debug_dist_path": (c_int, [_P, POINTER(c_int)]),
     "ibl_selftest_tc": (c_int, [_P, POINTER(c_float)]),
     "ibl_debug_gemm_tn": (c_int, [_P, _P, _P, _P, _P]),
     "ibl_debug_umma_strided": (c_int, [_P, _P, c_int, _P, c_int, c_int, c_int, _P, _P]),

@@ -152,7 +152,13 @@ int launch_dist_dense_tc(const __nv_bfloat16* q_hi, const __nv_bfloat16* q_lo, c
 size_t dist1_workspace_bytes(int m, int n, int d, size_t* off /*[9]*/);
 int launch_dist_topk_1pass(const float* q, int m, const float* db, int n, int n_valid, int d, int k, long long idx_base,
                            void* ws, float* out_dist, long long* out_idx, uint64_t* launches, cudaStream_t s);
-int dist1_last_flag_count(void* ws, int m, int n, int d, int* out, cudaStream_t s);
+const int* dist1_flag_counter(const void* ws, int m, int n, int d);
+// ... and the same guard + exact fallback after the bf16x3 screening of tc_gemm.cu
+size_t dist_guard_workspace_bytes(int m);
+int launch_dist_guard_bf16x3(const float* q, const float* q_sq, const float2* q_err, int m, const float* db,
+                             const float* db_sq, const float2* db_err, int n_valid, int d, const float* screened, int kc,
+                             int k, long long idx_base, void* ws, float* out_dist, long long* out_idx,
+                             uint64_t* launches, cudaStream_t s);
 int pca_tc_splits(int P, int D);
 int launch_pca_partial_tc(const __nv_bfloat16* w_hi, const __nv_bfloat16* w_lo, int P,
                           const __nv_bfloat16* v_hi, const __nv_bfloat16* v_lo, int N, int D,
@@ -192,7 +198,7 @@ int launch_l2_normalize_rows(const float* x, int N, int D, float* out, cudaStrea
 int launch_row_sqnorm(const float* x, int N, int D, float* out, cudaStream_t s);
 int launch_scale(const float* x, float s, int n, float* y, cudaStream_t st);
 int launch_planes_sqnorm(const float* x, int N, int D, __nv_bfloat16* hi, __nv_bfloat16* lo, float* sq,
-                         cudaStream_t st);
+                         float2* err, cudaStream_t st);   // err (may be null): per row {|lo|, |x - hi - lo|}
 int launch_l2dist_dense(const float* q, const float* qn, int m, const float* db, const float* dbn,
                         int n, int d, float* out, long long ld_out, cudaStream_t s);
 

@@ -81,7 +81,9 @@ struct ibl_engine {
   DevBuf mrg_d, mrg_i;
   DevBuf bw_g, bw_x, bw_part, bw_w;      // conv backward: dY planes, X planes, wgrad/bias partials, dgrad filter planes
   DevBuf d1_ws;                          // workspace of the single-pass distance/top-k path (tc_dist1.cu)
-  int d1_m = 0, d1_n = 0, d1_d = 0;      // shape of the last call on it (test hook ibl_debug_dist_flagged)
+  DevBuf q_err, db_err, guard_ws;        // guard of the bf16x3 screening paths: per-row error norms, workspace
+  const int* flag_counter = nullptr;     // guard counter of the last ibl_l2dist_topk call (null: no guard on its path)
+  int dist_path = -1;                    // ranking path of the last ibl_l2dist_topk call (ibl_debug_dist_path)
   DevBuf ssq, nv_part, nv_asum, nvw_pl;  // fused NetVLAD: |x|^2 partials, unit partials, W planes [64,512]
   DevBuf nv_ticket;                      // [images] arrival counters of the fused NetVLAD kernel (zero between launches)
   const float* nvw_pl_src = nullptr;
@@ -944,7 +946,8 @@ int ibl_l2dist_topk(ibl_engine* e, const float* q, int m, const float* db, int n
     // single fp16 tensor-core pass to screen, exact fp32 to decide, guard + exact fallback on the device
     size_t off[9];
     IBL_RET(e->d1_ws.ensure(dist1_workspace_bytes(m, n, d, off)));
-    e->d1_m = m; e->d1_n = n; e->d1_d = d;
+    e->flag_counter = dist1_flag_counter(e->d1_ws.p, m, n, d);
+    e->dist_path = 1;
     return launch_dist_topk_1pass(q, m, db, n, n_valid, d, k, (long long)idx_base, e->d1_ws.p, out_dist,
                                   reinterpret_cast<long long*>(out_idx), &e->launches, S(stream));
   }
@@ -956,11 +959,18 @@ int ibl_l2dist_topk(ibl_engine* e, const float* q, int m, const float* db, int n
     IBL_RET(e->q_pl.ensure(qe * 4));
     IBL_RET(e->db_pl.ensure(de * 4));
     __nv_bfloat16 *qh = e->q_pl.as<__nv_bfloat16>(), *dh = e->db_pl.as<__nv_bfloat16>();
-    // one pass per matrix: bf16 hi/lo planes for the tensor-core GEMM + exact fp32 squared norms
-    IBL_RET(launch_planes_sqnorm(q, m, d, qh, qh + qe, e->qn.as<float>(), s));
-    IBL_RET(launch_planes_sqnorm(db, n, d, dh, dh + de, e->dbn.as<float>(), s));
+    IBL_RET(e->q_err.ensure((size_t)m * sizeof(float2)));
+    IBL_RET(e->db_err.ensure((size_t)n * sizeof(float2)));
+    IBL_RET(e->guard_ws.ensure(dist_guard_workspace_bytes(m)));
+    const float2 *qerr = e->q_err.as<float2>(), *dberr = e->db_err.as<float2>();
+    // one pass per matrix: bf16 hi/lo planes for the tensor-core GEMM + exact fp32 squared norms + the norms of
+    // the lo planes and of the residuals (the guard's error model)
+    IBL_RET(launch_planes_sqnorm(q, m, d, qh, qh + qe, e->qn.as<float>(), e->q_err.as<float2>(), s));
+    IBL_RET(launch_planes_sqnorm(db, n, d, dh, dh + de, e->dbn.as<float>(), e->db_err.as<float2>(), s));
     e->launches += 2;
     const int kc = 16;                           // candidates kept per query before exact re-scoring
+    e->flag_counter = reinterpret_cast<const int*>(e->guard_ws.p);
+    e->dist_path = k <= 12 ? 2 : 3;
     if (k <= 12) {
       // SM pairs (2-CTA clusters multicasting the database tile, tc_gemm.cu) unless IBL_DIST_2SM=0
       static const bool two_sm = [] { const char* v = getenv("IBL_DIST_2SM"); return !v || atoi(v) != 0; }();
@@ -973,6 +983,7 @@ int ibl_l2dist_topk(ibl_engine* e, const float* q, int m, const float* db, int n
                                    &runs, two_sm, s));
       e->launches++;
       const long long* ci = e->cand_i.as<long long>();
+      const float* cd = e->cand_d.as<float>();
       if (runs > 1) {
         IBL_RET(e->mrg_d.ensure((size_t)m * kc * sizeof(float)));
         IBL_RET(e->mrg_i.ensure((size_t)m * kc * sizeof(int64_t)));
@@ -980,11 +991,15 @@ int ibl_l2dist_topk(ibl_engine* e, const float* q, int m, const float* db, int n
                                   e->mrg_d.as<float>(), e->mrg_i.as<int64_t>(), s));
         e->launches++;
         ci = e->mrg_i.as<long long>();
+        cd = e->mrg_d.as<float>();
       }
       IBL_RET(launch_rescore_sort(q, e->qn.as<float>(), m, db, e->dbn.as<float>(), d, ci, kc, k, idx_base,
                                   out_dist, reinterpret_cast<long long*>(out_idx), s));
       e->launches++;
-      return IBL_OK;
+      // guard: queries whose 16 survivors cannot be shown to hold the exact top-k are ranked by exact brute force
+      return launch_dist_guard_bf16x3(q, e->qn.as<float>(), qerr, m, db, e->dbn.as<float>(), dberr, n_valid, d, cd, kc,
+                                      k, idx_base, e->guard_ws.p, out_dist, reinterpret_cast<long long*>(out_idx),
+                                      &e->launches, s);
     }
     // k > 12: dense tiles on the tensor cores, row select, then the same exact re-scoring
     const int CHT = 32768;
@@ -1005,6 +1020,7 @@ int ibl_l2dist_topk(ibl_engine* e, const float* q, int m, const float* db, int n
       e->launches += 2;
     }
     const long long* ci = e->cand_i.as<long long>();
+    const float* cd = e->cand_d.as<float>();
     if (ncht > 1) {
       IBL_RET(e->mrg_d.ensure((size_t)m * kk * sizeof(float)));
       IBL_RET(e->mrg_i.ensure((size_t)m * kk * sizeof(int64_t)));
@@ -1012,13 +1028,18 @@ int ibl_l2dist_topk(ibl_engine* e, const float* q, int m, const float* db, int n
                                 e->mrg_d.as<float>(), e->mrg_i.as<int64_t>(), s));
       e->launches++;
       ci = e->mrg_i.as<long long>();
+      cd = e->mrg_d.as<float>();
     }
     IBL_RET(launch_rescore_sort(q, e->qn.as<float>(), m, db, e->dbn.as<float>(), d, ci, kk, k, idx_base, out_dist,
                                 reinterpret_cast<long long*>(out_idx), s));
     e->launches++;
-    return IBL_OK;
+    return launch_dist_guard_bf16x3(q, e->qn.as<float>(), qerr, m, db, e->dbn.as<float>(), dberr, n_valid, d, cd, kk, k,
+                                    idx_base, e->guard_ws.p, out_dist, reinterpret_cast<long long*>(out_idx),
+                                    &e->launches, s);
   }
   const int CH = 32768;                         // database rows per dense chunk
+  e->dist_path = 0;
+  e->flag_counter = nullptr;                    // exact: nothing to guard
   const int nch = n_valid > 0 ? cdiv(n_valid, CH) : 1;
   IBL_REQUIRE((long long)nch * k <= 8192, "database shard too large for one call; shard it");
   IBL_RET(e->qn.ensure((size_t)m * sizeof(float)));
@@ -1105,14 +1126,22 @@ int ibl_l2dist_topk_host(ibl_engine* e, const float* q_host, int m, const float*
   return IBL_OK;
 }
 
-// test hook: how many queries the guard of the single-pass distance path listed in the last ibl_l2dist_topk call
-// (they were re-ranked by exact brute force on the device).  Synchronises the stream.
+// test hook: how many queries the screening guard listed in the last ibl_l2dist_topk call (they were re-ranked by
+// exact brute force on the device); -1 when that call took the exact fp32 path.  Synchronises the stream.
 int ibl_debug_dist_flagged(ibl_engine* e, int* count, void* stream) {
   IBL_REQUIRE(e && count, "null argument");
   *count = -1;
-  if (!e->d1_ws.p || !e->d1_m) return IBL_OK;
+  if (!e->flag_counter) return IBL_OK;
   DeviceGuard g(e->device);
-  return dist1_last_flag_count(e->d1_ws.p, e->d1_m, e->d1_n, e->d1_d, count, S(stream));
+  IBL_CUDA_OK(cudaMemcpyAsync(count, e->flag_counter, sizeof(int), cudaMemcpyDeviceToHost, S(stream)));
+  IBL_CUDA_OK(cudaStreamSynchronize(S(stream)));
+  return IBL_OK;
+}
+
+int ibl_debug_dist_path(ibl_engine* e, int* path) {
+  IBL_REQUIRE(e && path, "null argument");
+  *path = e->dist_path;
+  return IBL_OK;
 }
 
 int ibl_selftest_tc(ibl_engine* e, float* max_rel_err) {

@@ -258,42 +258,56 @@ int launch_scale(const float* x, float s, int n, float* y, cudaStream_t st) {
 
 namespace ibl {
 // One pass over a row-major fp32 matrix: bf16 hi/lo planes + squared row norms (what the distance GEMM and
-// its epilogue need), instead of separate f32_to_planes and row_sqnorm passes.  One block per row.
+// its epilogue need), instead of separate f32_to_planes and row_sqnorm passes.  One block per row.  With err, also
+// the norms of the lo plane and of the residual x - hi - lo (the screening guard's error model, tc_dist1.cu).
 __global__ void __launch_bounds__(256)
 planes_sqnorm_kernel(const float* __restrict__ x, int D, __nv_bfloat16* __restrict__ hi,
-                     __nv_bfloat16* __restrict__ lo, float* __restrict__ sq) {
-  __shared__ float red[8];
+                     __nv_bfloat16* __restrict__ lo, float* __restrict__ sq, float2* __restrict__ err) {
+  __shared__ float red[8], redl[8], redr[8];
   const long long r = blockIdx.x;
   const float4* p = reinterpret_cast<const float4*>(x + r * D);
   uint2* ph = reinterpret_cast<uint2*>(hi + r * D);
   uint2* pl = reinterpret_cast<uint2*>(lo + r * D);
-  float ss = 0.f;
+  float ss = 0.f, ll = 0.f, rr = 0.f;
   for (int i = threadIdx.x; i < D / 4; i += blockDim.x) {
     const float4 v = __ldg(p + i);
     ss = fmaf(v.x, v.x, ss); ss = fmaf(v.y, v.y, ss); ss = fmaf(v.z, v.z, ss); ss = fmaf(v.w, v.w, ss);
     const __nv_bfloat16 h0 = __float2bfloat16_rn(v.x), h1 = __float2bfloat16_rn(v.y);
     const __nv_bfloat16 h2 = __float2bfloat16_rn(v.z), h3 = __float2bfloat16_rn(v.w);
     __nv_bfloat162 a(h0, h1), b(h2, h3);
-    __nv_bfloat162 c = __floats2bfloat162_rn(v.x - __bfloat162float(h0), v.y - __bfloat162float(h1));
-    __nv_bfloat162 d = __floats2bfloat162_rn(v.z - __bfloat162float(h2), v.w - __bfloat162float(h3));
+    const float4 t = make_float4(v.x - __bfloat162float(h0), v.y - __bfloat162float(h1), v.z - __bfloat162float(h2),
+                                 v.w - __bfloat162float(h3));   // exact
+    __nv_bfloat162 c = __floats2bfloat162_rn(t.x, t.y);
+    __nv_bfloat162 d = __floats2bfloat162_rn(t.z, t.w);
     ph[i] = make_uint2(*reinterpret_cast<uint32_t*>(&a), *reinterpret_cast<uint32_t*>(&b));
     pl[i] = make_uint2(*reinterpret_cast<uint32_t*>(&c), *reinterpret_cast<uint32_t*>(&d));
+    if (err) {
+      const float2 lc = __bfloat1622float2(c), ld = __bfloat1622float2(d);
+      ll = fmaf(lc.x, lc.x, ll); ll = fmaf(lc.y, lc.y, ll); ll = fmaf(ld.x, ld.x, ll); ll = fmaf(ld.y, ld.y, ll);
+      const float r0 = t.x - lc.x, r1 = t.y - lc.y, r2 = t.z - ld.x, r3 = t.w - ld.y;
+      rr = fmaf(r0, r0, rr); rr = fmaf(r1, r1, rr); rr = fmaf(r2, r2, rr); rr = fmaf(r3, r3, rr);
+    }
   }
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = ss;
+  for (int o = 16; o > 0; o >>= 1) {
+    ss += __shfl_xor_sync(0xffffffffu, ss, o);
+    ll += __shfl_xor_sync(0xffffffffu, ll, o);
+    rr += __shfl_xor_sync(0xffffffffu, rr, o);
+  }
+  if ((threadIdx.x & 31) == 0) { red[threadIdx.x >> 5] = ss; redl[threadIdx.x >> 5] = ll; redr[threadIdx.x >> 5] = rr; }
   __syncthreads();
   if (threadIdx.x == 0) {
-    float tot = 0.f;
-    for (int i = 0; i < (int)(blockDim.x >> 5); ++i) tot += red[i];
+    float tot = 0.f, tl = 0.f, tr = 0.f;
+    for (int i = 0; i < (int)(blockDim.x >> 5); ++i) { tot += red[i]; tl += redl[i]; tr += redr[i]; }
     sq[r] = tot;
+    if (err) err[r] = make_float2(sqrtf(tl), sqrtf(tr));
   }
 }
 int launch_planes_sqnorm(const float* x, int N, int D, __nv_bfloat16* hi, __nv_bfloat16* lo, float* sq,
-                         cudaStream_t st) {
+                         float2* err, cudaStream_t st) {
   IBL_REQUIRE(D % 4 == 0, "planes_sqnorm: D must be a multiple of 4");
   if (N <= 0) return IBL_OK;
-  planes_sqnorm_kernel<<<N, 256, 0, st>>>(x, D, hi, lo, sq);
+  planes_sqnorm_kernel<<<N, 256, 0, st>>>(x, D, hi, lo, sq, err);
   IBL_CUDA_OK(cudaGetLastError());
   return IBL_OK;
 }

@@ -5,8 +5,8 @@
 // fp32 anyway.  Here:
 //   1. rows_f16_kernel        one pass per matrix: fp16 plane of each row scaled by a power of two (row max in
 //                             [0.5,1): no overflow, 11 significant bits), exact fp32 |x|^2 (same summation order as
-//                             planes_sqnorm_kernel, so the exact distances below are unchanged), the 4-norm and
-//                             the max of each row (error model of the guard);
+//                             planes_sqnorm_kernel, so the exact distances below are unchanged) and the norm of
+//                             each row's rounding residual x - 2^e plane (error model of the guard);
 //   2. gemm_f16_top16_kernel  wgmma f16 (fp16 x fp16 -> fp32 in registers), ONE MMA per K step and 64-row
 //                             half, 128 queries x 128 database rows per tile, 5-stage TMA ring, running
 //                             top-16 per query in registers across the CTA's database range;
@@ -14,12 +14,15 @@
 //                             survivors (|q|^2 + |d|^2 - 2 q.d, bit-identical to round 1's rescore_sort_kernel),
 //                             final (dist, idx) sort, and the GUARD: a database row that was NOT kept has a
 //                             screened distance >= s16 (the 16th screened distance); its exact distance is
-//                             >= s16 - B, B = 8 sigma of the fp16 rounding error of one dot product (from the rows'
-//                             4-norms) + the absolute error of fp16 subnormals.  If s16 - B < (k-th exact distance)
-//                             the query is appended to a device-side list;
-//   4. dist_exact_chunk_kernel / dist_exact_merge_kernel   listed queries (none, in practice: the k-th to 16th gap
-//                             is ~50 B for descriptor-like data) are ranked again by exact fp32 brute force,
-//                             without any host round trip: the kernels size their work from the device counter.
+//                             >= s16 - B, B = d1_screen_bound: a rigorous bound of the operand rounding (the rows'
+//                             residual norms, Cauchy-Schwarz) + a statistical allowance for the tensor core's fp32
+//                             accumulation.  If s16 - B <= (k-th exact distance) the query is appended to a
+//                             device-side list;
+//   4. dist_exact_scan_kernel / dist_exact_finish_kernel   listed queries (about 0.1% of retrieval-like queries at
+//                             4096 dimensions, 10% at 32768, measured on synth.make_gallery) are ranked again by
+//                             exact fp32 brute force, without any host round trip: the kernels size their work from
+//                             the device counter, and one pass over the database serves every listed query.
+//   5. dist_guard_kernel      the same guard and fallback after the bf16x3 screening of tc_gemm.cu.
 #include <cuda_fp16.h>
 #include <stdlib.h>
 
@@ -31,49 +34,61 @@ namespace ibl {
 using namespace tc;
 
 // ---- 1. fp16 planes -----------------------------------------------------------------------------
-// aux[r] = {|x|^2 (exact fp32), 2^e (x = plane * 2^e), (sum x^4)^(1/4), max|x|}
+// aux[r] = {|x|^2 (exact fp32), 2^e (x = plane * 2^e), |x - 2^e plane| (the rounding residual), max|x|}
 __global__ void __launch_bounds__(256)
 rows_f16_kernel(const float* __restrict__ x, int D, __half* __restrict__ plane, float4* __restrict__ aux) {
-  __shared__ float red[8], red4[8], redm[8];
-  __shared__ float scale_s;
+  __shared__ float red[8], redm[8];
+  __shared__ float scale_s, sc_s, tot_s, m_s;
   const long long r = blockIdx.x;
   const float4* p = reinterpret_cast<const float4*>(x + r * D);
-  float ss = 0.f, s4 = 0.f, mx = 0.f;
+  float ss = 0.f, mx = 0.f;
   for (int i = threadIdx.x; i < D / 4; i += blockDim.x) {
     const float4 v = __ldg(p + i);
     ss = fmaf(v.x, v.x, ss); ss = fmaf(v.y, v.y, ss); ss = fmaf(v.z, v.z, ss); ss = fmaf(v.w, v.w, ss);
-    const float a = v.x * v.x, b = v.y * v.y, c = v.z * v.z, d = v.w * v.w;
-    s4 = fmaf(a, a, s4); s4 = fmaf(b, b, s4); s4 = fmaf(c, c, s4); s4 = fmaf(d, d, s4);
     mx = fmaxf(fmaxf(mx, fmaxf(fabsf(v.x), fabsf(v.y))), fmaxf(fabsf(v.z), fabsf(v.w)));
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
     ss += __shfl_xor_sync(0xffffffffu, ss, o);
-    s4 += __shfl_xor_sync(0xffffffffu, s4, o);
     mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
   }
-  if ((threadIdx.x & 31) == 0) { red[threadIdx.x >> 5] = ss; red4[threadIdx.x >> 5] = s4; redm[threadIdx.x >> 5] = mx; }
+  if ((threadIdx.x & 31) == 0) { red[threadIdx.x >> 5] = ss; redm[threadIdx.x >> 5] = mx; }
   __syncthreads();
   if (threadIdx.x == 0) {
-    float tot = 0.f, tot4 = 0.f, m = 0.f;
-    for (int i = 0; i < (int)(blockDim.x >> 5); ++i) { tot += red[i]; tot4 += red4[i]; m = fmaxf(m, redm[i]); }
+    float tot = 0.f, m = 0.f;
+    for (int i = 0; i < (int)(blockDim.x >> 5); ++i) { tot += red[i]; m = fmaxf(m, redm[i]); }
     int e = 0;
     if (m > 0.f && m < INFINITY) frexpf(m, &e);       // m = f * 2^e, f in [0.5, 1)
-    const float sc = ldexpf(1.f, e);
     scale_s = ldexpf(1.f, -e);
-    aux[r] = make_float4(tot, sc, sqrtf(sqrtf(tot4)), m);
+    sc_s = ldexpf(1.f, e);
+    tot_s = tot;
+    m_s = m;
   }
   __syncthreads();
-  const float inv = scale_s;
+  const float inv = scale_s, sc = sc_s;
   uint2* ph = reinterpret_cast<uint2*>(plane + r * D);
+  float rr = 0.f;                                      // |x - 2^e plane|^2: every element's rounding, subnormals included
   for (int i = threadIdx.x; i < D / 4; i += blockDim.x) {   // second read of the row: L1/L2 hits
     const float4 v = __ldg(p + i);
     const __half2 a = __floats2half2_rn(v.x * inv, v.y * inv), b = __floats2half2_rn(v.z * inv, v.w * inv);
     ph[i] = make_uint2(*reinterpret_cast<const uint32_t*>(&a), *reinterpret_cast<const uint32_t*>(&b));
+    const float2 fa = __half22float2(a), fb = __half22float2(b);
+    const float r0 = v.x - fa.x * sc, r1 = v.y - fa.y * sc, r2 = v.z - fb.x * sc, r3 = v.w - fb.y * sc;
+    rr = fmaf(r0, r0, rr); rr = fmaf(r1, r1, rr); rr = fmaf(r2, r2, rr); rr = fmaf(r3, r3, rr);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) rr += __shfl_xor_sync(0xffffffffu, rr, o);
+  __syncthreads();                                     // red[] is reused
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = rr;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float tr = 0.f;
+    for (int i = 0; i < (int)(blockDim.x >> 5); ++i) tr += red[i];
+    aux[r] = make_float4(tot_s, sc, sqrtf(tr), m_s);
   }
 }
 
-// max over the database rows of (4-norm, max|x|, |x|^2): the guard's bound for rows that were not kept
+// max over the database rows of (residual norm, max|x|, |x|^2): the guard's bound for rows that were not kept
 __global__ void dist_colmax_kernel(const float4* __restrict__ aux, int n, float* __restrict__ out3) {
   float a = 0.f, b = 0.f, c = 0.f;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
@@ -354,12 +369,27 @@ struct FinishArgs {
   int m, d, runs, k_out, n_valid;
   long long idx_base;
   float* out_dist; long long* out_idx;
-  int* flag_count; int* flag_list;
+  int* flag_count; int* flag_list; int* list_cnt;
 };
 
-// kappa = 8 standard deviations; rms relative rounding error of fp16 RN = 2^-11 * 0.41; two operands (sqrt 2);
-// distance = -2 dot (factor 2)  ->  8 * 2 * 1.414 * 0.41 * 2^-11
-#define D1_GUARD_C (8.f * 2.f * 1.41421356f * 0.41f * 4.8828125e-4f)
+// The guard's B: how far a screened distance can lie from |q|^2 + |d|^2 - 2 q.d (the same fp32 norms).  Write
+// x = op(x) + r, op = what the MMA reads (the scaled fp16 plane, or bf16 hi + lo with the lo.lo product dropped).
+//   operand rounding, rigorous (Cauchy-Schwarz, per pair, the database side by its maximum over the rows):
+//       |q.d - screened dot| <= |lo_q| |lo_d| + |q| |r_d| + |r_q| |d| + |r_q| |r_d|
+//   fp32 accumulation in the tensor core, STATISTICAL (modelled, not bounded): kappa = 8 sigma of a random walk of
+//       one 2^-24 rounding per accumulator update (one per MMA and 16-wide K step), relative to the product
+//       magnitudes (|q| + |lo_q| + |r_q|)(max|d| + max|lo_d| + max|r_d|);
+//   the epilogue's fma: 2^-23 (|q|^2 + max|d|^2); distance = -2 dot; (1 + d 2^-23) for the fp32 evaluation of B.
+// tests/test_host_screening.py mirrors this function and checks the operand part against emulated rounding.
+#define D1_ACC_KAPPA 8.f
+__device__ __forceinline__ float d1_screen_bound(float q_sq, float q_lo, float q_res, float db_sq_max, float db_lo_max,
+                                                 float db_res_max, int d, int mmas_per_k16) {
+  const float nq = sqrtf(q_sq), dm = sqrtf(db_sq_max);
+  const float dot = q_lo * db_lo_max + nq * db_res_max + q_res * dm + q_res * db_res_max;
+  const float acc = D1_ACC_KAPPA * 5.9604645e-8f * sqrtf((float)(d / 16) * mmas_per_k16) * (nq + q_lo + q_res) *
+                    (dm + db_lo_max + db_res_max);
+  return (2.f * (dot + acc) + 1.1920929e-7f * (q_sq + db_sq_max)) * (1.f + (float)d * 1.1920929e-7f);
+}
 
 __global__ void __launch_bounds__(128)
 dist_finish_kernel(const FinishArgs g) {
@@ -447,110 +477,208 @@ dist_finish_kernel(const FinishArgs g) {
     bool flag = (s16k == ~0ull) || (ek == ~0ull);        // cannot happen with n_valid > 16; be safe
     if (!flag) {
       const float s16 = d1_unord((uint32_t)(s16k >> 32)), e_k = d1_unord((uint32_t)(ek >> 32));
-      // statistical part: 8 sigma of the fp16 rounding error of one dot product (Cauchy-Schwarz on the 4-norms);
-      // absolute part: values below 2^-14 of the row max are fp16 subnormals, error <= 2^-24 * row max each:
-      // |dot error| <= 2^-24 sqrt(D) (dmax |q| + qmax |d|), distance = -2 dot
-      const float bound = D1_GUARD_C * qa.z * __ldg(g.db_max2) +
-                          2.f * 5.9604645e-8f * sqrtf((float)d) *
-                              (__ldg(g.db_max2 + 1) * sqrtf(qa.x) + qa.w * sqrtf(__ldg(g.db_max2 + 2)));
+      // fp16 operands: no lo plane, one MMA per K step; the residuals include the subnormals' rounding
+      const float bound = d1_screen_bound(qa.x, 0.f, qa.z, __ldg(g.db_max2 + 2), 0.f, __ldg(g.db_max2), d, 1);
       flag = !(s16 - bound > e_k);                       // also catches NaN
     }
-    if (flag) g.flag_list[atomicAdd(g.flag_count, 1)] = (int)row;
+    if (flag) {
+      const int f = atomicAdd(g.flag_count, 1);
+      g.flag_list[f] = (int)row;
+      g.list_cnt[f] = 0;
+    }
   }
 }
 
 // ---- 4. exact brute force for the listed queries ----------------------------------------------------
-constexpr int DX_CHUNK = 4096;    // database rows per work item
+// A listed query already has k re-scored rows at exact distances <= e_k, so its true top-k lies at exact distance
+// <= e_k.  One pass over the database scores every row against every listed query (the row stays in L1 across the
+// queries: the database is read once however many queries are listed) and appends the rows at <= e_k to the query's
+// list; a second kernel sorts each list.  A list that overflows (more than DX_CAP rows within e_k: heavy ties) is
+// ranked by a blockwise scan of the whole database instead.
+constexpr int DX_CAP = 256;       // listed rows per query
+// byte offset of the lists after the [m] list counters (the 8-byte keys need 8-byte alignment whatever m is)
+static size_t dx_lists_at(int m) { return ((size_t)m * 4 + 255) & ~(size_t)255; }
 
 struct ExactArgs {
   const float* q; const float* db;
-  const float4* q_aux; const float4* db_aux;
-  int m, d, n_valid, k, nchunks;
+  const float* q_sq; const float* db_sq;   // exact fp32 |x|^2 of every row, sq_stride floats apart
+  int sq_stride;
+  int m, d, n_valid, k;
   long long idx_base;
   const int* flag_count; const int* flag_list;
-  unsigned long long* scratch;   // [m][nchunks][16] keys
+  int* list_cnt;                 // [m] per listed query (zeroed by the guard that lists it)
+  unsigned long long* lists;     // [m][DX_CAP] (dist, row) keys
   float* out_dist; long long* out_idx;
 };
 
-// work item = (listed query f, chunk c): exact distances of DX_CHUNK rows, the 16 smallest keys to scratch
-__global__ void __launch_bounds__(256)
-dist_exact_chunk_kernel(const ExactArgs g) {
+// Listed queries in groups of up to DX_QG staged in shared memory; one warp per database row (grid-stride), the
+// row's float4 slices loaded once and multiplied into every staged query, in d1_exact's order (lane-strided FMAs,
+// xor-shuffle tree, the same final fma): the distances are bit-identical to the re-scored ones.
+constexpr int DX_QG = 8;
+constexpr int DX_QSMEM = 128 * 1024;      // staged query rows: min(DX_QG, 32768 / d) of them
+constexpr int DX_SCAN_WARPS = 16;
+__global__ void __launch_bounds__(DX_SCAN_WARPS * 32)
+dist_exact_scan_kernel(const ExactArgs g) {
   extern __shared__ __align__(16) float qs[];
-  __shared__ unsigned long long best[8][16];
   const int count = *g.flag_count;
-  const int items = count * g.nchunks;
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  const bool staged = g.d <= 16384;
-  for (int item = blockIdx.x; item < items; item += gridDim.x) {
-    const int f = item / g.nchunks, c = item - f * g.nchunks;
-    const long long row = g.flag_list[f];
+  if (count == 0) return;
+  const int lane = threadIdx.x & 31;
+  const int warps = gridDim.x * DX_SCAN_WARPS;
+  const int qg = min(DX_QG, max(1, (DX_QSMEM / 4) / g.d));
+  for (int f0 = 0; f0 < count; f0 += qg) {
+    const int nq = min(qg, count - f0);
     __syncthreads();
-    if (staged)
-      for (int i = threadIdx.x * 4; i < g.d; i += 256 * 4)
-        *reinterpret_cast<float4*>(qs + i) = __ldg(reinterpret_cast<const float4*>(g.q + row * g.d + i));
-    __syncthreads();
-    const float* qrow = staged ? qs : (g.q + row * g.d);
-    const float an = __ldg(&g.q_aux[row].x);
-    unsigned long long mine[16];               // this warp's 16 best (every lane holds the same list)
-#pragma unroll
-    for (int j = 0; j < 16; ++j) mine[j] = ~0ull;
-    const int j0 = c * DX_CHUNK, j1 = min(g.n_valid, j0 + DX_CHUNK);
-    for (int j = j0 + wid; j < j1; j += 8) {
-      const float dist = d1_exact(qrow, g.db + (long long)j * g.d, g.d, lane, an, __ldg(&g.db_aux[j].x));
-      unsigned long long key = ((unsigned long long)d1_ord(dist) << 32) | (unsigned)j;
-      if (key < mine[15]) {
-        mine[15] = key;
-#pragma unroll
-        for (int s = 15; s > 0; --s)
-          if (mine[s] < mine[s - 1]) { const unsigned long long t = mine[s]; mine[s] = mine[s - 1]; mine[s - 1] = t; }
-      }
+    for (int t = 0; t < nq; ++t) {
+      const float* src = g.q + (long long)g.flag_list[f0 + t] * g.d;
+      for (int i = threadIdx.x * 4; i < g.d; i += DX_SCAN_WARPS * 32 * 4)
+        *reinterpret_cast<float4*>(qs + t * g.d + i) = __ldg(reinterpret_cast<const float4*>(src + i));
     }
-    if (lane == 0)
-#pragma unroll
-      for (int j = 0; j < 16; ++j) best[wid][j] = mine[j];
     __syncthreads();
-    if (threadIdx.x == 0) {                    // 16 smallest of the 8 sorted lists (rare path: serial merge)
-      int head[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-      unsigned long long* out = g.scratch + ((long long)row * g.nchunks + c) * 16;
-      for (int t = 0; t < 16; ++t) {
-        int bw = 0;
-        unsigned long long bk = ~0ull;
-        for (int w = 0; w < 8; ++w)
-          if (head[w] < 16 && best[w][head[w]] < bk) { bk = best[w][head[w]]; bw = w; }
-        out[t] = bk;
-        if (bk != ~0ull) ++head[bw];
+    for (int j = blockIdx.x * DX_SCAN_WARPS + (threadIdx.x >> 5); j < g.n_valid; j += warps) {
+      const float* dp = g.db + (long long)j * g.d;
+      float acc[DX_QG];
+#pragma unroll
+      for (int t = 0; t < DX_QG; ++t) acc[t] = 0.f;
+#pragma unroll 2
+      for (int i = lane * 4; i < g.d; i += 128) {
+        const float4 b = __ldg(reinterpret_cast<const float4*>(dp + i));
+#pragma unroll
+        for (int t = 0; t < DX_QG; ++t) {
+          if (t < nq) {
+            const float4 a = *reinterpret_cast<const float4*>(qs + t * g.d + i);
+            acc[t] = fmaf(a.x, b.x, acc[t]); acc[t] = fmaf(a.y, b.y, acc[t]);
+            acc[t] = fmaf(a.z, b.z, acc[t]); acc[t] = fmaf(a.w, b.w, acc[t]);
+          }
+        }
+      }
+      const float bn = __ldg(g.db_sq + (long long)j * g.sq_stride);
+#pragma unroll
+      for (int t = 0; t < DX_QG; ++t) {
+        if (t < nq) {
+          float v = acc[t];
+#pragma unroll
+          for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+          const int f = f0 + t;
+          const long long row = g.flag_list[f];
+          const float dist = fmaf(-2.f, v, __ldg(g.q_sq + row * g.sq_stride) + bn);
+          if (lane == 0 && dist <= g.out_dist[row * g.k + g.k - 1]) {   // e_k of the re-scored list
+            const int at = atomicAdd(g.list_cnt + f, 1);
+            if (at < DX_CAP) g.lists[(long long)f * DX_CAP + at] = ((unsigned long long)d1_ord(dist) << 32) | (unsigned)j;
+          }
+        }
       }
     }
   }
 }
 
-// one block per listed query: merge its nchunks x 16 keys, write the final top-k over the guarded result
-__global__ void __launch_bounds__(128)
-dist_exact_merge_kernel(const ExactArgs g) {
+// the attribute is per device
+static int dx_scan_attr() {
+  static DeviceOnce done;
+  if (!done.done()) {
+    IBL_CUDA_OK(cudaFuncSetAttribute(dist_exact_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DX_QSMEM));
+    done.mark();
+  }
+  return IBL_OK;
+}
+
+static size_t dx_scan_smem(int d) { return (size_t)min(DX_QG, max(1, (DX_QSMEM / 4) / d)) * d * sizeof(float); }
+
+// 512 keys in shared memory, ascending (256 threads)
+__device__ __forceinline__ void dx_sort512(unsigned long long* keys) {
+  for (int size = 2; size <= 512; size <<= 1) {
+    for (int stride = size >> 1; stride > 0; stride >>= 1) {
+      __syncthreads();
+      const int i = threadIdx.x;
+      const int lo = 2 * i - (i & (stride - 1));
+      const int hi = lo + stride;
+      const bool up = ((lo & size) == 0);
+      const unsigned long long a = keys[lo], b = keys[hi];
+      if ((a > b) == up) { keys[lo] = b; keys[hi] = a; }
+    }
+  }
+  __syncthreads();
+}
+
+// one block per listed query: sort its list (or, on overflow, scan the database 256 rows at a time keeping the 256
+// best) and write the final top-k
+__global__ void __launch_bounds__(256)
+dist_exact_finish_kernel(const ExactArgs g) {
+  __shared__ unsigned long long keys[512];
   const int count = *g.flag_count;
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   for (int f = blockIdx.x; f < count; f += gridDim.x) {
     const long long row = g.flag_list[f];
-    const unsigned long long* src = g.scratch + row * g.nchunks * 16;
-    if (threadIdx.x == 0) {                    // rare path: a serial k-way selection is fine
-      unsigned long long prev = 0;
-      bool first = true;
-      for (int t = 0; t < g.k; ++t) {
-        unsigned long long bk = ~0ull;
-        for (int i = 0; i < g.nchunks * 16; ++i) {
-          const unsigned long long key = src[i];
-          if ((first || key > prev) && key < bk) bk = key;
+    const int cnt = g.list_cnt[f];
+    __syncthreads();
+    for (int i = threadIdx.x; i < 512; i += 256)
+      keys[i] = (cnt <= DX_CAP && i < cnt) ? g.lists[(long long)f * DX_CAP + i] : ~0ull;
+    __syncthreads();
+    if (cnt <= DX_CAP) {
+      dx_sort512(keys);
+    } else {
+      const float* qrow = g.q + row * g.d;
+      const float an = __ldg(g.q_sq + row * g.sq_stride);
+      for (int j0 = 0; j0 < g.n_valid; j0 += 256) {     // keys[0, 256): best so far; keys[256, 512): this chunk
+        for (int t = wid; t < 256; t += 8) {
+          const int j = j0 + t;
+          unsigned long long key = ~0ull;
+          if (j < g.n_valid) {
+            const float dist = d1_exact(qrow, g.db + (long long)j * g.d, g.d, lane, an,
+                                        __ldg(g.db_sq + (long long)j * g.sq_stride));
+            key = ((unsigned long long)d1_ord(dist) << 32) | (unsigned)j;
+          }
+          if (lane == 0) keys[256 + t] = key;
         }
-        if (bk == ~0ull) {
-          g.out_dist[row * g.k + t] = INFINITY;
-          g.out_idx[row * g.k + t] = -1;
-        } else {
-          g.out_dist[row * g.k + t] = d1_unord((uint32_t)(bk >> 32));
-          g.out_idx[row * g.k + t] = g.idx_base + (long long)(uint32_t)(bk & 0xffffffffu);
-        }
-        prev = bk;
-        first = false;
+        dx_sort512(keys);
       }
     }
+    if ((int)threadIdx.x < g.k) {
+      const unsigned long long key = keys[threadIdx.x];
+      g.out_dist[row * g.k + threadIdx.x] = key == ~0ull ? INFINITY : d1_unord((uint32_t)(key >> 32));
+      g.out_idx[row * g.k + threadIdx.x] = key == ~0ull ? -1 : g.idx_base + (long long)(uint32_t)(key & 0xffffffffu);
+    }
+  }
+}
+
+// ---- 5. guard + exact fallback for the bf16x3 screening paths (tc_gemm.cu) -----------------------------
+// max over the database rows of (|lo|, |x - hi - lo|, |x|^2)
+__global__ void dist_guard_colmax_kernel(const float2* __restrict__ err, const float* __restrict__ sq, int n,
+                                         float* __restrict__ out3) {
+  float a = 0.f, b = 0.f, c = 0.f;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const float2 v = __ldg(err + i);
+    a = fmaxf(a, v.x);
+    b = fmaxf(b, v.y);
+    c = fmaxf(c, __ldg(sq + i));
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    a = fmaxf(a, __shfl_xor_sync(0xffffffffu, a, o));
+    b = fmaxf(b, __shfl_xor_sync(0xffffffffu, b, o));
+    c = fmaxf(c, __shfl_xor_sync(0xffffffffu, c, o));
+  }
+  if ((threadIdx.x & 31) == 0) {     // non-negative floats order like their bit patterns
+    atomicMax(reinterpret_cast<int*>(out3), __float_as_int(a));
+    atomicMax(reinterpret_cast<int*>(out3) + 1, __float_as_int(b));
+    atomicMax(reinterpret_cast<int*>(out3) + 2, __float_as_int(c));
+  }
+}
+
+// one thread per query.  screened [m][kc]: the kc smallest screened distances, ascending; a row that is not among
+// them has a screened distance >= the last.  Same test as dist_finish_kernel's guard, with three MMAs per K step.
+__global__ void dist_guard_kernel(const float* __restrict__ screened, int kc, const float* __restrict__ q_sq,
+                                  const float2* __restrict__ q_err, const float* __restrict__ db_max3,
+                                  const float* __restrict__ out_dist, int k, int m, int d, int n_valid,
+                                  int* flag_count, int* flag_list, int* list_cnt) {
+  const int row = blockIdx.x * blockDim.x + threadIdx.x;
+  if (row >= m || n_valid <= kc) return;                // every valid row was re-scored
+  const float s = screened[(long long)row * kc + kc - 1], e_k = out_dist[(long long)row * k + k - 1];
+  const float2 qe = q_err[row];
+  const float bound = d1_screen_bound(q_sq[row], qe.x, qe.y, db_max3[2], db_max3[0], db_max3[1], d, 3);
+  if (!(s - bound > e_k)) {                             // also catches NaN
+    const int f = atomicAdd(flag_count, 1);
+    flag_list[f] = row;
+    list_cnt[f] = 0;
   }
 }
 
@@ -580,8 +708,7 @@ size_t dist1_workspace_bytes(int m, int n, int d, size_t* off /*[8]*/) {
   off[5] = take((size_t)m * 4 + (size_t)m * 4);     // guard list | shared gates
   off[6] = take((size_t)8 * m * 16 * 4);
   off[7] = take((size_t)8 * m * 16 * 4);
-  const int nchunks = cdiv(n > 0 ? n : 1, DX_CHUNK);
-  off[8] = take((size_t)m * nchunks * 16 * 8);
+  off[8] = take(dx_lists_at(m) + (size_t)m * DX_CAP * 8);   // list counters | lists of the exact fallback
   return o;
 }
 
@@ -602,7 +729,8 @@ int launch_dist_topk_1pass(const float* q, int m, const float* db, int n, int n_
   unsigned* gate = reinterpret_cast<unsigned*>(w + off[5] + (size_t)m * 4);
   float* cd = reinterpret_cast<float*>(w + off[6]);
   int* ci = reinterpret_cast<int*>(w + off[7]);
-  unsigned long long* scratch = reinterpret_cast<unsigned long long*>(w + off[8]);
+  int* lcnt = reinterpret_cast<int*>(w + off[8]);
+  unsigned long long* lists = reinterpret_cast<unsigned long long*>(w + off[8] + dx_lists_at(m));
 
   IBL_CUDA_OK(cudaMemsetAsync(w + off[4], 0, 32, s));
   IBL_CUDA_OK(cudaMemsetAsync(gate, 0xFF, (size_t)m * 4, s));      // orderable +max: no gate yet
@@ -633,7 +761,6 @@ int launch_dist_topk_1pass(const float* q, int m, const float* db, int n, int n_
   if (!attr_done.done()) {
     IBL_CUDA_OK(cudaFuncSetAttribute(gemm_f16_top16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, D1_SMEM));
     IBL_CUDA_OK(cudaFuncSetAttribute(dist_finish_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
-    IBL_CUDA_OK(cudaFuncSetAttribute(dist_exact_chunk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
     attr_done.mark();
   }
   const int sms = device_sm_count();
@@ -643,28 +770,63 @@ int launch_dist_topk_1pass(const float* q, int m, const float* db, int n, int n_
   FinishArgs f{};
   f.q = q; f.db = db; f.q_aux = qa; f.db_aux = da; f.db_max2 = dmax2; f.cand_d = cd; f.cand_i = ci;
   f.m = m; f.d = d; f.runs = g.items_per_mtile; f.k_out = k; f.n_valid = n_valid; f.idx_base = idx_base;
-  f.out_dist = out_dist; f.out_idx = out_idx; f.flag_count = fcount; f.flag_list = flist;
+  f.out_dist = out_dist; f.out_idx = out_idx; f.flag_count = fcount; f.flag_list = flist; f.list_cnt = lcnt;
   const size_t qsm = d <= 16384 ? (size_t)d * sizeof(float) : 16;
   dist_finish_kernel<<<m, 128, qsm, s>>>(f);
   IBL_CUDA_OK(cudaGetLastError());
 
   ExactArgs x{};
-  x.q = q; x.db = db; x.q_aux = qa; x.db_aux = da; x.m = m; x.d = d; x.n_valid = n_valid; x.k = k;
-  x.nchunks = cdiv(n_valid, DX_CHUNK); x.idx_base = idx_base; x.flag_count = fcount; x.flag_list = flist;
-  x.scratch = scratch; x.out_dist = out_dist; x.out_idx = out_idx;
-  dist_exact_chunk_kernel<<<device_sm_count() * 2, 256, qsm, s>>>(x);     // exits at once when nothing is listed
-  dist_exact_merge_kernel<<<32, 128, 0, s>>>(x);
+  x.q = q; x.db = db; x.q_sq = reinterpret_cast<const float*>(qa); x.db_sq = reinterpret_cast<const float*>(da);
+  x.sq_stride = 4; x.m = m; x.d = d; x.n_valid = n_valid; x.k = k;
+  x.idx_base = idx_base; x.flag_count = fcount; x.flag_list = flist; x.list_cnt = lcnt; x.lists = lists;
+  x.out_dist = out_dist; x.out_idx = out_idx;
+  IBL_RET(dx_scan_attr());
+  dist_exact_scan_kernel<<<device_sm_count(), DX_SCAN_WARPS * 32, dx_scan_smem(d), s>>>(x);   // exits at once when nothing is listed
+  dist_exact_finish_kernel<<<64, 256, 0, s>>>(x);
   IBL_CUDA_OK(cudaGetLastError());
   if (launches) *launches += 7;
   return IBL_OK;
 }
 
-// test hook: number of queries the guard listed in the last call on this workspace (synchronises)
-int dist1_last_flag_count(void* ws, int m, int n, int d, int* out, cudaStream_t s) {
+// the guard's counter of listed queries in this workspace (test hook ibl_debug_dist_flagged)
+const int* dist1_flag_counter(const void* ws, int m, int n, int d) {
   size_t off[9];
   dist1_workspace_bytes(m, n, d, off);
-  IBL_CUDA_OK(cudaMemcpyAsync(out, reinterpret_cast<uint8_t*>(ws) + off[4] + 16, sizeof(int), cudaMemcpyDeviceToHost, s));
-  IBL_CUDA_OK(cudaStreamSynchronize(s));
+  return reinterpret_cast<const int*>(reinterpret_cast<const uint8_t*>(ws) + off[4] + 16);
+}
+
+// layout: flag count, database maxima (256 B) | flag list [m], list counters [m] | lists [m][DX_CAP] keys
+static size_t guard_lists_at(int m) { return 256 + (((size_t)m * 8 + 255) & ~(size_t)255); }
+size_t dist_guard_workspace_bytes(int m) { return guard_lists_at(m) + (size_t)m * DX_CAP * 8; }
+
+// Guard + exact fallback after a bf16x3 screening pass and its exact re-scoring (out_dist / out_idx hold the
+// re-scored top-k).  screened [m][kc]: the kc candidates' screened distances, ascending.  q_err / db_err per row:
+// {|lo|, |x - hi - lo|} (planes_sqnorm_kernel).  ws: dist_guard_workspace_bytes(m); its first int
+// counts the listed queries.
+int launch_dist_guard_bf16x3(const float* q, const float* q_sq, const float2* q_err, int m, const float* db,
+                             const float* db_sq, const float2* db_err, int n_valid, int d, const float* screened, int kc,
+                             int k, long long idx_base, void* ws, float* out_dist, long long* out_idx,
+                             uint64_t* launches, cudaStream_t s) {
+  IBL_REQUIRE(n_valid >= 1 && k >= 1 && k <= 128 && kc >= k, "bf16x3 guard: 1 <= k <= kc, k <= 128");
+  uint8_t* w = reinterpret_cast<uint8_t*>(ws);
+  int* fcount = reinterpret_cast<int*>(w);
+  float* dmax3 = reinterpret_cast<float*>(w + 16);
+  int* flist = reinterpret_cast<int*>(w + 256);
+  int* lcnt = flist + m;
+  unsigned long long* lists = reinterpret_cast<unsigned long long*>(w + guard_lists_at(m));
+  IBL_CUDA_OK(cudaMemsetAsync(w, 0, 32, s));
+  dist_guard_colmax_kernel<<<cdiv(n_valid, 256) < 64 ? cdiv(n_valid, 256) : 64, 256, 0, s>>>(db_err, db_sq, n_valid, dmax3);
+  dist_guard_kernel<<<cdiv(m, 128), 128, 0, s>>>(screened, kc, q_sq, q_err, dmax3, out_dist, k, m, d, n_valid, fcount,
+                                                flist, lcnt);
+  ExactArgs x{};
+  x.q = q; x.db = db; x.q_sq = q_sq; x.db_sq = db_sq; x.sq_stride = 1; x.m = m; x.d = d; x.n_valid = n_valid; x.k = k;
+  x.idx_base = idx_base; x.flag_count = fcount; x.flag_list = flist; x.list_cnt = lcnt; x.lists = lists;
+  x.out_dist = out_dist; x.out_idx = out_idx;
+  IBL_RET(dx_scan_attr());
+  dist_exact_scan_kernel<<<device_sm_count(), DX_SCAN_WARPS * 32, dx_scan_smem(d), s>>>(x);   // exits at once when nothing is listed
+  dist_exact_finish_kernel<<<64, 256, 0, s>>>(x);
+  IBL_CUDA_OK(cudaGetLastError());
+  if (launches) *launches += 4;
   return IBL_OK;
 }
 

@@ -408,9 +408,16 @@ class Engine:
         return out_dist_host, out_idx_host
 
     def dist_flagged(self) -> int:
-        """Queries re-ranked by exact brute force in the last l2dist_topk call (-1: single-pass path not taken)."""
+        """Queries re-ranked by exact brute force in the last l2dist_topk call (-1: it took the exact fp32 path)."""
         c = c_int()
         check(self.lib.ibl_debug_dist_flagged(self.h, byref(c), _stream(self.device)), "ibl_debug_dist_flagged")
+        return c.value
+
+    def dist_path(self) -> int:
+        """Ranking path of the last l2dist_topk call: 0 exact fp32, 1 single-pass fp16 screening, 2 bf16x3 top-16
+        screening, 3 bf16x3 dense screening (-1: no call yet)."""
+        c = c_int()
+        check(self.lib.ibl_debug_dist_path(self.h, byref(c)), "ibl_debug_dist_path")
         return c.value
 
     def gemm_nt(self, a: torch.Tensor, b: torch.Tensor, alpha: float = 1.0, mode: int = CONV_SIMT_FP32) -> torch.Tensor:

@@ -23,6 +23,8 @@ VARIANTS = [
     ({"IBL_DIST_SCREEN": "3", "IBL_DIST_2SM": "0"}, "retrieval_vs_reference or topk"),   # ... on one SM
     ({"IBL_DIST_SCREEN": "3", "IBL_DIST_2SM": "0", "IBL_DIST_BN": "128", "IBL_GEMM_MC": "1"}, "retrieval_vs_reference or topk"),
 ]
+# the distance-screening variants also run the whole exact-ranking suite
+RANKING_ENVS = {"IBL_DIST_SCREEN", "IBL_DIST_2SM"}
 
 
 @pytest.mark.gpu
@@ -30,9 +32,12 @@ VARIANTS = [
 def test_variant_matches_references(env, expr):
     child_env = dict(os.environ)
     child_env.update(env)
-    r = subprocess.run([sys.executable, "-m", "pytest", os.path.join(ROOT, "tests", "test_gpu_parity.py"), "-q", "-x",
-                        "-k", expr, "-p", "no:cacheprovider"], cwd=ROOT, env=child_env, capture_output=True, text=True,
-                       timeout=600)
+    files = [os.path.join(ROOT, "tests", "test_gpu_parity.py")]
+    if RANKING_ENVS & set(env):
+        files.append(os.path.join(ROOT, "tests", "test_gpu_ranking.py"))
+        expr = f"({expr}) or test_gpu_ranking.py"
+    r = subprocess.run([sys.executable, "-m", "pytest", *files, "-q", "-x", "-k", expr, "-p", "no:cacheprovider"],
+                       cwd=ROOT, env=child_env, capture_output=True, text=True, timeout=600)
     tail = (r.stdout + r.stderr)[-2000:]
     assert r.returncode == 0, tail
     assert " passed" in r.stdout and "failed" not in r.stdout, tail

@@ -65,6 +65,7 @@ def main():
     ap.add_argument("--rerank", action="store_true", help="k-reciprocal re-ranking, as examples/test.py --rerank")
     ap.add_argument("--rr-topk", type=int, default=25)
     ap.add_argument("--lambda-value", type=float, default=0.0)
+    ap.add_argument("--nms", action="store_true", help="spatial NMS on the ranking, as examples/test.py --nms")
     args = ap.parse_args()
 
     init_dist(args.launcher, args)                        # one process per GPU, NCCL
@@ -92,7 +93,8 @@ def main():
     dataset = sorted(list(set(ds.q_test) | set(ds.db_test)))
     recalls = evaluator.evaluate(loader(ds.q_test), dataset, ds.q_test, ds.db_test, ds.test_pos,
                                  gallery_loader=loader(ds.db_test), vlad=True, pca=None, gpu=args.gpu,
-                                 rerank=args.rerank, rr_topk=args.rr_topk, lambda_value=args.lambda_value)
+                                 rerank=args.rerank, rr_topk=args.rr_topk, lambda_value=args.lambda_value,
+                                 nms=args.nms)
     synchronize()
     if args.rank == 0:
         print("RECALLS " + ",".join("%.6f" % r for r in recalls))

@@ -215,6 +215,28 @@ int ibl_topk_merge(ibl_engine* e, const float* cand_dist, const int64_t* cand_id
 int ibl_l2dist_topk_host(ibl_engine* e, const float* q_host, int m, const float* db_host, int n,
                          int d, int k, float* out_dist_host, int64_t* out_idx_host, void* stream);
 
+/* ---- k-reciprocal re-ranking (reference ibl/utils/rerank.py:37-100, used by
+ * Evaluator.evaluate(rerank=True), ibl/evaluators.py:194-199) ------------------------------------------------
+ * Rows of X [N,d] are the queries followed by the gallery.  d(i,j) = |x_i|^2 + |x_j|^2 - 2 x_i.x_j in exact fp32;
+ * the reference ranks and weighs by d^2 (rerank.py:42), normalised per row by M_i = max_j d(i,j)^2.
+ * Neighbour pass, for rows row0 .. row0+n_rows-1 (one slice per rank): out_idx [n_rows,w] = the first w columns
+ * ascending by (d^2, index), out_dist [n_rows,w] their exact distances d (not squared), out_rowmax [n_rows] = M_i.
+ * Screening on the tensor cores, every listed value re-scored in exact fp32; rows whose screened lists cannot be
+ * shown exact are ranked by an exact scan.  1 <= w <= min(128, N). */
+int ibl_knn_rowmax(ibl_engine* e, const float* X, int N, int d, int row0, int n_rows, int w, int64_t* out_idx,
+                   float* out_dist, float* out_rowmax, void* stream);
+/* Sparse stage: from the [N,w] lists and M of ALL rows (ibl_knn_rowmax over 0..N-1, possibly gathered from several
+ * ranks), the k-reciprocal sets and their expansion (k1, rerank.py:51-68), V (rerank.py:69-70), the mean over the
+ * first k2 neighbours (rerank.py:71-76) and the Jaccard distance (rerank.py:78-93) -> for each of the m queries the
+ * top k gallery rows ascending by (final, index): out_dist [m,k] = final = (1-lambda) jac + lambda d^2/M,
+ * out_idx [m,k] gallery indices 0..N-m-1.  With lambda > 0, orig_idx [m,k_orig] (min(k, N-m) <= k_orig <= 256) is the
+ * original ranking of each query over the gallery (ibl_l2dist_topk); with lambda = 0 it is not read.  Needs
+ * k1 + 1 <= w <= 128, N >= k1 + 1, 1 <= k2 <= w, 1 <= k <= 128.  Synchronises the stream three to five times to size
+ * its sparse matrices; no [m,n] or [N,N] array is allocated. */
+int ibl_rerank_topk(ibl_engine* e, const float* X, int N, int m, int d, const int64_t* nbr_idx, const float* nbr_dist,
+                    int w, const float* rowmax, int k1, int k2, float lambda_value, const int64_t* orig_idx, int k_orig,
+                    int k, float* out_dist, int64_t* out_idx, void* stream);
+
 /* C[m,n] = alpha * A[m,k] . B[n,k]^T on the engine's GEMM kernels: the products of PCA.train (pca.py:38-67,
  * torch.matmul there).  mode IBL_CONV_SIMT_FP32 (fp32 CUDA cores) or IBL_CONV_TC_BF16X3 (tensor cores, k % 64 == 0). */
 int ibl_gemm_nt(ibl_engine* e, const float* A, int m, const float* B, int n, int k, float alpha, float* C, int mode,
@@ -227,6 +249,11 @@ int ibl_debug_dist_flagged(ibl_engine* e, int* count, void* stream);
 /* Ranking path of the last ibl_l2dist_topk call: 0 exact fp32 CUDA cores, 1 single-pass fp16 screening,
  * 2 bf16x3 screening with a running top-16, 3 bf16x3 dense tiles + row select (-1: no call yet). */
 int ibl_debug_dist_path(ibl_engine* e, int* path);
+/* Rows of the last ibl_knn_rowmax call that its guards sent to the exact scan of all N columns (-1: no call yet).
+ * Synchronises. */
+int ibl_debug_knn_flagged(ibl_engine* e, int* count, void* stream);
+/* Device memory (bytes) held by the re-ranking workspaces of e (ibl_knn_rowmax + ibl_rerank_topk). */
+int ibl_debug_rerank_workspace_bytes(ibl_engine* e, uint64_t* bytes);
 /* Runs the wgmma/TMA building blocks against CUDA-core results on the device;
  * returns IBL_OK when all agree. max_rel_err (may be NULL) receives the worst error. */
 int ibl_selftest_tc(ibl_engine* e, float* max_rel_err);

@@ -57,6 +57,11 @@ SIGNATURES = {
     "ibl_argsort_rows": (c_int, [_P, _P, c_int, c_int, _P, _P]),
     "ibl_topk_merge": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, _P, _P, _P]),
     "ibl_l2dist_topk_host": (c_int, [_P, _P, c_int, _P, c_int, c_int, c_int, _P, _P, _P]),
+    "ibl_knn_rowmax": (c_int, [_P, _P, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P]),
+    "ibl_rerank_topk": (c_int, [_P, _P, c_int, c_int, c_int, _P, _P, c_int, _P, c_int, c_int, c_float, _P, c_int,
+                                c_int, _P, _P, _P]),
+    "ibl_debug_rerank_workspace_bytes": (c_int, [_P, POINTER(c_uint64)]),
+    "ibl_debug_knn_flagged": (c_int, [_P, POINTER(c_int), _P]),
     "ibl_gemm_nt": (c_int, [_P, _P, c_int, _P, c_int, c_int, c_float, _P, c_int, _P]),
     "ibl_debug_dist_flagged": (c_int, [_P, POINTER(c_int), _P]),
     "ibl_debug_dist_path": (c_int, [_P, POINTER(c_int)]),

@@ -202,6 +202,19 @@ int launch_planes_sqnorm(const float* x, int N, int D, __nv_bfloat16* hi, __nv_b
 int launch_l2dist_dense(const float* q, const float* qn, int m, const float* db, const float* dbn,
                         int n, int d, float* out, long long ld_out, cudaStream_t s);
 
+// rerank.cu  (k-reciprocal re-ranking: exact neighbour pass + sparse stage)
+size_t knn_rowmax_workspace_bytes(int N, int d, int n_rows, int w);
+const int* knn_rowmax_flag_counter(const void* ws, int N, int d, int n_rows, int w);
+int launch_knn_rowmax(const float* X, int N, int d, int row0, int n_rows, int w, void* ws, long long* out_idx,
+                      float* out_dist, float* out_max, uint64_t* launches, cudaStream_t s);
+struct RerankWs;
+RerankWs* rerank_ws_create();
+void rerank_ws_destroy(RerankWs* w);
+size_t rerank_ws_bytes(const RerankWs* w);
+int launch_rerank_topk(RerankWs* W, const float* X, int N, int m, int d, const long long* nbr, const float* nbr_dist,
+                       int w, const float* rowmax, int k1, int k2, float lam, const long long* orig, int k_orig, int k,
+                       float* out_dist, long long* out_idx, uint64_t* launches, cudaStream_t s);
+
 // topk.cu
 int launch_topk_rows(const float* dist, long long ld, int m, int n_valid, int k, int64_t idx_base,
                      float* out_dist, int64_t* out_idx, bool accumulate, cudaStream_t s);

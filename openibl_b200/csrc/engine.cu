@@ -82,6 +82,9 @@ struct ibl_engine {
   DevBuf bw_g, bw_x, bw_part, bw_w;      // conv backward: dY planes, X planes, wgrad/bias partials, dgrad filter planes
   DevBuf d1_ws;                          // workspace of the single-pass distance/top-k path (tc_dist1.cu)
   DevBuf q_err, db_err, guard_ws;        // guard of the bf16x3 screening paths: per-row error norms, workspace
+  DevBuf knn_ws;                         // neighbour pass of the re-ranking (rerank.cu)
+  const int* knn_flag_counter = nullptr; // its count of rows sent to the exact scan (null: no call yet)
+  RerankWs* rr_ws = nullptr;             // sparse stage of the re-ranking: CSR matrices, inverted index, pair buffers
   const int* flag_counter = nullptr;     // guard counter of the last ibl_l2dist_topk call (null: no guard on its path)
   int dist_path = -1;                    // ranking path of the last ibl_l2dist_topk call (ibl_debug_dist_path)
   DevBuf ssq, nv_part, nv_asum, nvw_pl;  // fused NetVLAD: |x|^2 partials, unit partials, W planes [64,512]
@@ -277,6 +280,8 @@ int ibl_engine_destroy(ibl_engine* e) {
                     &e->stage_in, &e->stage_out, &e->stage_out2, &e->stage_u8, &e->q_pl, &e->db_pl, &e->v_pl, &e->pca_pl,
                     &e->mrg_d, &e->mrg_i, &e->d1_ws, &e->bw_g, &e->bw_x, &e->bw_part, &e->bw_w, &e->ssq, &e->nv_part, &e->nv_asum, &e->nvw_pl, &e->nv_ticket};
   for (DevBuf* b : bufs) b->release();
+  e->knn_ws.release();
+  rerank_ws_destroy(e->rr_ws);
   delete e;
   return IBL_OK;
 }
@@ -1104,6 +1109,63 @@ int ibl_topk_merge(ibl_engine* e, const float* cand_dist, const int64_t* cand_id
   DeviceGuard g(e->device);
   e->launches++;
   return launch_topk_merge(cand_dist, cand_idx, parts, m, k_in, k_out, out_dist, out_idx, S(stream));
+}
+
+// k-reciprocal re-ranking, neighbour pass (reference ibl/utils/rerank.py:42-45, the rows' argsort and column max)
+int ibl_knn_rowmax(ibl_engine* e, const float* X, int N, int d, int row0, int n_rows, int w, int64_t* out_idx,
+                   float* out_dist, float* out_rowmax, void* stream) {
+  IBL_REQUIRE(e && X, "null argument");
+  IBL_REQUIRE(N >= 1 && d >= 1, "bad shape");
+  IBL_REQUIRE(w >= 1 && w <= 128, "knn_rowmax: 1 <= w <= 128");
+  IBL_REQUIRE(w <= N, "knn_rowmax: w <= N");
+  IBL_REQUIRE(row0 >= 0 && n_rows >= 0 && (long long)row0 + n_rows <= N, "knn_rowmax: rows out of range");
+  if (n_rows == 0) return IBL_OK;
+  IBL_REQUIRE(out_idx && out_dist && out_rowmax, "null argument");
+  DeviceGuard g(e->device);
+  IBL_RET(e->knn_ws.ensure(knn_rowmax_workspace_bytes(N, d, n_rows, w)));
+  e->knn_flag_counter = knn_rowmax_flag_counter(e->knn_ws.p, N, d, n_rows, w);
+  return launch_knn_rowmax(X, N, d, row0, n_rows, w, e->knn_ws.p, reinterpret_cast<long long*>(out_idx), out_dist,
+                           out_rowmax, &e->launches, S(stream));
+}
+
+// k-reciprocal re-ranking, sparse stage (reference ibl/utils/rerank.py:46-100)
+int ibl_rerank_topk(ibl_engine* e, const float* X, int N, int m, int d, const int64_t* nbr_idx, const float* nbr_dist,
+                    int w, const float* rowmax, int k1, int k2, float lambda_value, const int64_t* orig_idx, int k_orig,
+                    int k, float* out_dist, int64_t* out_idx, void* stream) {
+  IBL_REQUIRE(e && X && nbr_idx && nbr_dist && rowmax && out_dist && out_idx, "null argument");
+  IBL_REQUIRE(N >= 1 && d >= 1 && m >= 1 && m < N, "bad shape (1 <= m < N)");
+  IBL_REQUIRE(k1 >= 0 && k1 + 1 <= w && w <= 128, "re-ranking: k1 + 1 <= w <= 128");
+  IBL_REQUIRE(N >= k1 + 1, "re-ranking needs at least k1 + 1 images");
+  IBL_REQUIRE(k2 >= 1 && k2 <= w, "re-ranking: 1 <= k2 <= w");
+  IBL_REQUIRE(k >= 1 && k <= 128, "re-ranking: 1 <= k <= 128");
+  IBL_REQUIRE(lambda_value >= 0.f && lambda_value <= 1.f, "re-ranking: 0 <= lambda <= 1");
+  IBL_REQUIRE(lambda_value == 0.f || (orig_idx && k_orig >= (k < N - m ? k : N - m) && k_orig <= 256),
+              "re-ranking with lambda > 0 needs the original ranking, min(k, N - m) <= k_orig <= 256");
+  DeviceGuard g(e->device);
+  if (!e->rr_ws) e->rr_ws = rerank_ws_create();
+  return launch_rerank_topk(e->rr_ws, X, N, m, d, reinterpret_cast<const long long*>(nbr_idx), nbr_dist, w, rowmax,
+                            k1, k2, lambda_value, reinterpret_cast<const long long*>(orig_idx),
+                            lambda_value == 0.f ? 0 : k_orig, k, out_dist, reinterpret_cast<long long*>(out_idx),
+                            &e->launches, S(stream));
+}
+
+// test hook: rows of the last ibl_knn_rowmax call that the guards sent to the exact scan (-1: no call yet).
+// Synchronises the stream.
+int ibl_debug_knn_flagged(ibl_engine* e, int* count, void* stream) {
+  IBL_REQUIRE(e && count, "null argument");
+  *count = -1;
+  if (!e->knn_flag_counter) return IBL_OK;
+  DeviceGuard g(e->device);
+  IBL_CUDA_OK(cudaMemcpyAsync(count, e->knn_flag_counter, sizeof(int), cudaMemcpyDeviceToHost, S(stream)));
+  IBL_CUDA_OK(cudaStreamSynchronize(S(stream)));
+  return IBL_OK;
+}
+
+// test hook: device memory the re-ranking workspaces of `e` hold now
+int ibl_debug_rerank_workspace_bytes(ibl_engine* e, uint64_t* bytes) {
+  IBL_REQUIRE(e && bytes, "null argument");
+  *bytes = e->knn_ws.cap + (e->rr_ws ? rerank_ws_bytes(e->rr_ws) : 0);
+  return IBL_OK;
 }
 
 int ibl_l2dist_topk_host(ibl_engine* e, const float* q_host, int m, const float* db_host, int n, int d,

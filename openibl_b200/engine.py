@@ -398,6 +398,56 @@ class Engine:
                                       _ptr(od), _ptr(oi), _stream(self.device)), "ibl_topk_merge")
         return od, oi
 
+    def knn_rowmax(self, x: torch.Tensor, w: int, row0: int = 0, n_rows: Optional[int] = None):
+        """Neighbour pass of k-reciprocal re-ranking over the rows x[row0:row0+n_rows] against all of x [N,d]:
+        -> (idx [n_rows,w] int64, exact distances [n_rows,w], row maximum of d^2 [n_rows]).  The lists are
+        ascending by (d^2, index), as the reference ranks the squared distances (rerank.py:42-45)."""
+        x = _require_cuda(x, "descriptors")
+        N, d = x.shape
+        if n_rows is None:
+            n_rows = N - row0
+        oi = torch.empty(n_rows, w, dtype=torch.int64, device=x.device)
+        od = torch.empty(n_rows, w, device=x.device)
+        om = torch.empty(n_rows, device=x.device)
+        check(self.lib.ibl_knn_rowmax(self.h, _ptr(x), N, d, int(row0), int(n_rows), int(w), _ptr(oi), _ptr(od),
+                                      _ptr(om), _stream(self.device)), "ibl_knn_rowmax")
+        return oi, od, om
+
+    def rerank_topk(self, x: torch.Tensor, m: int, nbr_idx: torch.Tensor, nbr_dist: torch.Tensor,
+                    rowmax: torch.Tensor, k1: int, k2: int, lambda_value: float, k: int,
+                    orig_idx: Optional[torch.Tensor] = None):
+        """Sparse stage of k-reciprocal re-ranking (rerank.py:46-100): x [N,d] = queries then gallery, the [N,w]
+        neighbour lists and row maxima of knn_rowmax over all N rows -> (final [m,k], gallery index [m,k])."""
+        x = _require_cuda(x, "descriptors")
+        nbr_idx = _require_cuda(nbr_idx, "neighbour lists", torch.int64)
+        nbr_dist = _require_cuda(nbr_dist, "neighbour distances")
+        rowmax = _require_cuda(rowmax, "row maxima")
+        N, d = x.shape
+        w = nbr_idx.shape[1]
+        k_orig = 0
+        if orig_idx is not None:
+            orig_idx = _require_cuda(orig_idx, "original ranking", torch.int64)
+            k_orig = orig_idx.shape[1]
+        od = torch.empty(m, k, device=x.device)
+        oi = torch.empty(m, k, dtype=torch.int64, device=x.device)
+        check(self.lib.ibl_rerank_topk(self.h, _ptr(x), N, int(m), d, _ptr(nbr_idx), _ptr(nbr_dist), int(w),
+                                       _ptr(rowmax), int(k1), int(k2), c_float(lambda_value), _ptr(orig_idx),
+                                       int(k_orig), int(k), _ptr(od), _ptr(oi), _stream(self.device)),
+              "ibl_rerank_topk")
+        return od, oi
+
+    def knn_flagged(self) -> int:
+        """Rows of the last knn_rowmax call that the guards sent to the exact scan (-1: no call yet)."""
+        c = c_int()
+        check(self.lib.ibl_debug_knn_flagged(self.h, byref(c), _stream(self.device)), "ibl_debug_knn_flagged")
+        return c.value
+
+    def rerank_workspace_bytes(self) -> int:
+        """Device memory held by this engine's re-ranking workspaces."""
+        c = c_uint64()
+        check(self.lib.ibl_debug_rerank_workspace_bytes(self.h, byref(c)), "ibl_debug_rerank_workspace_bytes")
+        return c.value
+
     def l2dist_topk_host(self, q_host: torch.Tensor, db_host: torch.Tensor, k: int,
                          out_dist_host: torch.Tensor, out_idx_host: torch.Tensor):
         m, d = q_host.shape

@@ -23,7 +23,7 @@ from .engine import Engine
 from .utils.data.sampler import slice_bounds
 
 __all__ = ["extract_cnn_feature", "extract_features", "pairwise_distance", "spatial_nms",
-           "evaluate_all", "recalls_from_topk", "sharded_topk", "Evaluator"]
+           "evaluate_all", "recalls_from_topk", "sharded_topk", "sharded_rerank_topk", "Evaluator"]
 
 
 def _rank_world():
@@ -220,6 +220,64 @@ def sharded_topk(q: torch.Tensor, db_shard: torch.Tensor, k: int, idx_base: int,
     return _merge_fn(gd, gi, k)
 
 
+def sharded_rerank_topk(x: torch.Tensor, shard: torch.Tensor, k: int, idx_base: int, n_valid: int, k1: int = 20,
+                        k2: int = 6, lambda_value: float = 0.3):
+    """k-reciprocal re-ranking (rerank.py:32-100) of all queries against the sharded gallery, top k only.
+
+    X = [queries; gallery] is assembled on every rank (the gallery takes one device all-gather); each rank runs the
+    neighbour pass (first max(k1+1, k2) neighbours by squared distance, exact row maxima) for its slice of the N rows;
+    the packed lists (int32 index, fp32 distance bits, and the row maximum: 8 w + 4 bytes per row) take one
+    all-gather; rank 0 runs the sparse stage.  Returns (final [m,k], gallery index [m,k]) on rank 0 and None on the
+    other ranks.  Nothing of size [m,n] or [N,N] is built, and the result does not depend on the world size."""
+    rank, world = _rank_world()
+    m = x.shape[0]
+    n = int(n_valid)
+    if world > 1:
+        t = torch.tensor([n], dtype=torch.int64, device=x.device)
+        dist.all_reduce(t)
+        n = int(t.item())
+    N = m + n
+    w = max(k1 + 1, k2)
+    if N < k1 + 1:
+        raise ValueError("re-ranking needs at least k1 + 1 images")
+    if k1 < 0 or k2 < 1 or w > 128:
+        raise ValueError(f"re-ranking supports 0 <= k1 <= 127 and 1 <= k2 <= 128 (k1={k1}, k2={k2})")
+    if not 1 <= k <= 128:
+        raise ValueError(f"re-ranking keeps 1 <= k <= 128 ranks per query (k={k})")
+    if not 0.0 <= lambda_value <= 1.0:
+        raise ValueError(f"lambda_value must lie in [0, 1] (got {lambda_value})")
+    if int(idx_base) != slice_bounds(n, world, rank)[0]:
+        raise ValueError(f"sharded_rerank_topk expects rank {rank}'s gallery shard to be its slice_bounds slice "
+                         f"(first row {slice_bounds(n, world, rank)[0]}, got idx_base {idx_base})")
+    eng = Engine.get(x.device)
+    if world == 1:
+        y = shard[:n]
+    else:
+        _, _, per_g = slice_bounds(n, world, rank)
+        y = _all_gather_rows(shard[:min(per_g, shard.shape[0])], per_g)[:n]
+    X = torch.cat([x, y]).float().contiguous()
+    lo, cnt, per = slice_bounds(N, world, rank)
+    idx, dd, mx = eng.knn_rowmax(X, w, lo, cnt)
+    if world > 1:
+        packed = torch.zeros(per, 2 * w + 1, dtype=torch.int32, device=x.device)
+        packed[:cnt, :w] = idx.to(torch.int32)
+        packed[:cnt, w:2 * w] = dd.view(torch.int32)
+        packed[:cnt, 2 * w] = mx.view(torch.int32)
+        gathered = torch.empty(world * per, 2 * w + 1, dtype=torch.int32, device=x.device)
+        dist.all_gather_into_tensor(gathered, packed)      # rank-major: row r*per + i is global row r*per + i
+        if rank != 0:
+            return None
+        g = gathered[:N]
+        idx = g[:, :w].to(torch.int64).contiguous()
+        dd = g[:, w:2 * w].contiguous().view(torch.float32)
+        mx = g[:, 2 * w].contiguous().view(torch.float32)
+    orig = None
+    if lambda_value > 0:
+        # the first k rows of each query's original ranking can precede the rows without overlap (jac = 1)
+        _, orig = eng.l2dist_topk(x.float().contiguous(), y.float().contiguous(), min(k + 8, 128, n))
+    return eng.rerank_topk(X, m, idx, dd, mx, k1, k2, lambda_value, k, orig)
+
+
 def _slice_names(items, world, rank):
     """File names DistributedSliceSampler(items) hands to `rank` (sampler.py:208-219): a contiguous slice of
     ceil(n/world) items whose tail wraps to the head."""
@@ -289,7 +347,6 @@ class Evaluator(object):
             lo, cnt, per = slice_bounds(len(gallery), world, rank)
             shard = torch.stack([features[f] for f, _, _, _ in gallery[lo:lo + cnt]]) if cnt else \
                 torch.zeros(1, x.shape[1], device=x.device)
-        dev = x.device
         _, idx = sharded_topk(x, shard, k, idx_base=lo, n_valid=cnt, _rank_fn=self._rank_fn, _merge_fn=self._merge_fn)
         if world > 1:
             self.last_stats["nvlink_bytes"] = self.last_stats.get("nvlink_bytes", 0) + (world - 1) * idx.numel() * 8
@@ -300,20 +357,19 @@ class Evaluator(object):
                 print("  top-{:<4}{:12.1%}".format(kk, recalls[i]))
         if not rerank:
             return recalls
-        # evaluators.py:194-201: k-reciprocal re-ranking needs the dense q-g, q-q and g-g matrices; they are
-        # built on the GPU (tensor-core dense distance tiles) and re-ranked there (utils/rerank.py), rank 0 only,
-        # as in the reference (the other ranks score the original matrix).  The database rows are gathered
-        # over NVLink (device memory), never through the host.
-        eng = Engine.get(dev)
-        _, _, per = slice_bounds(len(gallery), world, rank)
-        y = _all_gather_rows(shard[:per] if shard.shape[0] >= per else shard, per)[: len(gallery)].contiguous()
-        distmat = eng.l2dist_dense(x, y)
+        # evaluators.py:194-201: k-reciprocal re-ranking on sparse data (sharded_rerank_topk): the neighbour pass is
+        # split over the ranks, the sparse stage runs on rank 0, and no q-g, q-q or g-g matrix is built.  The other
+        # ranks keep the first-pass recalls, as the reference's non-zero ranks score the original matrix.
         if self.rank == 0:
             print("Applying re-ranking ...")
-            from .utils.rerank import re_ranking
-            distmat = re_ranking(distmat, eng.l2dist_dense(x, x), eng.l2dist_dense(y, y), k1=rr_topk, k2=1,
-                                 lambda_value=lambda_value)
-        return evaluate_all(distmat, ground_truth, gallery, nms=nms)
+        res = sharded_rerank_topk(x, shard, k, idx_base=lo, n_valid=cnt, k1=rr_topk, k2=1, lambda_value=lambda_value)
+        if res is None:
+            return recalls
+        recalls = recalls_from_topk(res[1].cpu().numpy(), ground_truth, gallery, (1, 5, 10), nms)
+        print("Recall Scores:")
+        for i, kk in enumerate((1, 5, 10)):
+            print("  top-{:<4}{:12.1%}".format(kk, recalls[i]))
+        return recalls
 
     @staticmethod
     def _gather_named(local, names):

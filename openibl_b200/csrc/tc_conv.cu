@@ -30,17 +30,17 @@ using namespace tc;
 // ---- host: driver entry point ---------------------------------------------------------------
 namespace tc {
 EncodeTiledFn get_encode_tiled() {
-  static EncodeTiledFn fn = nullptr;
-  static bool tried = false;
-  if (!tried) {
-    tried = true;
+  // initialised exactly once even when several host threads (nn.DataParallel replicas, one per GPU) make their
+  // first call together: a plain "tried" flag could let a second thread see the flag before the pointer was stored
+  static const EncodeTiledFn fn = []() -> EncodeTiledFn {
     void* p = nullptr;
     cudaDriverEntryPointQueryResult qres;
     if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) ==
             cudaSuccess &&
         qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(p);
-  }
+      return reinterpret_cast<EncodeTiledFn>(p);
+    return nullptr;
+  }();
   return fn;
 }
 

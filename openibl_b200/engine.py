@@ -4,6 +4,7 @@ torch.distributed only; every FLOP of the hot path runs in libiblb200.so."""
 from __future__ import annotations
 
 import ctypes
+import threading
 from ctypes import byref, c_float, c_int, c_uint64, c_void_p
 from typing import Optional, Sequence
 
@@ -13,6 +14,9 @@ from . import _cabi
 from ._cabi import CONV_SIMT_FP32, CONV_TC_BF16X3, OUT_PCA, OUT_POOL, OUT_VLAD, check
 
 _engines = {}
+# nn.DataParallel runs one replica per device in threads of one process; their first forwards may ask for engines at
+# the same moment.  Each device still gets exactly one engine, and a thread only ever uses its own device's engine.
+_engines_lock = threading.Lock()
 
 
 def invalidate_caches() -> None:
@@ -22,7 +26,9 @@ def invalidate_caches() -> None:
     updates, the reference's own `_init_params`, netvlad.py:41-42) do not bump `_version`, so code that
     mutates parameters that way must call this (the model mirror does so from `_init_params`,
     `load_state_dict` and `reset_params`, and re-binds on every forward in training mode)."""
-    for eng in _engines.values():
+    with _engines_lock:
+        engines = list(_engines.values())
+    for eng in engines:
         eng.invalidate()
 
 
@@ -74,9 +80,13 @@ class Engine:
         if isinstance(device, torch.device):
             device = device.index if device.index is not None else torch.cuda.current_device()
         device = int(device)
-        if device not in _engines:
-            _engines[device] = Engine(device)
-        return _engines[device]
+        eng = _engines.get(device)
+        if eng is None:
+            with _engines_lock:
+                eng = _engines.get(device)
+                if eng is None:
+                    eng = _engines[device] = Engine(device)
+        return eng
 
     def __del__(self):
         try:

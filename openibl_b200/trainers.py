@@ -1,10 +1,15 @@
-"""Host-side mirror of the SFRS training step (reference ibl/trainers.py:165-320): `SFRSTrainer` with the same
-constructor, `train`, `_parse_data`, `_forward`, `_get_hard_loss` and `_get_loss`.
+"""Host-side mirror of the reference's training steps (ibl/trainers.py):
+
+* `Trainer` (trainers.py:11-162): NetVLAD (triplet loss) and SARE (`sare_ind` / `sare_joint`) training of `EmbedNet`
+  (or of the bare `VGG` with max pooling, `vlad=False`), as examples/netvlad_img.py drives it;
+* `SFRSTrainer` (trainers.py:165-320): the SFRS step, with the same constructor, `train`, `_parse_data`, `_forward`,
+  `_get_hard_loss` and `_get_loss`.
 
 What runs where: the model forward/backward (VGG trunk suffix, NetVLAD) is libiblb200 through the autograd Functions of
-openibl_b200.models; the loss algebra below works on a handful of [B, n, 9, 32768] region descriptors and [B, n, 9, 9]
-similarity matrices per step and is plain torch, as in the reference.  BASELINE configs[4] drives this with
-tuple_size = 4 under DistributedDataParallel (examples/sfrs_step_synthetic.py)."""
+openibl_b200.models; the loss algebra below works on a handful of [B, n, 32768] descriptors (and, for SFRS,
+[B, n, 9, 9] similarity matrices) per step and is plain torch, as in the reference.  BASELINE configs[4] drives the
+SFRS step with tuple_size = 4 under DistributedDataParallel (examples/sfrs_step_synthetic.py); tools/bench_train.py
+times the `Trainer` step."""
 from __future__ import annotations
 
 import time
@@ -20,6 +25,69 @@ def _rank():
         return torch.distributed.get_rank()
     except Exception:
         return 0
+
+
+class Trainer(object):
+    """NetVLAD (CVPR'16, loss_type='triplet') and SARE (ICCV'19, 'sare_ind' / 'sare_joint') training.
+
+    The losses are the reference's Euclidean versions (trainers.py:90-140): the triplet margin loss on L2 distances,
+    and SARE's log-softmax over negated squared distances -- not the dot-product versions `SFRSTrainer` uses.
+    `_get_loss` raises ValueError for an unknown loss type (the reference's `assert ("...")` always passes and then
+    fails on the unbound `loss`)."""
+
+    def __init__(self, model, margin=0.3, gpu=None, temp=0.07):
+        self.model, self.gpu, self.margin, self.temp = model, gpu, margin, temp
+
+    # ---- one epoch (trainers.py:24-61) ------------------------------------------------------------------------
+    def train(self, epoch, sub_id, data_loader, optimizer, train_iters, print_freq=1, vlad=True, loss_type="triplet"):
+        self.model.train()
+        batch_time, data_time, losses = AverageMeter(), AverageMeter(), AverageMeter()
+        end = time.time()
+        data_loader.new_epoch()
+        for i in range(train_iters):
+            inputs = self._parse_data(data_loader.next())
+            data_time.update(time.time() - end)
+            loss = self._forward(inputs, vlad, loss_type)
+            losses.update(loss.item())
+            optimizer.zero_grad()
+            loss.backward()
+            optimizer.step()
+            batch_time.update(time.time() - end)
+            end = time.time()
+            if (i + 1) % print_freq == 0 and _rank() == 0:
+                print("Epoch: [{}-{}][{}/{}]\tTime {:.3f} ({:.3f})\tData {:.3f} ({:.3f})\tLoss {:.3f} ({:.3f})".format(
+                    epoch, sub_id, i + 1, train_iters, batch_time.val, batch_time.avg, data_time.val, data_time.avg,
+                    losses.val, losses.avg))
+
+    def _parse_data(self, inputs):
+        """trainers.py:64-68: the collated tuple positions -> [B, N, C, H, W] on the device."""
+        imgs = torch.stack([item[0] for item in inputs]).permute(1, 0, 2, 3, 4)
+        return imgs.cuda(self.gpu)
+
+    def _forward(self, inputs, vlad, loss_type):
+        """trainers.py:70-80: the loss on the VLAD descriptor when `vlad`, else on the max-pooled conv5 feature."""
+        B, N, C, H, W = inputs.size()
+        outputs_pool, outputs_vlad = self.model(inputs.reshape(-1, C, H, W))
+        return self._get_loss(outputs_vlad if vlad else outputs_pool, loss_type, B, N)
+
+    def _get_loss(self, outputs, loss_type, B, N):
+        """trainers.py:82-162.  outputs [B*N, L], tuple order (anchor, positive, N-2 negatives)."""
+        outputs = outputs.reshape(B, N, -1)
+        L = outputs.size(-1)
+        a, p, n = outputs[:, 0], outputs[:, 1], outputs[:, 2:]
+        if loss_type == "triplet":
+            ae = a.unsqueeze(1).expand_as(n).reshape(-1, L)
+            pe = p.unsqueeze(1).expand_as(n).reshape(-1, L)
+            return F.triplet_margin_loss(ae, pe, n.reshape(-1, L), margin=self.margin, p=2, reduction="mean")
+        if loss_type not in ("sare_joint", "sare_ind"):
+            raise ValueError("Unknown loss function: {}".format(loss_type))
+        dist_pos = ((a - p) ** 2).sum(1).view(B, 1)                                        # [B,1]
+        dist_neg = ((a.unsqueeze(1).expand_as(n).reshape(-1, L) - n.reshape(-1, L)) ** 2).sum(1).view(B, -1)
+        if loss_type == "sare_joint":
+            logits = -torch.cat((dist_pos, dist_neg), 1)                                   # [B, 1+n]
+        else:
+            logits = -torch.stack((dist_pos.expand_as(dist_neg), dist_neg), 2).reshape(-1, 2)   # [B*n, 2]
+        return (-F.log_softmax(logits, 1)[:, 0]).mean()
 
 
 class SFRSTrainer(object):

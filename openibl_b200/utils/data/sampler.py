@@ -1,10 +1,15 @@
 """DistributedSliceSampler (ibl/utils/data/sampler.py:194-223): rank r reads the r-th contiguous
 slice of ceil(N/world) items, the tail wrapping to the head; extract_features un-pads by
-truncation.  Part of the hot-path contract (SURVEY 8e)."""
+truncation.  Part of the hot-path contract (SURVEY 8e).
+
+Like the reference module (sampler.py:9-12) this one re-exports torch's samplers, so that
+`from ibl.utils.data.sampler import SubsetRandomSampler` (examples/cluster.py:21) resolves."""
 import math
 
 import torch.distributed as dist
-from torch.utils.data.sampler import Sampler
+from torch.utils.data import BatchSampler  # noqa: F401
+from torch.utils.data.sampler import (  # noqa: F401
+    RandomSampler, Sampler, SequentialSampler, SubsetRandomSampler, WeightedRandomSampler)
 
 
 def slice_bounds(n, world, rank):

@@ -276,8 +276,9 @@ int ibl_debug_gemm_tn(ibl_engine* e, const float* A, const float* B, float* C, v
 int ibl_debug_umma_strided(ibl_engine* e, const void* A, int rows, const void* B, int s0, int group_rows,
                            int base_mode, float* D, void* stream);
 /* Average device time (ms) of one backbone layer over `reps` launches, weights from the engine
- * (tools/bench_layers.py).  layer 0 = conv1_1 (x NCHW [N,3,H,W]); 1..12 = conv1_2..conv5_3
- * (x NHWC [N,H,W,Cin] fp32).  Synchronises. */
+ * (tools/bench_layers.py).  layer 0 = the tensor-core conv1_1 (x NCHW [N,3,H,W]); 1..12 = conv1_2..conv5_3
+ * (x NHWC [N,H,W,Cin] fp32), where bn_override forces the N tile (64/128) when it divides Cout, 0 = default.
+ * Synchronises. */
 int ibl_debug_time_layer(ibl_engine* e, int layer, const float* x, int N, int H, int W, int bn_override,
                          int reps, float* ms_out);
 

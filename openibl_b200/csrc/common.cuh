@@ -80,8 +80,7 @@ struct ConvParams {
 int launch_repack_weights(const float* w_oihw, int cout, int cin, ConvParams& p, cudaStream_t s);
 int launch_conv3x3_simt(const float* x_nhwc, const ConvParams& p, int N, int H, int W, int cin,
                         int cout, bool relu, float* y_nhwc, cudaStream_t s);
-int launch_conv1_1(const float* x_nchw, const ConvParams& p, int N, int H, int W, bool to_planes,
-                   float* y_nhwc, __nv_bfloat16* y_hi, __nv_bfloat16* y_lo, cudaStream_t s);
+int launch_conv1_1(const float* x_nchw, const ConvParams& p, int N, int H, int W, float* y_nhwc, cudaStream_t s);
 int launch_maxpool2x2(const float* x, int N, int H, int W, int C, float* y, cudaStream_t s);
 int launch_nhwc_to_nchw(const float* x, int N, int S, int C, float* y, cudaStream_t s);
 int launch_u8_hwc_to_nchw_norm(const uint8_t* x, int N, int H, int W, const float* mean, const float* stdv, float* y,
@@ -140,11 +139,11 @@ int launch_global_maxpool_planes(const __nv_bfloat16* hi, const __nv_bfloat16* l
                                  cudaStream_t s);
 
 // tc_gemm.cu  (wgmma NT GEMM on bf16 hi/lo planes: distance/top-16, dense distance, PCA partials)
-int dist_top16_max_runs(int m, int n_valid, bool pairs);
+int dist_top16_max_runs(int n_valid);
 int launch_dist_top16_tc(const __nv_bfloat16* q_hi, const __nv_bfloat16* q_lo, const float* qn, int m,
                          const __nv_bfloat16* d_hi, const __nv_bfloat16* d_lo, const float* dn, int n,
                          int n_valid, int K, float* cand_d, long long* cand_i, int max_runs, int* runs_out,
-                         bool pairs, cudaStream_t s);
+                         cudaStream_t s);
 int launch_dist_dense_tc(const __nv_bfloat16* q_hi, const __nv_bfloat16* q_lo, const float* qn, int m,
                          const __nv_bfloat16* d_hi, const __nv_bfloat16* d_lo, const float* dn, int n, int K,
                          float* out, long long ld_out, cudaStream_t s);

@@ -140,7 +140,7 @@ int vgg_forward_impl(ibl_engine* e, const float* x, int N, int H, int W, float* 
   int h = H, w = W;
   int cur = 0;
   if (e->conv_mode == IBL_CONV_SIMT_FP32) {
-    IBL_RET(launch_conv1_1(x, e->conv[0], N, h, w, false, e->act[0].as<float>(), nullptr, nullptr, s));
+    IBL_RET(launch_conv1_1(x, e->conv[0], N, h, w, e->act[0].as<float>(), s));
     e->launches++;
     for (int l = 1; l <= last_layer; ++l) {
       const ConvLayer& L = kVgg16[l];
@@ -165,9 +165,9 @@ int vgg_forward_impl(ibl_engine* e, const float* x, int N, int H, int W, float* 
   size_t elems = (size_t)N * h * w * 64;
   int first_l = 1;
   // conv1_1 + conv1_2 + pool in one kernel (tc_conv.cu: conv1_fused_tc_kernel): the 2.5 GB conv1_1 activation never
-  // goes to HBM.  IBL_CONV1_FUSED=0 keeps the two separate kernels (A/B measurements, variant tests).
-  static const bool fused1_env = [] { const char* v = getenv("IBL_CONV1_FUSED"); return !v || atoi(v) != 0; }();
-  const bool fused1 = fused1_env && last_layer >= 2 && h >= 2 && w >= 2;
+  // goes to HBM.  A forward that stops at conv1_2 (last_layer 1) returns conv1_2's output in fp32; the fused kernel
+  // writes only hi/lo planes, so that forward runs conv1_1 and conv1_2 as two kernels.
+  const bool fused1 = last_layer >= 2 && h >= 2 && w >= 2;
   if (fused1) {
     const size_t out_elems = (size_t)N * (h / 2) * (w / 2) * 64;
     IBL_RET(launch_conv1_fused_tc(x, e->w0_oihw, e->conv[0].bias, e->conv[1], N, h, w, hi_of(1, out_elems),
@@ -178,12 +178,7 @@ int vgg_forward_impl(ibl_engine* e, const float* x, int N, int H, int W, float* 
     w /= 2;
     first_l = 2;
   } else {
-    static int simt1 = -1;   // IBL_CONV1_SIMT=1: keep conv1_1 on the CUDA cores (A/B experiments)
-    if (simt1 < 0) { const char* v = getenv("IBL_CONV1_SIMT"); simt1 = (v && atoi(v)) ? 1 : 0; }
-    if (simt1)
-      IBL_RET(launch_conv1_1(x, e->conv[0], N, h, w, true, nullptr, hi_of(0, elems), lo_of(0, elems), s));
-    else
-      IBL_RET(launch_conv1_1_tc(x, e->w0_oihw, e->conv[0].bias, N, h, w, hi_of(0, elems), lo_of(0, elems), s));
+    IBL_RET(launch_conv1_1_tc(x, e->w0_oihw, e->conv[0].bias, N, h, w, hi_of(0, elems), lo_of(0, elems), s));
     e->launches++;
   }
   for (int l = first_l; l <= last_layer; ++l) {
@@ -410,7 +405,7 @@ int ibl_vgg16_prefix_forward(ibl_engine* e, const float* x, int N, int H, int W,
   DeviceGuard g(e->device);
   if (n_layers == 1) {
     e->launches++;
-    return launch_conv1_1(x, e->conv[0], N, H, W, false, out_nhwc, nullptr, nullptr, S(stream));
+    return launch_conv1_1(x, e->conv[0], N, H, W, out_nhwc, S(stream));
   }
   return vgg_forward_impl(e, x, N, H, W, out_nhwc, S(stream), nullptr, n_layers - 1);
 }
@@ -426,7 +421,7 @@ int ibl_vgg16_layer_forward(ibl_engine* e, int layer, const float* x, int N, int
   const ConvLayer& L = kVgg16[layer];
   if (layer == 0) {
     e->launches++;
-    return launch_conv1_1(x, e->conv[0], N, H, W, false, y_nhwc, nullptr, nullptr, s);
+    return launch_conv1_1(x, e->conv[0], N, H, W, y_nhwc, s);
   }
   if (e->conv_mode == IBL_CONV_SIMT_FP32) {
     e->launches++;
@@ -697,8 +692,7 @@ int ibl_extract_host(ibl_engine* e, const float* x_host, int N, int H, int W, un
   }
   const size_t img_elems = (size_t)3 * H * W;
   // uneven split: only the first (small) part's copy is exposed; the rest streams in behind its compute
-  static const int split_div = [] { const char* v = getenv("IBL_HOST_SPLIT"); const int d = v ? atoi(v) : 0; return d >= 2 ? d : 4; }();
-  const int n_first = halves == 2 ? (N / split_div > 0 ? N / split_div : 1) : N;
+  const int n_first = halves == 2 ? N / 4 : N;
   for (int i = 0; i < halves; ++i) {
     const int n0 = i == 0 ? 0 : n_first, nb = i == 0 ? n_first : N - n_first;
     IBL_CUDA_OK(cudaMemcpyAsync(e->stage_in.as<float>() + n0 * img_elems, x_host + n0 * img_elems,
@@ -945,9 +939,7 @@ int ibl_l2dist_topk(ibl_engine* e, const float* q, int m, const float* db, int n
   IBL_REQUIRE(n_valid >= 0 && n_valid <= n, "n_valid out of range");
   IBL_REQUIRE(k >= 1 && k <= 128, "top-k supports 1 <= k <= 128");
   DeviceGuard g(e->device);
-  // IBL_DIST_SCREEN=3 selects the bf16x3 screening kernel of tc_gemm.cu (A/B measurements, variant tests)
-  static const int screen_env = [] { const char* v = getenv("IBL_DIST_SCREEN"); return v ? atoi(v) : 1; }();
-  if (e->gemm_mode == IBL_CONV_TC_BF16X3 && d % 64 == 0 && n_valid > 0 && k <= 12 && m > 128 && screen_env != 3) {
+  if (e->gemm_mode == IBL_CONV_TC_BF16X3 && d % 64 == 0 && n_valid > 0 && k <= 12 && m > 128) {
     // single fp16 tensor-core pass to screen, exact fp32 to decide, guard + exact fallback on the device
     size_t off[9];
     IBL_RET(e->d1_ws.ensure(dist1_workspace_bytes(m, n, d, off)));
@@ -977,15 +969,14 @@ int ibl_l2dist_topk(ibl_engine* e, const float* q, int m, const float* db, int n
     e->flag_counter = reinterpret_cast<const int*>(e->guard_ws.p);
     e->dist_path = k <= 12 ? 2 : 3;
     if (k <= 12) {
-      // SM pairs (2-CTA clusters multicasting the database tile, tc_gemm.cu) unless IBL_DIST_2SM=0
-      static const bool two_sm = [] { const char* v = getenv("IBL_DIST_2SM"); return !v || atoi(v) != 0; }();
-      const int max_runs = dist_top16_max_runs(m, n_valid, two_sm);
+      // m <= 128 here: one row tile of the bf16x3 top-16 screen (tc_gemm.cu)
+      const int max_runs = dist_top16_max_runs(n_valid);
       IBL_RET(e->cand_d.ensure((size_t)max_runs * m * kc * sizeof(float)));
       IBL_RET(e->cand_i.ensure((size_t)max_runs * m * kc * sizeof(int64_t)));
       int runs = 0;
       IBL_RET(launch_dist_top16_tc(qh, qh + qe, e->qn.as<float>(), m, dh, dh + de, e->dbn.as<float>(), n,
                                    n_valid, d, e->cand_d.as<float>(), e->cand_i.as<long long>(), max_runs,
-                                   &runs, two_sm, s));
+                                   &runs, s));
       e->launches++;
       const long long* ci = e->cand_i.as<long long>();
       const float* cd = e->cand_d.as<float>();
@@ -1289,7 +1280,7 @@ int ibl_debug_umma_strided(ibl_engine* e, const void* A, int rows, const void* B
 }
 
 // Timing hooks (tools/bench_layers.py): average device time of one backbone layer over `reps`
-// back-to-back launches, weights taken from the engine (ibl_engine_set_vgg16).  layer 0 = conv1_1
+// back-to-back launches, weights taken from the engine (ibl_engine_set_vgg16).  layer 0 = the tensor-core conv1_1
 // (x is NCHW [N,3,H,W]); layers 1..12 take x NHWC [N,H,W,Cin] fp32 (converted to planes once).
 int ibl_debug_time_layer(ibl_engine* e, int layer, const float* x, int N, int H, int W, int bn_override,
                          int reps, float* ms_out) {
@@ -1313,8 +1304,7 @@ int ibl_debug_time_layer(ibl_engine* e, int layer, const float* x, int N, int H,
   for (int r = -1; r < reps && rc == IBL_OK; ++r) {       // r = -1 is a warm-up launch
     if (r == 0) cudaEventRecord(e0, nullptr);
     if (layer == 0)
-      rc = bn_override == 1 ? launch_conv1_1(x, e->conv[0], N, H, W, true, nullptr, oh_, oh_ + out_e, nullptr)
-                            : launch_conv1_1_tc(x, e->w0_oihw, e->conv[0].bias, N, H, W, oh_, oh_ + out_e, nullptr);
+      rc = launch_conv1_1_tc(x, e->w0_oihw, e->conv[0].bias, N, H, W, oh_, oh_ + out_e, nullptr);
     else
       rc = launch_conv3x3_tc(ih, ih + in_e, e->conv[layer], N, H, W, L.cin, L.cout, L.relu, L.pool,
                              layer == 12 ? nullptr : oh_, layer == 12 ? nullptr : oh_ + out_e,

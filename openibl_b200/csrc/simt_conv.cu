@@ -146,15 +146,12 @@ int launch_conv3x3_simt(const float* x, const ConvParams& p, int N, int H, int W
 // conv1_1: NCHW fp32 [N,3,H,W] -> NHWC [N,H,W,64], + bias + ReLU (vgg.py slot 0).  K = 27 does not
 // tile onto a TMA-fed tensor-core GEMM; this is the CUDA-core version: one pixel per thread, 64 accumulators in
 // registers, the 27x64 weights broadcast from shared memory (LDS.128 feeds 4 FMAs).  Each thread
-// writes its pixel's 64 channels as contiguous 16-byte stores (256 B fp32, or 128 B + 128 B of bf16
-// hi/lo planes), so every 128-byte line is fully written by one thread.
+// writes its pixel's 64 fp32 channels as contiguous 16-byte stores, so every 128-byte line is fully
+// written by one thread.
 // ------------------------------------------------------------------------------------------
-template <bool PLANES>
 __global__ void __launch_bounds__(128)
 conv1_1_kernel(const float* __restrict__ x, const float* __restrict__ w /*[27][64]*/,
-               const float* __restrict__ bias, float* __restrict__ y,
-               __nv_bfloat16* __restrict__ y_hi, __nv_bfloat16* __restrict__ y_lo, int N, int H,
-               int W) {
+               const float* __restrict__ bias, float* __restrict__ y, int N, int H, int W) {
   __shared__ __align__(16) float ws[27][64];
   __shared__ __align__(16) float bs[64];
   const int t = threadIdx.x;
@@ -193,39 +190,15 @@ conv1_1_kernel(const float* __restrict__ x, const float* __restrict__ w /*[27][6
   }
 #pragma unroll
   for (int j = 0; j < 64; ++j) acc[j] = fmaxf(acc[j], 0.f);
-  if (!PLANES) {
-    float4* o = reinterpret_cast<float4*>(y + pm * 64);
+  float4* o = reinterpret_cast<float4*>(y + pm * 64);
 #pragma unroll
-    for (int j = 0; j < 16; ++j) o[j] = make_float4(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]);
-  } else {
-    uint4* oh = reinterpret_cast<uint4*>(y_hi + pm * 64);
-    uint4* ol = reinterpret_cast<uint4*>(y_lo + pm * 64);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      uint32_t hi[4], lo[4];
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const float x0 = acc[8 * j + 2 * q], x1 = acc[8 * j + 2 * q + 1];
-        const __nv_bfloat16 h0 = __float2bfloat16_rn(x0), h1 = __float2bfloat16_rn(x1);
-        __nv_bfloat162 hh(h0, h1);
-        __nv_bfloat162 ll = __floats2bfloat162_rn(x0 - __bfloat162float(h0), x1 - __bfloat162float(h1));
-        hi[q] = *reinterpret_cast<uint32_t*>(&hh);
-        lo[q] = *reinterpret_cast<uint32_t*>(&ll);
-      }
-      oh[j] = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-      ol[j] = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-    }
-  }
+  for (int j = 0; j < 16; ++j) o[j] = make_float4(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]);
 }
 
-int launch_conv1_1(const float* x_nchw, const ConvParams& p, int N, int H, int W, bool to_planes,
-                   float* y, __nv_bfloat16* y_hi, __nv_bfloat16* y_lo, cudaStream_t s) {
+int launch_conv1_1(const float* x_nchw, const ConvParams& p, int N, int H, int W, float* y, cudaStream_t s) {
   long long M = (long long)N * H * W;
   unsigned blocks = (unsigned)((M + 127) / 128);
-  if (to_planes)
-    conv1_1_kernel<true><<<blocks, 128, 0, s>>>(x_nchw, p.w_tck, p.bias, nullptr, y_hi, y_lo, N, H, W);
-  else
-    conv1_1_kernel<false><<<blocks, 128, 0, s>>>(x_nchw, p.w_tck, p.bias, y, nullptr, nullptr, N, H, W);
+  conv1_1_kernel<<<blocks, 128, 0, s>>>(x_nchw, p.w_tck, p.bias, y, N, H, W);
   IBL_CUDA_OK(cudaGetLastError());
   return IBL_OK;
 }

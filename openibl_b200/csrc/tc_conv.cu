@@ -18,8 +18,6 @@
 //   warp 4     TMA producer
 // Epilogue: accumulator -> row-per-thread views (Acc128::rows32), + bias, ReLU, optional fused 2x2 max-pool
 // (warp shuffles), split into hi/lo planes (or fp32 for conv5_3), 16-byte stores.
-#include <stdlib.h>
-
 #include "common.cuh"
 #include "tc_common.cuh"
 
@@ -88,16 +86,7 @@ struct ConvTcArgs {
   float* y_f32;
   float* ssq;             // optional [n_tiles][N*H*W] per-pixel sum of squares of the outputs (no pool)
   long long ssq_stride;
-  float acc_scale;        // optional accumulator compensation factor (see tc_acc_scale)
 };
-
-// Optional compensation of a tensor-core accumulator that rounds toward zero: the epilogue multiplies the accumulator
-// by 1 + n_mma * c (n_mma = k16 MMA steps accumulated into the tile) before the bias is added.  IBL_TC_BIAS_COMP=<c>
-// sets c (default 0: the sm_90 accumulator needs no compensation at the 1e-4 descriptor tolerance).
-static float tc_acc_scale(int cin) {
-  static const float c = [] { const char* v = getenv("IBL_TC_BIAS_COMP"); return v ? (float)atof(v) : 0.f; }();
-  return 1.f + (float)(27 * (cin / 16)) * c;
-}
 
 __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
   __nv_bfloat162 t = __floats2bfloat162_rn(a, b);
@@ -127,8 +116,8 @@ __device__ __forceinline__ void conv_epilogue_tile(const ConvTcArgs& a, const Ac
     uint32_t raw[32];
     acc.rows32(ch, stg, raw);
     if (a.pool) {
-      // 2x2 max-pool BEFORE bias / ReLU / split (fmaf(., scale > 0, b) and max(., 0) are monotone, so the results are
-      // the same bits) as a two-step exchange: against the w-neighbour (lane ^ 1) every lane keeps one half of the 32
+      // 2x2 max-pool BEFORE bias / ReLU / split (. + b and max(., 0) are monotone, so the results are the same bits)
+      // as a two-step exchange: against the w-neighbour (lane ^ 1) every lane keeps one half of the 32
       // channels and sends the other, against the h-neighbour (lane ^ TW) one half of those 16 -- 24 shuffles instead
       // of 64, and each of the window's four lanes finishes 8 channels (bias, ReLU, hi/lo, ONE 16-byte store per plane)
       // instead of one lane doing all 32 while three idle.
@@ -153,7 +142,7 @@ __device__ __forceinline__ void conv_epilogue_tile(const ConvTcArgs& a, const Ac
         const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
-          w8[j] = fmaf(w8[j], a.acc_scale, bb[j]);
+          w8[j] = w8[j] + bb[j];
           if (a.relu) w8[j] = fmaxf(w8[j], 0.f);
         }
         const long long off = pix * a.cout + cbase;
@@ -182,10 +171,10 @@ __device__ __forceinline__ void conv_epilogue_tile(const ConvTcArgs& a, const Ac
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       const float4 b = __ldg(bp + j);
-      v[4 * j + 0] = fmaf(__uint_as_float(raw[4 * j + 0]), a.acc_scale, b.x);
-      v[4 * j + 1] = fmaf(__uint_as_float(raw[4 * j + 1]), a.acc_scale, b.y);
-      v[4 * j + 2] = fmaf(__uint_as_float(raw[4 * j + 2]), a.acc_scale, b.z);
-      v[4 * j + 3] = fmaf(__uint_as_float(raw[4 * j + 3]), a.acc_scale, b.w);
+      v[4 * j + 0] = __uint_as_float(raw[4 * j + 0]) + b.x;
+      v[4 * j + 1] = __uint_as_float(raw[4 * j + 1]) + b.y;
+      v[4 * j + 2] = __uint_as_float(raw[4 * j + 2]) + b.z;
+      v[4 * j + 3] = __uint_as_float(raw[4 * j + 3]) + b.w;
     }
     if (a.relu) {
 #pragma unroll
@@ -233,7 +222,7 @@ constexpr int TC_A_BYTES = TC_BM * TC_BK * 2;   // 16 KiB per plane
 // nine taps are nine views of it: tap (kh,kw) starts (kh*10 + kw) rows into the tile and consecutive 8-pixel
 // row groups are 10 rows (1280 B) apart.  The 128B swizzle is a function of the shared-memory address, so a
 // descriptor whose start is only 128-byte aligned and whose group stride is not a multiple of 1024 B reads the
-// TMA-written tile correctly (pinned on hardware by tests/test_gpu_variants.py through tc_probe.cu).
+// TMA-written tile correctly (pinned on hardware by tests/test_gpu_parity.py through tc_probe.cu).
 // L2->SM traffic of the A operand drops from 9 x 32 KiB to 45 KiB per chunk; the weights get their own ring.
 constexpr int TC_HALO_W = 10, TC_HALO_H = 18;
 constexpr int TC_HALO_PLANE = 23 * 1024;        // 180 rows x 128 B = 23040 B, padded to the swizzle period
@@ -247,11 +236,7 @@ struct ConvTcSmem {
   static constexpr int BYTES = A_RING + STAGES * STAGE_BYTES + ACC_STG_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
 };
 
-// PAIR: the grid is launched as clusters of two CTAs ("SM pairs") that share one work item = (two adjacent patches, one
-// N tile).  Each CTA stages its own activations and fetches only HALF of every weight tap, TMA-multicasting it into both
-// CTAs' shared memory: the per-SM L2->SM weight traffic halves.  A weight slot may be refilled only when the consumers
-// of BOTH CTAs have released it (arrival count 8: every consumer warp arrives on both CTAs' barriers).
-template <int BN, int STAGES, bool HALO, int NA, bool PAIR>
+template <int BN, int STAGES, bool HALO, int NA>
 __global__ void __launch_bounds__(160, 1)
 conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tm_xhi, const __grid_constant__ CUtensorMap tm_xlo,
                   const __grid_constant__ CUtensorMap tm_whi, const __grid_constant__ CUtensorMap tm_wlo,
@@ -272,9 +257,8 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tm_xhi, const __grid_const
   uint64_t* aempty_bar = afull_bar + NA;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = PAIR ? cluster_ctarank() : 0u;
-  const int worker = PAIR ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-  const int n_workers = PAIR ? (int)(gridDim.x >> 1) : (int)gridDim.x;
+  const int worker = (int)blockIdx.x;
+  const int n_workers = (int)gridDim.x;
   if (warp == 4 && lane == 0) {
     tma_prefetch_desc(&tm_xhi);
     tma_prefetch_desc(&tm_xlo);
@@ -282,7 +266,7 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tm_xhi, const __grid_const
     tma_prefetch_desc(&tm_wlo);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], PAIR ? 8 : 4);   // one arrival per consumer warp (of both CTAs of a pair)
+      mbar_init(&empty_bar[i], 4);   // one arrival per consumer warp
     }
     for (int i = 0; i < NA; ++i) {
       mbar_init(&afull_bar[i], 1);
@@ -292,7 +276,6 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tm_xhi, const __grid_const
     fence_proxy_async();
   }
   __syncthreads();
-  if (PAIR) cluster_sync_all();     // the peer's barriers exist before anything is multicast into this CTA
 
   const int TW = 1 << a.tw_log2;
   const int kchunks = a.cin / TC_BK;
@@ -300,8 +283,7 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tm_xhi, const __grid_const
   const int tiles_per_img = a.tiles_h * a.tiles_w;
   auto coords = [&](int tile, int& img, int& h0, int& w0, int& nt) {
     nt = tile % a.n_tiles;
-    // pair: an odd patch count leaves img == N for the last peer: TMA zero-fills, the epilogue stores nothing
-    const int pt = PAIR ? 2 * (tile / a.n_tiles) + (int)rank : tile / a.n_tiles;
+    const int pt = tile / a.n_tiles;
     img = pt / tiles_per_img;
     const int rem = pt - img * tiles_per_img;
     h0 = (rem / a.tiles_w) * (TC_BM >> a.tw_log2);
@@ -315,17 +297,10 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tm_xhi, const __grid_const
     const uint32_t bars_a = ring_a + STAGES * STAGE_BYTES + ACC_STG_BYTES;
     const uint32_t full_a = bars_a, empty_a = bars_a + 8 * STAGES;
     const uint32_t afull_a = bars_a + 16 * STAGES, aempty_a = afull_a + 8 * NA;
-    const int rank_u = (int)warp_uniform(rank);
-    // the two weight planes of one tap (into `st`, planes B_BYTES apart); a pair's CTAs each fetch one half of the rows
+    // the two weight planes of one tap (into `st`, planes B_BYTES apart)
     auto load_w = [&](uint32_t st, uint32_t fb, int c0, int n0, int tap) {
-      if (PAIR) {
-        constexpr int HB = B_BYTES / 2;
-        tma_load_3d_mc_a(st + rank_u * HB, &tm_whi, fb, c0, n0 + rank_u * (BN / 2), tap, 0x3);
-        tma_load_3d_mc_a(st + B_BYTES + rank_u * HB, &tm_wlo, fb, c0, n0 + rank_u * (BN / 2), tap, 0x3);
-      } else {
-        tma_load_3d_a(st, &tm_whi, fb, c0, n0, tap);
-        tma_load_3d_a(st + B_BYTES, &tm_wlo, fb, c0, n0, tap);
-      }
+      tma_load_3d_a(st, &tm_whi, fb, c0, n0, tap);
+      tma_load_3d_a(st + B_BYTES, &tm_wlo, fb, c0, n0, tap);
     };
     int stage = 0;
     uint32_t phase = 0;
@@ -423,11 +398,8 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tm_xhi, const __grid_const
     int stage = 0, astage = 0;
     uint32_t phase = 0, aphase = 0;
     (void)ring_a; (void)astage; (void)aphase;
-    auto release_w = [&](int st) {          // this warp is done reading weight slot st (in both CTAs' rings of a pair)
-      if (lane == 0) {
-        mbar_arrive(&empty_bar[st]);
-        if (PAIR) mbar_arrive_remote(mapa_u32(smem_u32(&empty_bar[st]), rank ^ 1u));
-      }
+    auto release_w = [&](int st) {          // this warp is done reading weight slot st
+      if (lane == 0) mbar_arrive(&empty_bar[st]);
     };
     for (int tile = worker; tile < a.total_tiles; tile += n_workers) {
       int img, h0, w0, nt;
@@ -502,43 +474,23 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tm_xhi, const __grid_const
     }
   }
   __syncthreads();
-  if (PAIR) cluster_sync_all();     // no CTA leaves while its peer may still multicast into it or arrive on its barriers
 }
 
 // ---- host launcher --------------------------------------------------------------------------
 template <int BN, int STAGES, bool HALO = false, int NA = 0>
 static int launch_tc_variant(const CUtensorMap& xhi, const CUtensorMap& xlo, const CUtensorMap& whi,
-                             const CUtensorMap& wlo, const ConvTcArgs& a, bool pair, cudaStream_t s) {
+                             const CUtensorMap& wlo, const ConvTcArgs& a, cudaStream_t s) {
   constexpr int smem = ConvTcSmem<BN, STAGES, HALO, NA>::BYTES;
   static_assert(smem <= 232448, "shared-memory budget");
-  static DeviceOnce attr_done;   // the attributes are per device
+  static DeviceOnce attr_done;   // the attribute is per device
   if (!attr_done.done()) {
-    IBL_CUDA_OK(cudaFuncSetAttribute(conv3x3_tc_kernel<BN, STAGES, HALO, NA, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    IBL_CUDA_OK(cudaFuncSetAttribute(conv3x3_tc_kernel<BN, STAGES, HALO, NA, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    IBL_CUDA_OK(cudaFuncSetAttribute(conv3x3_tc_kernel<BN, STAGES, HALO, NA>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     attr_done.mark();
   }
   const int sms = device_sm_count();
-  if (!pair) {
-    const int grid = a.total_tiles < sms ? a.total_tiles : sms;
-    conv3x3_tc_kernel<BN, STAGES, HALO, NA, false><<<grid, 160, smem, s>>>(xhi, xlo, whi, wlo, a);
-    IBL_CUDA_OK(cudaGetLastError());
-    return IBL_OK;
-  }
-  // a.total_tiles counts pair work items; one 2-CTA cluster per item, at most sms/2 clusters
-  const int pairs = a.total_tiles < sms / 2 ? a.total_tiles : sms / 2;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(2 * pairs);
-  cfg.blockDim = dim3(160);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = s;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  IBL_CUDA_OK(cudaLaunchKernelEx(&cfg, conv3x3_tc_kernel<BN, STAGES, HALO, NA, true>, xhi, xlo, whi, wlo, a));
+  const int grid = a.total_tiles < sms ? a.total_tiles : sms;
+  conv3x3_tc_kernel<BN, STAGES, HALO, NA><<<grid, 160, smem, s>>>(xhi, xlo, whi, wlo, a);
+  IBL_CUDA_OK(cudaGetLastError());
   return IBL_OK;
 }
 
@@ -569,30 +521,20 @@ int launch_conv3x3_tc(const __nv_bfloat16* x_hi, const __nv_bfloat16* x_lo, cons
   int bn = cout % 128 == 0 ? 128 : 64;
   if (g_tc_bn_override && cout % g_tc_bn_override == 0 && (g_tc_bn_override == 64 || g_tc_bn_override == 128))
     bn = g_tc_bn_override;
-  // Halo staging (16x8 patches): IBL_CONV_HALO=0 never, =1 (default) on the 128-wide tiles, =2 on every N tile.  The
-  // choice depends on Cout only, never on the batch (the variants walk K in different orders).
-  static const int halo_env = [] { const char* v = getenv("IBL_CONV_HALO"); return v ? atoi(v) : 1; }();
-  const bool halo = halo_env == 2 || (halo_env == 1 && bn == 128);
+  // Halo staging (16x8 patches) on the 128-wide tiles.  The choice depends on Cout only, never on the batch (the two
+  // kernels walk K in different orders).
+  const bool halo = bn == 128;
   if (halo) {
     a.tw_log2 = 3;
     a.tiles_w = cdiv(W, 8);
     a.tiles_h = cdiv(H, 16);
   }
-  // SM pairs (weight taps multicast to two CTAs with adjacent patches): IBL_CONV_2SM=0 (default) never, =1 where the
-  // weights are the larger operand stream (Cin >= 256: conv3_2 .. conv5_3), =2 on every layer.  Measured on an H100 at
-  // batch 32 x 480x640: =1 gave 949 images/s against 1063 without pairs (the cluster-wide slot release costs more
-  // than the halved weight traffic saves), hence off by default.  Each CTA still computes its own patch in the same
-  // order, so the results do not depend on the choice.
-  static const int pair_env = [] { const char* v = getenv("IBL_CONV_2SM"); return v ? atoi(v) : 0; }();
-  const long long patches = (long long)N * a.tiles_h * a.tiles_w;
-  const bool pair = patches >= 2 && (pair_env == 2 || (pair_env == 1 && cin >= 256));
   a.n_tiles = cout / bn;
-  a.total_tiles = (int)((pair ? (patches + 1) / 2 : patches) * a.n_tiles);
+  a.total_tiles = (int)((long long)N * a.tiles_h * a.tiles_w * a.n_tiles);
   a.relu = relu; a.pool = pool;
   a.bias = p.bias; a.y_hi = y_hi; a.y_lo = y_lo; a.y_f32 = y_f32;
   a.ssq = pool ? nullptr : ssq;
   a.ssq_stride = (long long)N * H * W;
-  a.acc_scale = tc_acc_scale(cin);
   if (ssq_parts) *ssq_parts = a.n_tiles;
 
   CUtensorMap m_xhi, m_xlo, m_whi, m_wlo;
@@ -606,16 +548,12 @@ int launch_conv3x3_tc(const __nv_bfloat16* x_hi, const __nv_bfloat16* x_lo, cons
   {
     uint64_t dims[3] = {(uint64_t)cin, (uint64_t)cout, 9};
     uint64_t str[2] = {(uint64_t)cin * 2, (uint64_t)cout * cin * 2};
-    uint32_t box[3] = {64, (uint32_t)(pair ? bn / 2 : bn), 1};
+    uint32_t box[3] = {64, (uint32_t)bn, 1};
     IBL_RET(make_tmap(&m_whi, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, p.w_hi, dims, str, box));
     IBL_RET(make_tmap(&m_wlo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, p.w_lo, dims, str, box));
   }
-  if (halo) {
-    if (bn == 64) return launch_tc_variant<64, 4, true, 3>(m_xhi, m_xlo, m_whi, m_wlo, a, pair, s);
-    return launch_tc_variant<128, 3, true, 2>(m_xhi, m_xlo, m_whi, m_wlo, a, pair, s);
-  }
-  if (bn == 64) return launch_tc_variant<64, 4>(m_xhi, m_xlo, m_whi, m_wlo, a, pair, s);
-  return launch_tc_variant<128, 3>(m_xhi, m_xlo, m_whi, m_wlo, a, pair, s);
+  if (halo) return launch_tc_variant<128, 3, true, 2>(m_xhi, m_xlo, m_whi, m_wlo, a, s);
+  return launch_tc_variant<64, 4>(m_xhi, m_xlo, m_whi, m_wlo, a, s);
 }
 
 // =====================================================================================================================
@@ -900,7 +838,6 @@ int launch_conv1_fused_tc(const float* x_nchw, const float* w1_oihw, const float
   a.total_tiles = (int)((long long)N * a.tiles_h * a.tiles_w);
   a.relu = 1; a.pool = 1;
   a.bias = p2.bias; a.y_hi = y_hi; a.y_lo = y_lo; a.y_f32 = nullptr; a.ssq = nullptr; a.ssq_stride = 0;
-  a.acc_scale = tc_acc_scale(64);
   CUtensorMap m_whi, m_wlo;
   {
     uint64_t dims[3] = {64, 64, 9};

@@ -12,8 +12,6 @@
 //
 // Work item = (row tile of 128, a run of column tiles, a run of K chunks); items are dealt
 // round-robin to a persistent grid.  Warp roles as in tc_conv.cu.
-#include <stdlib.h>
-
 #include "common.cuh"
 #include "tc_common.cuh"
 
@@ -270,29 +268,30 @@ static int launch_gemm_variant(const CUtensorMap* maps, const GemmTcArgs& g, cud
     IBL_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<BN, STAGES, EPI, MC>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     attr_done.mark();
   }
-  if (!MC) {
+  if constexpr (!MC) {
     const int grid = g.total_items < sm_count() ? g.total_items : sm_count();
     gemm_tc_kernel<BN, STAGES, EPI, false><<<grid, 160, smem, s>>>(maps[0], maps[1], maps[2], maps[3], g);
     IBL_CUDA_OK(cudaGetLastError());
     return IBL_OK;
+  } else {
+    // clusters of two CTAs; g.total_items counts PAIRS of row tiles
+    const int pairs = sm_count() / 2;
+    const int units = g.total_items < pairs ? g.total_items : pairs;
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(2 * units);
+    cfg.blockDim = dim3(160);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = s;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = 2;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    IBL_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BN, STAGES, EPI, true>, maps[0], maps[1], maps[2], maps[3], g));
+    return IBL_OK;
   }
-  // clusters of two CTAs; g.total_items counts PAIRS of row tiles
-  const int pairs = sm_count() / 2;
-  const int units = g.total_items < pairs ? g.total_items : pairs;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(2 * units);
-  cfg.blockDim = dim3(160);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = s;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  IBL_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BN, STAGES, EPI, true>, maps[0], maps[1], maps[2], maps[3], g));
-  return IBL_OK;
 }
 
 static int make_plane_maps(CUtensorMap* maps, const __nv_bfloat16* a_hi, const __nv_bfloat16* a_lo, int M,
@@ -326,58 +325,46 @@ static int pick_runs(int m_tiles, int n_tiles, int min_tiles_per_run, int units 
 }
 
 // Distance + running top-16 per (query, column run): cand_* [runs][M][16]; returns runs.
-// 128 x 128 tiles: the accumulator of one tile is 128 registers per consumer thread.
+// 128 x 128 tiles: the accumulator of one tile is 128 registers per consumer thread.  The engine calls it for
+// m <= 128 only (larger query sets take the single-pass screen of tc_dist1.cu), so it runs on ONE row tile and the
+// column runs alone spread it over the SMs.
 constexpr int DIST_BN = 128;
-
-// SM pairs (clusters of two CTAs sharing each database tile by TMA multicast) for the distance GEMMs.
-// IBL_GEMM_MC=1 forces them, =0 forbids them; unset, the dense GEMM uses them and the top-16 GEMM follows the caller
-// (`pairs`, IBL_DIST_2SM in the engine).  A single row tile always runs on one SM.
-static bool gemm_pairs(int m_tiles, bool pairs) {
-  static const int env = [] { const char* v = getenv("IBL_GEMM_MC"); return v ? (atoi(v) != 0 ? 1 : 0) : -1; }();
-  return m_tiles >= 2 && (env == 1 || (env == -1 && pairs));
-}
 
 int launch_dist_top16_tc(const __nv_bfloat16* q_hi, const __nv_bfloat16* q_lo, const float* qn, int m,
                          const __nv_bfloat16* d_hi, const __nv_bfloat16* d_lo, const float* dn, int n,
                          int n_valid, int K, float* cand_d, long long* cand_i, int max_runs, int* runs_out,
-                         bool pairs, cudaStream_t s) {
+                         cudaStream_t s) {
   IBL_REQUIRE(K % 64 == 0, "tensor-core distance needs dim % 64 == 0");
-  const int m_tiles = cdiv(m, GT_BM);
-  const bool mc = gemm_pairs(m_tiles, pairs);
+  IBL_REQUIRE(m >= 1 && m <= GT_BM, "top-16 distance GEMM takes one row tile (m <= 128)");
   CUtensorMap maps[4];
-  IBL_RET(make_plane_maps(maps, q_hi, q_lo, m, d_hi, d_lo, n, K, mc ? DIST_BN / 2 : DIST_BN));
+  IBL_RET(make_plane_maps(maps, q_hi, q_lo, m, d_hi, d_lo, n, K, DIST_BN));
   GemmTcArgs g{};
   g.M = m; g.N = n; g.K = K;
   g.n_tiles = cdiv(n_valid > 0 ? n_valid : 1, DIST_BN);
-  const int m_units = mc ? cdiv(m_tiles, 2) : m_tiles;
-  int runs = pick_runs(m_units, g.n_tiles, 2, mc ? sm_count() / 2 : 0);
+  int runs = pick_runs(1, g.n_tiles, 2);
   if (runs > max_runs) runs = max_runs;
   g.nt_per_item = cdiv(g.n_tiles, runs);
   g.items_per_mtile = cdiv(g.n_tiles, g.nt_per_item);
   g.kit_per_item = K / GT_BK;
-  g.total_items = m_units * g.items_per_mtile;
+  g.total_items = g.items_per_mtile;
   g.n_valid = n_valid;
   g.an = qn; g.bn = dn;
   g.cand_d = cand_d; g.cand_i = cand_i;
   *runs_out = g.items_per_mtile;
-  if (mc) return launch_gemm_variant<DIST_BN, 3, EPI_TOP16, true>(maps, g, s);
   return launch_gemm_variant<DIST_BN, 3, EPI_TOP16>(maps, g, s);
 }
 
-int dist_top16_max_runs(int m, int n_valid, bool pairs) {
-  const int m_tiles = cdiv(m, GT_BM);
-  const bool mc = gemm_pairs(m_tiles, pairs);
-  return pick_runs(mc ? cdiv(m_tiles, 2) : m_tiles, cdiv(n_valid > 0 ? n_valid : 1, DIST_BN), 2,
-                   mc ? sm_count() / 2 : 0);
-}
+int dist_top16_max_runs(int n_valid) { return pick_runs(1, cdiv(n_valid > 0 ? n_valid : 1, DIST_BN), 2); }
 
+// The dense distance GEMM runs on SM pairs (clusters of two CTAs sharing each database tile by TMA multicast)
+// whenever there are two row tiles to pair.
 int launch_dist_dense_tc(const __nv_bfloat16* q_hi, const __nv_bfloat16* q_lo, const float* qn, int m,
                          const __nv_bfloat16* d_hi, const __nv_bfloat16* d_lo, const float* dn, int n, int K,
                          float* out, long long ld_out, cudaStream_t s) {
   IBL_REQUIRE(K % 64 == 0, "tensor-core distance needs dim % 64 == 0");
   constexpr int BN = 128;
   const int m_tiles = cdiv(m, GT_BM);
-  const bool mc = gemm_pairs(m_tiles, true);
+  const bool mc = m_tiles >= 2;
   CUtensorMap maps[4];
   IBL_RET(make_plane_maps(maps, q_hi, q_lo, m, d_hi, d_lo, n, K, mc ? BN / 2 : BN));
   GemmTcArgs g{};

@@ -4,8 +4,6 @@
 // second NetVLAD contraction needs: vlad[c,k] = sum_s x^[s,c] a[s,k] reads the same [pixel][channel]
 // tile the first contraction (logits = x^ W^T, K-major) already staged, so the feature map is read
 // from HBM once.
-#include <stdlib.h>
-
 #include "common.cuh"
 #include "tc_common.cuh"
 
@@ -132,20 +130,9 @@ struct NvTcArgs {
   float* vlad_raw;                // [B][64][512] un-normalised VLAD (nullable)
   float* vlad_norm;               // [B][64*512] intra-normalised + L2-normalised descriptor (nullable)
   int* ticket;                    // [B] zero on entry; the unit that takes ticket G-1 finalises the image and resets it
-  unsigned long long* dbg;        // optional [gridDim][32] globaltimer stamps (IBL_NV_DEBUG=1)
 };
 
 constexpr int NV_STAGE = 65536, NV_NSTAGE = 3, NV_SLOT = 16384;
-
-__device__ __forceinline__ unsigned long long nv_now() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-  return t;
-}
-#define NV_STAMP(slot)                                                                    \
-  do {                                                                                    \
-    if (a.dbg && q == 0 && lane == 0 && (slot) < 32) a.dbg[blockIdx.x * 32 + (slot)] = nv_now(); \
-  } while (0)
 
 // The CTA's tiles in processing order: units blockIdx.x, +gridDim.x, ...; inside a unit tiles g, g+G, ...
 struct NvIter {
@@ -339,10 +326,8 @@ netvlad_tc_kernel(const __grid_constant__ CUtensorMap tm_xhi, const __grid_const
     int stage = 0; uint32_t phase = 0;
     auto release = [&](int st) { if (lane == 0) mbar_arrive(&empty_bar[st]); };
     float as0 = 0.f, as1 = 0.f;                  // sum_s a[s,k] for k = 2*lane, 2*lane+1 (this warp's rows)
-    int dslot = 1;
     NvIter cur;
     cur.init(blockIdx.x, gridDim.x, a.G, a.T, n_units);
-    NV_STAMP(0);
     for (int it = 0; cur.valid(); cur.next(), ++it) {
       const int unit = cur.u, b = unit / a.G;
       float* po = a.part + (long long)unit * 64 * 512;
@@ -384,7 +369,6 @@ netvlad_tc_kernel(const __grid_constant__ CUtensorMap tm_xhi, const __grid_const
           wgmma_wait<0>();
           zacc.fence_operands();
           release(prev);
-          NV_STAMP(dslot); ++dslot;                  // logits of this tile are ready
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             uint32_t r0[32];
@@ -426,7 +410,6 @@ netvlad_tc_kernel(const __grid_constant__ CUtensorMap tm_xhi, const __grid_const
         }
         fence_proxy_async();                       // generic-proxy smem writes -> visible to the tensor core
         wg_sync();                                 // every row of a' is written
-        NV_STAMP(dslot); ++dslot;                  // a' published
         // column sums of a over this warp's 32 rows: butterfly, lane L ends with columns 2L, 2L+1
         {
           float w32[32];
@@ -510,7 +493,6 @@ netvlad_tc_kernel(const __grid_constant__ CUtensorMap tm_xhi, const __grid_const
         asum_sm[q * 64 + 2 * lane] = as0;
         asum_sm[q * 64 + 2 * lane + 1] = as1;
         wg_sync();
-        NV_STAMP(dslot); ++dslot;                    // all MMAs of the unit retired
         if (threadIdx.x < 64) {
           const int k = threadIdx.x;
           a.asum_part[(long long)unit * 64 + k] = asum_sm[k] + asum_sm[64 + k] + asum_sm[128 + k] + asum_sm[192 + k];
@@ -526,15 +508,12 @@ netvlad_tc_kernel(const __grid_constant__ CUtensorMap tm_xhi, const __grid_const
           *flag_sm = lastu;
         }
         wg_sync();
-        NV_STAMP(dslot); ++dslot;                    // partial written
         if (*flag_sm) {
           __threadfence();
           nv_finalize_image(a, b, q, lane, asum_sm);
-          NV_STAMP(dslot); ++dslot;                  // image finalised
         }
         wg_sync();                                   // flag_sm / asum_sm are reused by the next unit
         as0 = 0.f; as1 = 0.f;
-        dslot = 1;
       }
     }
   }
@@ -577,12 +556,6 @@ int launch_netvlad_tc(const __nv_bfloat16* x_hi, const __nv_bfloat16* x_lo, int 
   a.ssq = ssq; a.ssq_parts = ssq_parts; a.normalize_input = normalize_input ? 1 : 0;
   a.part = part; a.asum_part = asum_part;
   a.cent = cent; a.vlad_raw = vlad_raw; a.vlad_norm = vlad_norm; a.ticket = ticket;
-  static unsigned long long* dbg_dev = nullptr;
-  static int dbg_on = -1;
-  if (dbg_on < 0) { const char* v = getenv("IBL_NV_DEBUG"); dbg_on = (v && atoi(v)) ? 1 : 0; }
-  if (dbg_on && !dbg_dev) { cudaMalloc(&dbg_dev, 256 * 32 * 8); }
-  if (dbg_on) cudaMemsetAsync(dbg_dev, 0, 256 * 32 * 8, s);
-  a.dbg = dbg_on ? dbg_dev : nullptr;
   const int smem = NV_NSTAGE * NV_STAGE + 2 * NV_SLOT + 1024 + 128 + 4 * 64 * 4 + 16;
   static DeviceOnce attr_done;   // the attribute is per device
   if (!attr_done.done()) {
@@ -593,18 +566,6 @@ int launch_netvlad_tc(const __nv_bfloat16* x_hi, const __nv_bfloat16* x_lo, int 
   const int units = B * a.G;
   netvlad_tc_kernel<<<units < sms ? units : sms, 160, smem, s>>>(mx_hi, mx_lo, mw_hi, mw_lo, a);
   IBL_CUDA_OK(cudaGetLastError());
-  if (dbg_on) {   // print phase stamps of a few CTAs (ns relative to the earliest stamp)
-    cudaStreamSynchronize(s);
-    static unsigned long long h[256 * 32];
-    cudaMemcpy(h, dbg_dev, sizeof(h), cudaMemcpyDeviceToHost);
-    unsigned long long t0 = ~0ull;
-    for (int i = 0; i < 256 * 32; ++i) if (h[i] && h[i] < t0) t0 = h[i];
-    for (int c : {0, 1, 60, 127}) {
-      fprintf(stderr, "[nv-debug] cta %3d:", c);
-      for (int j = 0; j < 12; ++j) fprintf(stderr, " %6lld", h[c * 32 + j] ? (long long)(h[c * 32 + j] - t0) : -1ll);
-      fprintf(stderr, "\n");
-    }
-  }
   return IBL_OK;
 }
 

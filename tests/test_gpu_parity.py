@@ -69,8 +69,8 @@ CONV_CASES = [
     (1, 35, 45, 64, 64, True, True),         # odd sizes: floor pooling, partial patches
     (2, 17, 23, 256, 512, False, False),     # no ReLU (conv5_3-like), two N tiles
     (1, 60, 80, 512, 512, True, True),
-    (1, 16, 24, 256, 256, True, False),      # 3 patches: the SM-pair kernel's last pair has an idle peer
-    (3, 30, 40, 512, 512, False, False),     # conv5-like, 30 patches, pair tiles + per-pixel sum of squares path
+    (1, 16, 24, 256, 256, True, False),      # 3 patches
+    (3, 30, 40, 512, 512, False, False),     # conv5-like, 30 patches
     (1, 33, 17, 128, 128, True, True),       # halo staging with ragged borders on both axes + fused pool
 ]
 
@@ -98,6 +98,26 @@ def test_conv3x3_layer_vs_oracle(eng, case):
         y = eng.debug_conv3x3(xd, w.cuda(), b.cuda(), relu=relu, pool=pool, mode=mode, bn=bn).cpu()
         assert y.shape == ref.shape, name
         assert rel_l2(y, ref) < tol, (name, rel_l2(y, ref))
+
+
+def test_umma_sw128_operand_accepts_unaligned_start_and_odd_group_stride():
+    """Halo staging reads nine tap views out of one TMA-written tile: starts that are 128-byte but not 1024-byte
+    aligned, 8-row groups 10 rows apart, descriptor base_offset = 0 (tensor-core MMA, here wgmma)."""
+    from openibl_b200.engine import Engine, _ptr, _stream
+    from openibl_b200._cabi import check
+    eng = Engine.get(0)
+    g = torch.Generator(device="cuda").manual_seed(5)
+    rows = 200
+    A = torch.randint(-8, 9, (rows, 64), device="cuda", generator=g).to(torch.bfloat16)
+    B = torch.randint(-8, 9, (64, 64), device="cuda", generator=g).to(torch.bfloat16)
+    D = torch.empty(128, 64, device="cuda")
+    m = torch.arange(128, device="cuda")
+    for group_rows, s0 in ((8, 0), (10, 0), (10, 1), (10, 11), (10, 22), (12, 3)):
+        idx = s0 + (m // 8) * group_rows + (m % 8)
+        want = A[idx].float() @ B.float().t()
+        check(eng.lib.ibl_debug_umma_strided(eng.h, _ptr(A), rows, _ptr(B), s0, group_rows, 0, _ptr(D), _stream(0)), "probe")
+        torch.cuda.synchronize()
+        assert torch.equal(D, want), (group_rows, s0)
 
 
 # ---------------------------------------------------------------------------------------------

@@ -6,7 +6,7 @@ select them cannot quietly skip one):
 
     0  exact fp32 on the CUDA cores      gemm mode 0, d % 64 != 0, or n_valid == 0
     1  single-pass fp16 screening        m > 128, k <= 12
-    2  bf16x3 screening, running top-16  m <= 128, k <= 12 (every m under IBL_DIST_SCREEN=3)
+    2  bf16x3 screening, running top-16  m <= 128, k <= 12
     3  bf16x3 dense tiles + row select   k > 12
 
 Every result is checked by `check_ranking` against fp64 distances, with a per-pair allowance for fp32 rounding
@@ -14,14 +14,12 @@ noise (see `noise` below) and no loose absolute tolerance.  The adversarial fami
 rounding errors are coherent across a row, so that a screening error bound that assumes independent element errors
 is wrong by orders of magnitude; they must still rank exactly."""
 import math
-import os
 
 import pytest
 import torch
 
 pytestmark = pytest.mark.gpu
 
-SCREEN3 = os.environ.get("IBL_DIST_SCREEN") == "3"
 PATH_NAMES = {0: "fp32", 1: "single-pass fp16", 2: "bf16x3 top-16", 3: "bf16x3 dense"}
 
 
@@ -37,7 +35,7 @@ def eng():
 def expected_path(mode, m, d, k, n_valid):
     if mode == 0 or d % 64 != 0 or n_valid == 0:
         return 0
-    if k <= 12 and m > 128 and not SCREEN3:
+    if k <= 12 and m > 128:
         return 1
     return 2 if k <= 12 else 3
 
@@ -179,7 +177,7 @@ def test_dims(eng, d):
         q, db = gallery(n, m, d, seed=d + m)
         for k in (1, 12, 13):
             paths = rank_all_paths(eng, q, db, k, what="dims")
-            tc = ({2} if SCREEN3 else {1, 2}) if k <= 12 else {3}
+            tc = {1, 2} if k <= 12 else {3}
             assert paths == ({0} if d % 64 else {0} | tc), paths
 
 

@@ -98,6 +98,33 @@ def test_conv1_1_backward_and_pool_backward(eng):
         assert torch.equal(gx.permute(0, 3, 1, 2).cpu(), ad.grad)
 
 
+@pytest.mark.parametrize("n_layers", [1, 2, 4])
+def test_vgg16_prefix_forward_vs_fp64(eng, n_layers):
+    """The frozen trunk prefix (train_layers='conv2' freezes layers [0, 2)) on an odd input, tensor-core mode, against
+    fp64 conv/ReLU/pool; rel-L2 <= 2e-5 as the per-layer tests.  1: the CUDA-core fp32 conv1_1.  2: the separate
+    tensor-core conv1_1 and the BN=64 conv1_2 with the fp32 epilogue and fused pool.  4: the fused conv1 kernel
+    feeding conv2_x with an fp32 output."""
+    from openibl_b200.engine import CONV_TC_BF16X3
+    ws, bs = _bind_vgg(eng)
+    x = torch.randn(2, 3, 70, 90, generator=torch.Generator().manual_seed(21))
+    ref = x.double()
+    for item in synth.VGG16_PLAN[: {1: 1, 2: 3, 4: 6}[n_layers]]:
+        if item == "P":
+            ref = torch.nn.functional.max_pool2d(ref, 2, 2)
+        else:
+            i = synth.VGG16_CONV_SLOTS.index(item[0])
+            ref = torch.nn.functional.conv2d(ref, ws[i].cpu().double(), bs[i].cpu().double(), padding=1).relu()
+    mode = eng.conv_mode
+    eng.conv_mode = CONV_TC_BF16X3
+    try:
+        y = eng.vgg16_prefix_forward(x.cuda(), n_layers)
+    finally:
+        eng.conv_mode = mode
+    assert y.shape == ref.permute(0, 2, 3, 1).shape
+    err = rel_l2(y.permute(0, 3, 1, 2).cpu(), ref)
+    assert err < 2e-5, err
+
+
 def _freeze_below_conv5(model):
     for layer in list(model.base_model.base.children())[:24]:
         for p in layer.parameters():

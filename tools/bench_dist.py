@@ -1,6 +1,5 @@
 #!/usr/bin/env python
-"""Times Engine.l2dist_topk (BASELINE configs[2] shape by default) with CUDA events; env switches select the kernel
-variant (IBL_DIST_BN=256|512, IBL_DIST_SCREEN=3), so run it once per variant."""
+"""Times Engine.l2dist_topk (BASELINE configs[2] shape by default) with CUDA events."""
 import os, sys, json
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -24,6 +23,6 @@ torch.cuda.synchronize()
 ms = e0.elapsed_time(e1) / reps
 exact = 2 - 2 * (qd[::97].double() @ dbd.double().t())
 wi = exact.topk(k, largest=False).indices
-print(json.dumps({"variant": {v: os.environ.get(v) for v in ("IBL_DIST_BN", "IBL_DIST_SCREEN")}, "m": m, "n": n, "d": d,
+print(json.dumps({"m": m, "n": n, "d": d,
                   "ms": ms, "pairs_per_s": m * n / ms * 1e3, "algorithmic_tflops": 2.0 * m * n * d / ms / 1e9,
                   "agree_fp64_subset": float((ik[::97] == wi).float().mean()), "flagged": eng.dist_flagged()}), flush=True)

@@ -1,5 +1,5 @@
 """Per-layer device times of the VGG16 backbone at batch 32, 480x640 (same process, CUDA events):
-conv1_1 on the CUDA cores, conv1_2..conv5_3 on the tensor cores (wgmma) with each admissible N tile."""
+conv1_1 and conv1_2..conv5_3 on the tensor cores (wgmma), the latter with each admissible N tile."""
 import ctypes, json, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -25,7 +25,7 @@ print(f"{'layer':8s} {'HxW':>9s} {'Cin':>4s} {'Cout':>4s} {'BN':>4s} {'ms':>8s} 
 for li, (hh, ww, cin, cout) in enumerate(shapes):
     if li == 0:
         x = torch.randn(B, 3, hh, ww, device="cuda")
-        bns = [0, 1]   # 0 = tensor-core conv1_1, 1 = CUDA-core conv1_1
+        bns = [0]
     else:
         x = torch.randn(B, hh, ww, cin, device="cuda").relu_()
         bns = [b for b in (64, 128) if cout % b == 0]

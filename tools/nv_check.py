@@ -1,6 +1,5 @@
 """Fused NetVLAD kernel check + timing (GPU): tensor-core path (nhwc) against the fp32 CUDA-core path (nchw) for a
-few shapes, then the device time of the kernels at B=32, S=1200 (cold L2 between reps: 256 MB scratch write).
-IBL_NV_CLUSTER=0 selects the one-SM kernel."""
+few shapes, then the device time of the kernels at B=32, S=1200 (cold L2 between reps: 256 MB scratch write)."""
 import os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -236,6 +236,16 @@ int ibl_knn_rowmax(ibl_engine* e, const float* X, int N, int d, int row0, int n_
 int ibl_rerank_topk(ibl_engine* e, const float* X, int N, int m, int d, const int64_t* nbr_idx, const float* nbr_dist,
                     int w, const float* rowmax, int k1, int k2, float lambda_value, const int64_t* orig_idx, int k_orig,
                     int k, float* out_dist, int64_t* out_idx, void* stream);
+/* The reference function itself, ibl/utils/rerank.py:30-100, on dense distance matrices: qg [m,n], qq [m,m] and
+ * gg [n,n], row-major fp32 device pointers -> out_final [m,n], the reference's final_dist.  With D = [[qq, qg],
+ * [qg^T, gg]] the reference squares D, divides every column by its maximum and transposes (rerank.py:41-42), so
+ * q(i,j) = D[j][i]^2 / max_r D[r][i]^2: the inputs are read that way and need not be symmetric.  Neighbour lists of
+ * w = max(k1 + 1, k2) columns ascending by (q, index), then the sparse stage of ibl_rerank_topk, then
+ * final = fl(fl(jac * fp32(1 - lambda)) + fl(q * fp32(lambda))), with 1 - lambda taken in double.  Needs m, n >= 1,
+ * m + n >= k1 + 1, k2 >= 1, w <= 128.  Workspace O((m+n) w) plus the sparse stage: nothing of size [N,N] or beyond
+ * the caller's arrays.  Synchronises the stream three to five times; bit-identical from run to run. */
+int ibl_rerank_dense(ibl_engine* e, const float* qg, const float* qq, const float* gg, int m, int n, int k1, int k2,
+                     double lambda_value, float* out_final, void* stream);
 
 /* C[m,n] = alpha * A[m,k] . B[n,k]^T on the engine's GEMM kernels: the products of PCA.train (pca.py:38-67,
  * torch.matmul there).  mode IBL_CONV_SIMT_FP32 (fp32 CUDA cores) or IBL_CONV_TC_BF16X3 (tensor cores, k % 64 == 0). */

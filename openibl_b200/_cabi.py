@@ -6,7 +6,7 @@ from __future__ import annotations
 
 import ctypes
 import os
-from ctypes import POINTER, c_char_p, c_float, c_int, c_int64, c_uint, c_uint64, c_void_p
+from ctypes import POINTER, c_char_p, c_double, c_float, c_int, c_int64, c_uint, c_uint64, c_void_p
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libiblb200.so")
@@ -60,6 +60,7 @@ SIGNATURES = {
     "ibl_knn_rowmax": (c_int, [_P, _P, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P]),
     "ibl_rerank_topk": (c_int, [_P, _P, c_int, c_int, c_int, _P, _P, c_int, _P, c_int, c_int, c_float, _P, c_int,
                                 c_int, _P, _P, _P]),
+    "ibl_rerank_dense": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, c_double, _P, _P]),
     "ibl_debug_rerank_workspace_bytes": (c_int, [_P, POINTER(c_uint64)]),
     "ibl_debug_knn_flagged": (c_int, [_P, POINTER(c_int), _P]),
     "ibl_gemm_nt": (c_int, [_P, _P, c_int, _P, c_int, c_int, c_float, _P, c_int, _P]),

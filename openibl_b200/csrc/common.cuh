@@ -213,6 +213,8 @@ size_t rerank_ws_bytes(const RerankWs* w);
 int launch_rerank_topk(RerankWs* W, const float* X, int N, int m, int d, const long long* nbr, const float* nbr_dist,
                        int w, const float* rowmax, int k1, int k2, float lam, const long long* orig, int k_orig, int k,
                        float* out_dist, long long* out_idx, uint64_t* launches, cudaStream_t s);
+int launch_rerank_dense(RerankWs* W, const float* qg, const float* qq, const float* gg, int m, int n, int k1, int k2,
+                        double lam, float* out, uint64_t* launches, cudaStream_t s);
 
 // topk.cu
 int launch_topk_rows(const float* dist, long long ld, int m, int n_valid, int k, int64_t idx_base,

@@ -1140,6 +1140,21 @@ int ibl_rerank_topk(ibl_engine* e, const float* X, int N, int m, int d, const in
                             &e->launches, S(stream));
 }
 
+// k-reciprocal re-ranking of dense distance matrices, the reference function's own call (ibl/utils/rerank.py:30-100)
+int ibl_rerank_dense(ibl_engine* e, const float* qg, const float* qq, const float* gg, int m, int n, int k1, int k2,
+                     double lambda_value, float* out_final, void* stream) {
+  IBL_REQUIRE(e && qg && qq && gg && out_final, "null argument");
+  IBL_REQUIRE(m >= 1 && n >= 1, "bad shape (m >= 1, n >= 1)");
+  IBL_REQUIRE(k1 >= 0 && k2 >= 1, "re-ranking: k1 >= 0, k2 >= 1");
+  IBL_REQUIRE((long long)m + n >= k1 + 1, "re-ranking needs at least k1 + 1 images");
+  IBL_REQUIRE((k1 + 1 > k2 ? k1 + 1 : k2) <= 128, "dense re-ranking: max(k1 + 1, k2) <= 128");
+  IBL_REQUIRE(k2 <= m + n, "dense re-ranking: k2 <= m + n");
+  IBL_REQUIRE(lambda_value >= 0.0 && lambda_value <= 1.0, "re-ranking: 0 <= lambda <= 1");
+  DeviceGuard g(e->device);
+  if (!e->rr_ws) e->rr_ws = rerank_ws_create();
+  return launch_rerank_dense(e->rr_ws, qg, qq, gg, m, n, k1, k2, lambda_value, out_final, &e->launches, S(stream));
+}
+
 // test hook: rows of the last ibl_knn_rowmax call that the guards sent to the exact scan (-1: no call yet).
 // Synchronises the stream.
 int ibl_debug_knn_flagged(ibl_engine* e, int* count, void* stream) {

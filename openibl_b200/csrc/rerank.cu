@@ -19,6 +19,13 @@
 //        top-k        over the overlap rows plus the rows that can precede every other one: the first k_orig rows
 //                     of the original ranking (lambda > 0) or the lowest-index rows without overlap (lambda = 0).
 //      No floating-point sum depends on scheduling: results are bit-identical from run to run.
+//   3. dense entry (launch_rerank_dense), the reference function's own call shape: q-g, q-q and g-g distance matrices
+//      in, the full [m,n] final matrix out.  D = [[qq, qg], [qg^T, gg]]; the reference squares D, divides every COLUMN
+//      by its maximum and transposes (rerank.py:41-42), so row i of its matrix is column i of D, q(i,j) = D[j][i]^2 / M_i
+//      with M_i = max_r D[r][i]^2.  Every read below is D[j][i]: the q-q and g-g inputs need not be bitwise symmetric.
+//        neighbour pass  dn_knn_kernel: per column of D, M_i and the first w rows ascending by (q, index)
+//        sparse stage    as above, the expansion reading the distances it recomputes from D (rr_expand_kernel<1, true>)
+//        output          every entry (1 - lambda) + lambda q, then the overlap pairs overwritten with their Jaccard term
 #include <cub/cub.cuh>
 
 #include <algorithm>
@@ -389,6 +396,121 @@ int launch_knn_rowmax(const float* X, int N, int d, int row0, int n_rows, int w,
 }
 
 // ------------------------------------------------------------------------------------------------------------------
+// 1b. neighbour pass over dense distance matrices (launch_rerank_dense)
+// ------------------------------------------------------------------------------------------------------------------
+
+// D = [[qq, qg], [qg^T, gg]] of m queries and n gallery rows, every input row-major fp32
+struct DenseSrc {
+  const float* qg; const float* qq; const float* gg;
+  int m, n;
+};
+
+// D[r][c]
+__device__ __forceinline__ float dense_at(const DenseSrc& s, long long r, long long c) {
+  if (r < s.m) return c < s.m ? s.qq[r * s.m + c] : s.qg[r * s.n + (c - s.m)];
+  return c < s.m ? s.qg[c * s.n + (r - s.m)] : s.gg[(r - s.m) * s.n + (c - s.m)];
+}
+
+constexpr int DN_WARPS = 4;          // row slices per block of 32 columns
+
+// tile[k][l] = D[r0 + k][c0 + l] for the entries inside D.  Every input is read along its rows: the qg^T block (rows
+// >= m, columns < m) as rows of qg, stored transposed.
+__device__ __forceinline__ void dn_load_tile(const DenseSrc& s, int N, int r0, int c0, int lane, float (*tile)[33]) {
+  __syncwarp();
+  if (!(r0 >= s.m && c0 + 31 < s.m)) {
+#pragma unroll 4
+    for (int k = 0; k < 32; ++k) {
+      const int r = r0 + k, c = c0 + lane;
+      if (r < N && c < N && !(r >= s.m && c < s.m)) tile[k][lane] = dense_at(s, r, c);
+    }
+  }
+  if (r0 + 31 >= s.m && c0 < s.m) {
+#pragma unroll 4
+    for (int k = 0; k < 32; ++k) {
+      const int r = r0 + lane, c = c0 + k;
+      if (r < N && c < N && r >= s.m && c < s.m) tile[lane][k] = dense_at(s, r, c);
+    }
+  }
+  __syncwarp();
+}
+
+// One block of DN_WARPS warps per 32 columns c0 .. c0+31 of D (rows of the reference's matrix), lane l on column
+// c0 + l; warp v streams down the 32-row tiles v, v + DN_WARPS, ...
+//   sweep 1: M_c = max_r fl(D[r][c]^2)
+//   sweep 2: keys (bits of q = fl(D[r][c]^2) / M_c, r), the slice's first w kept sorted in shared memory.  q >= 0, so
+//            its bits order like the value; a later row never displaces an equal q, as in a stable sort.
+// The DN_WARPS slices are merged per column -> idx [N,w], D[idx][c] [N,w], M [N]: the layout of launch_knn_rowmax.
+__global__ void __launch_bounds__(DN_WARPS * 32)
+dn_knn_kernel(const DenseSrc s, int w, long long* __restrict__ out_idx, float* __restrict__ out_dist,
+              float* __restrict__ out_max) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  unsigned long long* lst = reinterpret_cast<unsigned long long*>(smem);                 // [DN_WARPS][w][32]
+  float(*tiles)[32][33] = reinterpret_cast<float(*)[32][33]>(lst + (size_t)DN_WARPS * w * 32);
+  __shared__ float wmax[DN_WARPS][32];
+  const int N = s.m + s.n;
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  const int c0 = blockIdx.x * 32;
+  float(*tile)[33] = tiles[wid];
+  float mx = 0.f;
+  for (int r0 = wid * 32; r0 < N; r0 += DN_WARPS * 32) {
+    dn_load_tile(s, N, r0, c0, lane, tile);
+    const int nr = min(32, N - r0);
+    for (int k = 0; k < nr; ++k) {
+      const float v = tile[k][lane];
+      mx = fmaxf(mx, __fmul_rn(v, v));
+    }
+  }
+  wmax[wid][lane] = mx;
+  unsigned long long* my = lst + (size_t)wid * w * 32 + lane;         // slot t at my[t * 32]
+  for (int t = 0; t < w; ++t) my[t * 32] = ~0ull;
+  __syncthreads();
+  float M = wmax[0][lane];
+#pragma unroll
+  for (int v = 1; v < DN_WARPS; ++v) M = fmaxf(M, wmax[v][lane]);
+  unsigned long long thr = ~0ull;                                      // the slice's w-th key
+  for (int r0 = wid * 32; r0 < N; r0 += DN_WARPS * 32) {
+    dn_load_tile(s, N, r0, c0, lane, tile);
+    const int nr = min(32, N - r0);
+#pragma unroll 1
+    for (int k = 0; k < nr; ++k) {
+      const float v = tile[k][lane];
+      const unsigned long long key =
+          ((unsigned long long)__float_as_uint(__fdiv_rn(__fmul_rn(v, v), M)) << 32) | (unsigned)(r0 + k);
+      if (key < thr) {
+        int p = w - 1;
+        while (p > 0 && my[(p - 1) * 32] > key) {
+          my[p * 32] = my[(p - 1) * 32];
+          --p;
+        }
+        my[p * 32] = key;
+        thr = my[(w - 1) * 32];
+      }
+    }
+  }
+  __syncthreads();
+  const int c = c0 + lane;
+  if (wid != 0 || c >= N) return;
+  int h[DN_WARPS] = {};
+  for (int t = 0; t < w; ++t) {
+    unsigned long long best = ~0ull;
+    int bv = 0;
+#pragma unroll
+    for (int v = 0; v < DN_WARPS; ++v) {
+      const unsigned long long k = h[v] < w ? lst[((size_t)v * w + h[v]) * 32 + lane] : ~0ull;
+      if (k < best) { best = k; bv = v; }
+    }
+#pragma unroll
+    for (int v = 0; v < DN_WARPS; ++v) h[v] += (v == bv);
+    const long long r = best == ~0ull ? -1 : (long long)(uint32_t)(best & 0xffffffffu);
+    out_idx[(long long)c * w + t] = r;
+    out_dist[(long long)c * w + t] = r < 0 ? INFINITY : dense_at(s, r, c);
+  }
+  out_max[c] = M;
+}
+
+static size_t dn_knn_smem(int w) { return (size_t)DN_WARPS * w * 32 * 8 + (size_t)DN_WARPS * 32 * 33 * 4; }
+
+// ------------------------------------------------------------------------------------------------------------------
 // 2. sparse stage
 // ------------------------------------------------------------------------------------------------------------------
 
@@ -425,10 +547,12 @@ struct ExpandArgs {
   int N, cap;                                  // cap: power of two >= wr * (wc + 1)
   int* nnz;                                    // pass 0: [N] sizes
   const long long* rowptr; int* cols; float* vals;   // pass 1
+  DenseSrc dn;                                 // DENSE: the distances are read from D instead (x, d, sq unused)
 };
 
-// E_i and V_i for one row per block (128 threads).  pass 0 counts |E_i|, pass 1 writes the CSR row.
-template <int PASS>
+// E_i and V_i for one row per block (128 threads).  pass 0 counts |E_i|, pass 1 writes the CSR row.  A distance that
+// is not in the neighbour list comes from the descriptors (d1_exact) or, DENSE, from D[j][i].
+template <int PASS, bool DENSE = false>
 __global__ void __launch_bounds__(128)
 rr_expand_kernel(const ExpandArgs g) {
   extern __shared__ __align__(16) unsigned char smem[];
@@ -502,7 +626,10 @@ rr_expand_kernel(const ExpandArgs g) {
         const unsigned bal = __ballot_sync(0xffffffffu, hit);
         if (bal) { e = g.nbr_dist[(long long)i * g.w + q0 + __ffs(bal) - 1]; found = true; break; }
       }
-      if (!found) e = d1_exact(xr, g.x + (long long)j * g.d, g.d, lane, an, __ldg(g.sq + j));
+      if (!found) {
+        if constexpr (DENSE) e = dense_at(g.dn, j, i);
+        else e = d1_exact(xr, g.x + (long long)j * g.d, g.d, lane, an, __ldg(g.sq + j));
+      }
       if (lane == 0) val[t] = expf(-__fdiv_rn(__fmul_rn(e, e), M));
     }
     __syncthreads();
@@ -760,6 +887,39 @@ rr_topk_kernel(const TopkArgs g) {
   }
 }
 
+// final = fl(fl(jac * c1) + fl(q * c2)), c1 = fp32(1 - lambda), c2 = fp32(lambda): rerank.py:94 in float32 (NEP 50).
+// Separate roundings: a contracted FMA is one ulp off the reference.
+__device__ __forceinline__ float rr_dense_final(float jac, float q, float c1, float c2) {
+  return __fadd_rn(__fmul_rn(jac, c1), __fmul_rn(q, c2));
+}
+
+// every (query i, gallery j) with jac = 1, q = fl(qg[i][j]^2) / M_i (D[m+j][i] is qg[i][j])
+__global__ void rr_dense_base_kernel(const float* __restrict__ qg, const float* __restrict__ rowmax, int m, int n,
+                                     float c1, float c2, float* __restrict__ out) {
+  const long long total = (long long)m * n;
+  for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x; p < total; p += (long long)gridDim.x * blockDim.x) {
+    const int i = (int)(p / n);
+    const float v = __ldg(qg + p);
+    out[p] = rr_dense_final(1.f, __fdiv_rn(__fmul_rn(v, v), __ldg(rowmax + i)), c1, c2);
+  }
+}
+
+// the overlap pairs of a query chunk: t at the first position of each (query, row) run (rr_segment_sum_kernel).  Each
+// pair is written once, so the output does not depend on scheduling.
+__global__ void rr_dense_scatter_kernel(const unsigned long long* __restrict__ keys, const float* __restrict__ t,
+                                        long long T, int q0, long long n_gal, const float* __restrict__ qg,
+                                        const float* __restrict__ rowmax, float c1, float c2, float* __restrict__ out) {
+  const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= T) return;
+  const float tp = t[p];
+  if (tp < 0.f) return;
+  const unsigned long long k = keys[p];
+  const long long i = q0 + (long long)(k / (unsigned long long)n_gal), r = (long long)(k % (unsigned long long)n_gal);
+  const float jac = __fsub_rn(1.f, __fdiv_rn(tp, __fsub_rn(2.f, tp)));   // rerank.py:92
+  const float v = qg[i * n_gal + r];
+  out[i * n_gal + r] = rr_dense_final(jac, __fdiv_rn(__fmul_rn(v, v), rowmax[i]), c1, c2);
+}
+
 // |x|^2 in planes_sqnorm_kernel's summation order (gemm_simt.cu), so that a distance recomputed here is bit-identical
 // to the neighbour pass's distance of the same pair
 __global__ void __launch_bounds__(256)
@@ -807,21 +967,22 @@ struct RrBuf {
 
 struct RerankWs {
   RrBuf sets, nnz, rowptr, cols, vals, cols2, vals2, inv_v2, colptr, qcnt, qoff, pk, pk2, pv,
-      pv2, tsum, temp, xpad, sq, dmax;
+      pv2, tsum, temp, xpad, sq, dmax,
+      dn;   // launch_rerank_dense: neighbour lists, their distances and the row maxima
 };
 
 RerankWs* rerank_ws_create() { return new RerankWs(); }
 void rerank_ws_destroy(RerankWs* w) {
   if (!w) return;
   RrBuf* all[] = {&w->sets, &w->nnz, &w->rowptr, &w->cols, &w->vals, &w->cols2, &w->vals2, &w->inv_v2, &w->colptr, &w->qcnt, &w->qoff, &w->pk, &w->pk2, &w->pv,
-                  &w->pv2, &w->tsum, &w->temp, &w->xpad, &w->sq, &w->dmax};
+                  &w->pv2, &w->tsum, &w->temp, &w->xpad, &w->sq, &w->dmax, &w->dn};
   for (RrBuf* b : all)
     if (b->p) cudaFree(b->p);
   delete w;
 }
 size_t rerank_ws_bytes(const RerankWs* w) {
   const RrBuf* all[] = {&w->sets, &w->nnz, &w->rowptr, &w->cols, &w->vals, &w->cols2, &w->vals2, &w->inv_v2, &w->colptr, &w->qcnt, &w->qoff, &w->pk, &w->pk2, &w->pv,
-                        &w->pv2, &w->tsum, &w->temp, &w->xpad, &w->sq, &w->dmax};
+                        &w->pv2, &w->tsum, &w->temp, &w->xpad, &w->sq, &w->dmax, &w->dn};
   size_t s = 0;
   for (const RrBuf* b : all) s += b->cap;
   return s;
@@ -852,23 +1013,33 @@ static int csr_rows(RerankWs* W, const int* nnz, int N, RrBuf& rowptr, long long
   return IBL_OK;
 }
 
-int launch_rerank_topk(RerankWs* W, const float* X, int N, int m, int d, const long long* nbr, const float* nbr_dist,
-                       int w, const float* rowmax, int k1, int k2, float lam, const long long* orig, int k_orig, int k,
-                       float* out_dist, long long* out_idx, uint64_t* launches, cudaStream_t s) {
+// Shared-memory limits of the kernels a path launches, set once per device.  Each path sets only its own kernels:
+// setting an attribute loads the kernel's module, which the other path need not pay for.
+template <bool DENSE>
+static int rr_set_attributes() {
+  static DeviceOnce attr;
+  if (attr.done()) return IBL_OK;
+  IBL_CUDA_OK(cudaFuncSetAttribute(rr_expand_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+  IBL_CUDA_OK(cudaFuncSetAttribute(rr_expand_kernel<1, DENSE>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+  IBL_CUDA_OK(cudaFuncSetAttribute(rr_mean_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+  IBL_CUDA_OK(cudaFuncSetAttribute(rr_mean_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+  if (DENSE)
+    IBL_CUDA_OK(cudaFuncSetAttribute(dn_knn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dn_knn_smem(128)));
+  attr.mark();
+  return IBL_OK;
+}
+
+// The sparse stage from the [N,w] lists and M of all rows (ea: the distance source, nbr, nbr_dist, w, rowmax) up to
+// the Jaccard sums.  For every chunk [q0, q1) of queries, emit(q0, q1, base, T) runs with the T stably sorted
+// (query - q0, row) keys in W->pk2, t at the first position of each run in W->tsum (-1 elsewhere) and the chunk's
+// offsets qoff[q0..q1] - base in W->qoff.
+template <bool DENSE, class Emit>
+static int rerank_sparse(RerankWs* W, ExpandArgs ea, int N, int m, int k1, int k2, uint64_t& nl, cudaStream_t s,
+                         Emit&& emit) {
   const int wr = k1 + 1, wc = half_round_even(k1) + 1;
   const long long n_gal = (long long)N - m;
-  uint64_t nl = 0;
-  // the exact routine wants rows of a multiple of 4 floats
-  const int dp = (d + 3) / 4 * 4;
-  const float* x = X;
-  if (dp != d) {
-    IBL_RET(W->xpad.ensure((size_t)N * dp * 4));
-    IBL_CUDA_OK(cudaMemsetAsync(W->xpad.p, 0, (size_t)N * dp * 4, s));
-    IBL_CUDA_OK(cudaMemcpy2DAsync(W->xpad.p, (size_t)dp * 4, X, (size_t)d * 4, (size_t)d * 4, N, cudaMemcpyDeviceToDevice, s));
-    x = W->xpad.as<float>();
-  }
-  IBL_RET(W->sq.ensure((size_t)N * 4));
-  rr_sqnorm_kernel<<<N, 256, 0, s>>>(x, dp, W->sq.as<float>());
+  const long long* nbr = ea.nbr;
+  const int w = ea.w;
   // k-reciprocal sets
   IBL_RET(W->sets.ensure((size_t)N * (wr + wc + 2) * 4));
   int* kr = W->sets.as<int>();
@@ -880,20 +1051,11 @@ int launch_rerank_topk(RerankWs* W, const float* X, int N, int m, int d, const l
   IBL_CUDA_OK(cudaGetLastError());
   nl += 3;
   // expansion + V
-  ExpandArgs ea{};
-  ea.x = x; ea.d = dp; ea.sq = W->sq.as<float>(); ea.nbr = nbr; ea.nbr_dist = nbr_dist; ea.w = w; ea.rowmax = rowmax;
   ea.kr = kr; ea.kr_cnt = krc; ea.wr = wr; ea.kc = kc; ea.kc_cnt = kcc; ea.wc = wc; ea.N = N;
   ea.cap = pow2_at_least((long long)wr * (wc + 1));
   const size_t esm = (size_t)ea.cap * 8 + (size_t)wr * 4;
   IBL_REQUIRE(esm <= 200 * 1024, "re-ranking: k1 too large for the expansion kernel's shared memory");
-  static DeviceOnce attr;
-  if (!attr.done()) {
-    IBL_CUDA_OK(cudaFuncSetAttribute(rr_expand_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    IBL_CUDA_OK(cudaFuncSetAttribute(rr_expand_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    IBL_CUDA_OK(cudaFuncSetAttribute(rr_mean_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    IBL_CUDA_OK(cudaFuncSetAttribute(rr_mean_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    attr.mark();
-  }
+  IBL_RET(rr_set_attributes<DENSE>());
   IBL_RET(W->nnz.ensure((size_t)N * 4));
   ea.nnz = W->nnz.as<int>();
   rr_expand_kernel<0><<<N, 128, esm, s>>>(ea);
@@ -904,7 +1066,7 @@ int launch_rerank_topk(RerankWs* W, const float* X, int N, int m, int d, const l
   IBL_RET(W->cols.ensure((size_t)nnz * 4));
   IBL_RET(W->vals.ensure((size_t)nnz * 4));
   ea.rowptr = W->rowptr.as<long long>(); ea.cols = W->cols.as<int>(); ea.vals = W->vals.as<float>();
-  rr_expand_kernel<1><<<N, 128, esm, s>>>(ea);
+  rr_expand_kernel<1, DENSE><<<N, 128, esm, s>>>(ea);
   IBL_CUDA_OK(cudaGetLastError());
   nl += 4;
   const long long* rowptr = W->rowptr.as<long long>();
@@ -980,7 +1142,6 @@ int launch_rerank_topk(RerankWs* W, const float* X, int N, int m, int d, const l
   for (int i = 0; i < m; ++i) qo[i + 1] = qo[i] + qc[i];
   IBL_CUDA_OK(cudaMemcpyAsync(W->qoff.p, qo.data(), (size_t)(m + 1) * 8, cudaMemcpyHostToDevice, s));
   const long long budget = 1ll << 22;            // pairs sorted at once (4M: ~100 MB with the sort's buffers)
-  const float oml = (float)(1.0 - (double)lam);  // numpy casts the scalar (1 - lambda) to float32
   for (int q0 = 0; q0 < m;) {
     int q1 = q0 + 1;
     while (q1 < m && qo[q1 + 1] - qo[q0] <= budget && q1 - q0 < 65535) ++q1;
@@ -1011,16 +1172,77 @@ int launch_rerank_topk(RerankWs* W, const float* X, int N, int m, int d, const l
       IBL_CUDA_OK(cudaGetLastError());
       nl += 3;
     }
+    IBL_RET(emit(q0, q1, qo[q0], T));
+    q0 = q1;
+  }
+  return IBL_OK;
+}
+
+int launch_rerank_topk(RerankWs* W, const float* X, int N, int m, int d, const long long* nbr, const float* nbr_dist,
+                       int w, const float* rowmax, int k1, int k2, float lam, const long long* orig, int k_orig, int k,
+                       float* out_dist, long long* out_idx, uint64_t* launches, cudaStream_t s) {
+  const long long n_gal = (long long)N - m;
+  uint64_t nl = 0;
+  // the exact routine wants rows of a multiple of 4 floats
+  const int dp = (d + 3) / 4 * 4;
+  const float* x = X;
+  if (dp != d) {
+    IBL_RET(W->xpad.ensure((size_t)N * dp * 4));
+    IBL_CUDA_OK(cudaMemsetAsync(W->xpad.p, 0, (size_t)N * dp * 4, s));
+    IBL_CUDA_OK(cudaMemcpy2DAsync(W->xpad.p, (size_t)dp * 4, X, (size_t)d * 4, (size_t)d * 4, N, cudaMemcpyDeviceToDevice, s));
+    x = W->xpad.as<float>();
+  }
+  IBL_RET(W->sq.ensure((size_t)N * 4));
+  rr_sqnorm_kernel<<<N, 256, 0, s>>>(x, dp, W->sq.as<float>());
+  ExpandArgs ea{};
+  ea.x = x; ea.d = dp; ea.sq = W->sq.as<float>(); ea.nbr = nbr; ea.nbr_dist = nbr_dist; ea.w = w; ea.rowmax = rowmax;
+  const float oml = (float)(1.0 - (double)lam);  // numpy casts the scalar (1 - lambda) to float32
+  IBL_RET(rerank_sparse<false>(W, ea, N, m, k1, k2, nl, s, [&](int q0, int q1, long long base, long long) -> int {
     TopkArgs ta{};
     ta.x = x; ta.d = dp; ta.sq = W->sq.as<float>(); ta.rowmax = rowmax; ta.m = m; ta.n_gal = n_gal;
     ta.keys = W->pk2.as<unsigned long long>(); ta.t = W->tsum.as<float>(); ta.qoff = W->qoff.as<long long>();
-    ta.base = qo[q0]; ta.q0 = q0; ta.orig = orig; ta.k_orig = k_orig; ta.lam = lam; ta.oml = oml; ta.k = k;
+    ta.base = base; ta.q0 = q0; ta.orig = orig; ta.k_orig = k_orig; ta.lam = lam; ta.oml = oml; ta.k = k;
     ta.out_dist = out_dist; ta.out_idx = out_idx;
     rr_topk_kernel<<<q1 - q0, 256, 0, s>>>(ta);
     IBL_CUDA_OK(cudaGetLastError());
     nl += 1;
-    q0 = q1;
-  }
+    return IBL_OK;
+  }));
+  if (launches) *launches += nl;
+  return IBL_OK;
+}
+
+int launch_rerank_dense(RerankWs* W, const float* qg, const float* qq, const float* gg, int m, int n, int k1, int k2,
+                        double lam, float* out, uint64_t* launches, cudaStream_t s) {
+  const int N = m + n, w = std::max(k1 + 1, k2);
+  IBL_REQUIRE(w <= 128 && w <= N, "dense re-ranking: max(k1 + 1, k2) <= min(128, m + n)");
+  IBL_RET(rr_set_attributes<true>());
+  uint64_t nl = 0;
+  // neighbour lists [N,w] int64, their D[j][i] [N,w] and M [N]
+  IBL_RET(W->dn.ensure((size_t)N * w * 12 + (size_t)N * 4));
+  long long* nbr = W->dn.as<long long>();
+  float* nd = reinterpret_cast<float*>(nbr + (size_t)N * w);
+  float* mx = nd + (size_t)N * w;
+  const DenseSrc src{qg, qq, gg, m, n};
+  dn_knn_kernel<<<cdiv(N, 32), DN_WARPS * 32, dn_knn_smem(w), s>>>(src, w, nbr, nd, mx);
+  IBL_CUDA_OK(cudaGetLastError());
+  // 1 - lambda in double, then float32: numpy's (1 - lambda_value) is a Python float cast to the array's type
+  const float c1 = (float)(1.0 - lam), c2 = (float)lam;
+  rr_dense_base_kernel<<<std::min(cdiv((long long)m * n, 256), 32 * device_sm_count()), 256, 0, s>>>(qg, mx, m, n, c1,
+                                                                                                      c2, out);
+  IBL_CUDA_OK(cudaGetLastError());
+  nl += 2;
+  ExpandArgs ea{};
+  ea.sq = mx;   // not read with a dense source; a valid pointer all the same
+  ea.nbr = nbr; ea.nbr_dist = nd; ea.w = w; ea.rowmax = mx; ea.dn = src;
+  IBL_RET(rerank_sparse<true>(W, ea, N, m, k1, k2, nl, s, [&](int q0, int, long long, long long T) -> int {
+    if (T == 0) return IBL_OK;
+    rr_dense_scatter_kernel<<<cdiv(T, 256), 256, 0, s>>>(W->pk2.as<unsigned long long>(), W->tsum.as<float>(), T, q0,
+                                                         n, qg, mx, c1, c2, out);
+    IBL_CUDA_OK(cudaGetLastError());
+    nl += 1;
+    return IBL_OK;
+  }));
   if (launches) *launches += nl;
   return IBL_OK;
 }

@@ -5,7 +5,7 @@ from __future__ import annotations
 
 import ctypes
 import threading
-from ctypes import byref, c_float, c_int, c_uint64, c_void_p
+from ctypes import byref, c_double, c_float, c_int, c_uint64, c_void_p
 from typing import Optional, Sequence
 
 import torch
@@ -445,6 +445,25 @@ class Engine:
                                        int(k_orig), int(k), _ptr(od), _ptr(oi), _stream(self.device)),
               "ibl_rerank_topk")
         return od, oi
+
+    def rerank_dense(self, qg: torch.Tensor, qq: torch.Tensor, gg: torch.Tensor, k1: int = 20, k2: int = 6,
+                     lambda_value: float = 0.3) -> torch.Tensor:
+        """k-reciprocal re-ranking of dense distance matrices, the reference's re_ranking (rerank.py:32-100):
+        qg [m,n], qq [m,m], gg [n,n] -> final [m,n] on this engine's device.  Neighbour lists of max(k1 + 1, k2)
+        <= 128 columns; nothing of size [m+n, m+n] is allocated."""
+        qg = _require_cuda(qg, "query-gallery distances")
+        qq = _require_cuda(qq, "query-query distances")
+        gg = _require_cuda(gg, "gallery-gallery distances")
+        m, n = qg.shape
+        if tuple(qq.shape) != (m, m) or tuple(gg.shape) != (n, n):
+            raise ValueError(f"re_ranking: shapes qg {tuple(qg.shape)}, qq {tuple(qq.shape)}, gg {tuple(gg.shape)} "
+                             "do not fit together")
+        if m + n < k1 + 1:
+            raise ValueError("re_ranking needs at least k1 + 1 images")
+        out = torch.empty(m, n, device=qg.device)
+        check(self.lib.ibl_rerank_dense(self.h, _ptr(qg), _ptr(qq), _ptr(gg), m, n, int(k1), int(k2),
+                                        c_double(lambda_value), _ptr(out), _stream(self.device)), "ibl_rerank_dense")
+        return out
 
     def knn_flagged(self) -> int:
         """Rows of the last knn_rowmax call that the guards sent to the exact scan (-1: no call yet)."""

@@ -3,8 +3,18 @@ ibl/utils/rerank.py:32-100 -- `re_ranking(q_g_dist, q_q_dist, g_g_dist, k1, k2, 
 query x gallery distances -- used by Evaluator.evaluate(rerank=True) (ibl/evaluators.py:194-199).
 
 The reference walks the N = m + n rows in Python (np.where / np.intersect1d / np.unique per row, an inverted
-index for the Jaccard term).  This version states the same algorithm as dense set algebra on whatever device
-the distances live on (the GPU in the evaluator):
+index for the Jaccard term).  Two implementations follow it:
+
+  * Host inputs (numpy arrays or CPU tensors, `device=None`), a CUDA device present and max(k1 + 1, k2) <= 128:
+    the inputs are copied to the current CUDA device and re-ranked there by Engine.rerank_dense (ibl_rerank_dense,
+    rerank.cu): dense neighbour lists, then the sparse stage of the evaluator's re-ranking, then the full [m,n]
+    output, in the reference's arithmetic and summation order.  Workspace O(N * k1): no [N,N] temporary.  This is
+    the call of the SFRS sampler refresh (examples/netvlad_img_sfrs.py:84).  The result comes back to the host.
+  * CUDA-tensor inputs, an explicit `device=`, no CUDA device, or wider neighbour lists: the dense torch
+    restatement below, on the inputs' (or the given) device.  It builds several [N,N] temporaries; the tests use
+    it as an independent oracle for the device paths.
+
+The torch restatement states the algorithm as dense set algebra:
 
   * neighbour lists      R   = the k1+1 nearest columns of each row of the row-max-normalised squared distances
   * k-reciprocal sets    Kr  [N,N] bool:  Kr[i,j]  <=>  j in R[i] and i in R[j]              (rerank.py:53-57)
@@ -16,8 +26,8 @@ the distances live on (the GPU in the evaluator):
   * Jaccard              1 - t/(2-t),  t[i,r] = sum_j min(V[i,j], V[r,j]), evaluated over the non-zero columns
                          of each query row only                                                (rerank.py:78-92)
 
-Out of the accelerated hot path (SURVEY 8f rank 3): plain torch ops, no custom kernel.  Pinned against the
-unmodified reference function on seeded inputs (tests/golden/rerank.npz)."""
+Both are pinned against the unmodified reference function on seeded inputs (tests/golden/rerank.npz,
+tests/golden/rerank_sfrs.npz)."""
 import numpy as np
 import torch
 
@@ -41,14 +51,33 @@ def _reciprocal_sets(rank_lists, width):
     return S
 
 
+def _on_host(a):
+    return isinstance(a, np.ndarray) or (isinstance(a, torch.Tensor) and a.device.type == "cpu")
+
+
 def re_ranking(q_g_dist, q_q_dist, g_g_dist, k1=20, k2=6, lambda_value=0.3, device=None):
     as_numpy = isinstance(q_g_dist, np.ndarray)
-    t = (lambda a: torch.as_tensor(a)) if device is None else (lambda a: torch.as_tensor(a).to(device))
-    qg, qq, gg = t(q_g_dist).float(), t(q_q_dist).float(), t(g_g_dist).float()
-    m, n = qg.shape
+    m, n = q_g_dist.shape
     N = m + n
     if N < k1 + 1:
         raise ValueError("re_ranking needs at least k1 + 1 images")
+    if (device is None and all(_on_host(a) for a in (q_g_dist, q_q_dist, g_g_dist)) and torch.cuda.is_available()
+            and m >= 1 and n >= 1 and max(k1 + 1, k2) <= min(128, N)):
+        # host arrays, as the SFRS sampler refresh passes them: the sparse device path (Engine.rerank_dense)
+        from ..engine import Engine
+        dev = torch.cuda.current_device()
+        qg, qq, gg = (torch.as_tensor(a).to(dev).float().contiguous() for a in (q_g_dist, q_q_dist, g_g_dist))
+        final = Engine.get(dev).rerank_dense(qg, qq, gg, k1, k2, lambda_value).cpu()
+        return final.numpy() if as_numpy else final
+    t = (lambda a: torch.as_tensor(a)) if device is None else (lambda a: torch.as_tensor(a).to(device))
+    final = _re_ranking_torch(t(q_g_dist).float(), t(q_q_dist).float(), t(g_g_dist).float(), k1, k2, lambda_value)
+    return final.cpu().numpy() if as_numpy else final
+
+
+def _re_ranking_torch(qg, qq, gg, k1, k2, lambda_value):
+    """The dense set-algebra restatement on qg's device -> final [m,n] there."""
+    m, n = qg.shape
+    N = m + n
     dist = torch.cat([torch.cat([qq, qg], dim=1), torch.cat([qg.t(), gg], dim=1)], dim=0)
     dist = dist.pow(2)
     dist = (dist / dist.max(dim=0, keepdim=True).values).t().contiguous()    # rerank.py:42-43
@@ -84,5 +113,4 @@ def re_ranking(q_g_dist, q_q_dist, g_g_dist, k1=20, k2=6, lambda_value=0.3, devi
         tmin = torch.minimum(cols, vals.unsqueeze(2)).sum(dim=1)   # [b,N]
         jac[i0:i0 + rows.shape[0]] = 1.0 - tmin / (2.0 - tmin)
     final = jac * (1 - lambda_value) + od * lambda_value
-    final = final[:, m:]
-    return final.cpu().numpy() if as_numpy else final
+    return final[:, m:]

@@ -10,8 +10,9 @@
 //             hi/lo planes delivers -- the layout the second NetVLAD contraction already uses (tc_netvlad.cu).
 //             conv_wgrad_tc_kernel: one CTA per (tap, 128 output channels, 128 input channels, pixel split);
 //             64-pixel K steps (boxes of 16 x 4 pixels; the X box is shifted by the tap, TMA zero-fills the
-//             padding), bf16x3, one 128 x 128 fp32 wgmma accumulator, partial sums per split reduced by
-//             wgrad_reduce_kernel into the OIHW gradient.
+//             padding), bf16x3, one 128 x 128 fp32 wgmma accumulator restarted every WG_CHAIN_BOXES boxes and
+//             added into the split's partial sum, partial sums per split reduced by wgrad_reduce_kernel into the
+//             OIHW gradient.
 //   db, ReLU mask, 2x2 max-pool backward: small CUDA-core kernels.
 #include <stdlib.h>
 
@@ -139,6 +140,11 @@ struct WgradArgs {
 constexpr int WG_BOX = 8192;                    // [64 px][64 ch] bf16
 constexpr int WG_STAGE = 8 * WG_BOX;            // dY hi c0,c1 | dY lo c0,c1 | X hi c0,c1 | X lo c0,c1 = 64 KiB
 constexpr int WG_STAGES = 3;
+// The wgmma fp32 accumulator loses a little toward zero on every accumulation: a sum of positive products over one
+// chain comes out smaller by ~3e-8 per MMA (measured on H100: 1e-3 after the 23,040 MMAs of a 1,920-box chain).  The
+// consumer therefore restarts its chain every WG_CHAIN_BOXES boxes (96 MMAs) and adds the finished chain into its own
+// [128 x 128] slice of the split's partial with ordinary fp32 adds, in a fixed order.
+constexpr int WG_CHAIN_BOXES = 8;
 
 __global__ void __launch_bounds__(160, 1)
 conv_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tm_ghi, const __grid_constant__ CUtensorMap tm_glo,
@@ -209,42 +215,46 @@ conv_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tm_ghi, const __grid_co
       Acc128<128> acc;
       int stage = 0; uint32_t phase = 0;
       int prev = -1;
-      for (long long b = b0; b < b1; ++b) {
-        mbar_wait(&full_bar[stage], phase);
-        const uint32_t sa = smem_a + stage * WG_STAGE;
-        wgmma_fence();
+      for (long long c0 = b0; c0 < b1; c0 += WG_CHAIN_BOXES) {
+        const long long c1 = (c0 + WG_CHAIN_BOXES < b1) ? c0 + WG_CHAIN_BOXES : b1;
+        for (long long b = c0; b < c1; ++b) {
+          mbar_wait(&full_bar[stage], phase);
+          const uint32_t sa = smem_a + stage * WG_STAGE;
+          wgmma_fence();
 #pragma unroll
-        for (int ks = 0; ks < 4; ++ks) {          // 16 pixel rows (2048 B) per MMA
-          const uint32_t off = ks * 2048;
-          // A = dY: output channels 0-63 / 64-127 of the tile are the two 64-channel boxes (one MN atom each)
-          const uint64_t gh0 = gmma_desc_mnmajor_sw128(sa + off, WG_BOX);
-          const uint64_t gh1 = gmma_desc_mnmajor_sw128(sa + WG_BOX + off, WG_BOX);
-          const uint64_t gl0 = gmma_desc_mnmajor_sw128(sa + 2 * WG_BOX + off, WG_BOX);
-          const uint64_t gl1 = gmma_desc_mnmajor_sw128(sa + 3 * WG_BOX + off, WG_BOX);
-          // B = X: 128 input channels = two MN atoms WG_BOX apart
-          const uint64_t xh = gmma_desc_mnmajor_sw128(sa + 4 * WG_BOX + off, WG_BOX);
-          const uint64_t xl = gmma_desc_mnmajor_sw128(sa + 6 * WG_BOX + off, WG_BOX);
-          acc.mma<false, 1, 1>(gl0, gl1, xh, (b == b0 && ks == 0) ? 0u : 1u);
-          acc.mma<false, 1, 1>(gh0, gh1, xl, 1u);
-          acc.mma<false, 1, 1>(gh0, gh1, xh, 1u);
+          for (int ks = 0; ks < 4; ++ks) {          // 16 pixel rows (2048 B) per MMA
+            const uint32_t off = ks * 2048;
+            // A = dY: output channels 0-63 / 64-127 of the tile are the two 64-channel boxes (one MN atom each)
+            const uint64_t gh0 = gmma_desc_mnmajor_sw128(sa + off, WG_BOX);
+            const uint64_t gh1 = gmma_desc_mnmajor_sw128(sa + WG_BOX + off, WG_BOX);
+            const uint64_t gl0 = gmma_desc_mnmajor_sw128(sa + 2 * WG_BOX + off, WG_BOX);
+            const uint64_t gl1 = gmma_desc_mnmajor_sw128(sa + 3 * WG_BOX + off, WG_BOX);
+            // B = X: 128 input channels = two MN atoms WG_BOX apart
+            const uint64_t xh = gmma_desc_mnmajor_sw128(sa + 4 * WG_BOX + off, WG_BOX);
+            const uint64_t xl = gmma_desc_mnmajor_sw128(sa + 6 * WG_BOX + off, WG_BOX);
+            acc.mma<false, 1, 1>(gl0, gl1, xh, (b == c0 && ks == 0) ? 0u : 1u);
+            acc.mma<false, 1, 1>(gh0, gh1, xl, 1u);
+            acc.mma<false, 1, 1>(gh0, gh1, xh, 1u);
+          }
+          wgmma_commit();
+          wgmma_wait<1>();
+          if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+          prev = stage;
+          if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
         }
-        wgmma_commit();
-        wgmma_wait<1>();
-        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
-        prev = stage;
-        if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
-      }
-      wgmma_wait<0>();
-      acc.fence_operands();
+        wgmma_wait<0>();
+        acc.fence_operands();
+        // the finished chain -> this thread's row of the slice: the first chain stores, later ones load-add-store
 #pragma unroll
-      for (int ch = 0; ch < 4; ++ch) {
-        uint32_t r[32];
-        acc.rows32(ch, stg, r);
-        if (co < a.cout) {
+        for (int ch = 0; ch < 4; ++ch) {
+          uint32_t r[32];
+          acc.rows32(ch, stg, r);
+          if (co < a.cout) {
 #pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const int ci = nt * 128 + ch * 32 + j;
-            if (ci < a.cin) po[ch * 32 + j] = __uint_as_float(r[j]);
+            for (int j = 0; j < 32; ++j) {
+              const int ci = nt * 128 + ch * 32 + j;
+              if (ci < a.cin) po[ch * 32 + j] = (c0 == b0 ? 0.f : po[ch * 32 + j]) + __uint_as_float(r[j]);
+            }
           }
         }
       }

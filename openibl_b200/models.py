@@ -8,7 +8,7 @@ the engine re-lays them out when their version counters change.
 
 No CPU path: calling a model on CPU tensors raises.  Training (config 5, SURVEY 8 f1): NetVLAD and the trainable
 suffix of the VGG trunk (conv5_x when `train_layers='conv5'`, vgg.py:50-53) are `torch.autograd.Function`s whose
-forward AND backward run in libiblb200 (tcgen05 dgrad / wgrad, NetVLAD backward kernels); the region algebra of
+forward AND backward run in libiblb200 (Hopper wgmma dgrad / wgrad, NetVLAD backward kernels); the region algebra of
 EmbedRegionNet's train branch (sums of quarter VLADs, two normalisations, a 9x9 matmul per pair) stays in torch.
 """
 from __future__ import annotations

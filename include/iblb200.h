@@ -285,9 +285,14 @@ int ibl_debug_gemm_tn(ibl_engine* e, const float* A, const float* B, float* C, v
  * taps out of one halo tile. */
 int ibl_debug_umma_strided(ibl_engine* e, const void* A, int rows, const void* B, int s0, int group_rows,
                            int base_mode, float* D, void* stream);
+/* The same probe with the second m64 half of the view starting `half_rows` rows after the first (the 8x16 halo
+ * patch: view row m is row s0 + ((m%64)/8)*group_rows + (m/64)*half_rows + (m%8)), base_offset 0. */
+int ibl_debug_umma_halo_view(ibl_engine* e, const void* A, int rows, const void* B, int s0, int group_rows,
+                             int half_rows, float* D, void* stream);
 /* Average device time (ms) of one backbone layer over `reps` launches, weights from the engine
  * (tools/bench_layers.py).  layer 0 = the tensor-core conv1_1 (x NCHW [N,3,H,W]); 1..12 = conv1_2..conv5_3
- * (x NHWC [N,H,W,Cin] fp32), where bn_override forces the N tile (64/128) when it divides Cout, 0 = default.
+ * (x NHWC [N,H,W,Cin] fp32), where bn_override forces the N tile (64/128) when it divides Cout, 0 = default;
+ * layer -1 = the fused conv1_1 + conv1_2 + 2x2 pool kernel of the forward (x NCHW [N,3,H,W]).
  * Synchronises. */
 int ibl_debug_time_layer(ibl_engine* e, int layer, const float* x, int N, int H, int W, int bn_override,
                          int reps, float* ms_out);

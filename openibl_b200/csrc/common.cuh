@@ -126,8 +126,8 @@ int launch_conv1_1_wgrad(const float* x_nchw, const __nv_bfloat16* g_hi, const _
 int launch_conv1_1_tc(const float* x_nchw, const float* w_oihw, const float* bias, int N, int H, int W,
                       __nv_bfloat16* y_hi, __nv_bfloat16* y_lo, cudaStream_t s);
 // tc_probe.cu
-int debug_gmma_strided(const void* A, int rows, const void* B, int s0, int group_rows, int base_mode, float* D,
-                       cudaStream_t s);
+int debug_gmma_strided(const void* A, int rows, const void* B, int s0, int group_rows, int half_rows, int base_mode,
+                       float* D, cudaStream_t s);
 // tc_netvlad.cu
 int debug_gemm_tn(const float* A, const float* B, float* C, cudaStream_t s);
 int netvlad_tc_units(int B, int S);

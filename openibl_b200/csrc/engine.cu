@@ -1291,7 +1291,15 @@ int ibl_debug_umma_strided(ibl_engine* e, const void* A, int rows, const void* B
   IBL_REQUIRE(e && A && B && D, "null argument");
   DeviceGuard g(e->device);
   e->launches += 1;
-  return debug_gmma_strided(A, rows, B, s0, group_rows, base_mode, D, S(stream));
+  return debug_gmma_strided(A, rows, B, s0, group_rows, 8 * group_rows, base_mode, D, S(stream));
+}
+
+int ibl_debug_umma_halo_view(ibl_engine* e, const void* A, int rows, const void* B, int s0, int group_rows,
+                             int half_rows, float* D, void* stream) {
+  IBL_REQUIRE(e && A && B && D, "null argument");
+  DeviceGuard g(e->device);
+  e->launches += 1;
+  return debug_gmma_strided(A, rows, B, s0, group_rows, half_rows, 0, D, S(stream));
 }
 
 // Timing hooks (tools/bench_layers.py): average device time of one backbone layer over `reps`
@@ -1299,10 +1307,11 @@ int ibl_debug_umma_strided(ibl_engine* e, const void* A, int rows, const void* B
 // (x is NCHW [N,3,H,W]); layers 1..12 take x NHWC [N,H,W,Cin] fp32 (converted to planes once).
 int ibl_debug_time_layer(ibl_engine* e, int layer, const float* x, int N, int H, int W, int bn_override,
                          int reps, float* ms_out) {
-  IBL_REQUIRE(e && x && ms_out && layer >= 0 && layer <= 12 && reps >= 1, "bad argument");
+  IBL_REQUIRE(e && x && ms_out && layer >= -1 && layer <= 12 && reps >= 1, "bad argument");
   if (!e->vgg_ready) { set_last_error("ibl_engine_set_vgg16 was not called"); return IBL_ERR_NOT_READY; }
   DeviceGuard g(e->device);
-  const ConvLayer& L = kVgg16[layer];
+  const bool fused1 = layer < 0;                           // conv1_1 + conv1_2 + pool: conv1_2's shape, input NCHW
+  const ConvLayer& L = kVgg16[fused1 ? 1 : layer];
   const size_t in_e = (size_t)N * H * W * L.cin;
   const int oh = L.pool ? H / 2 : H, ow = L.pool ? W / 2 : W;
   const size_t out_e = (size_t)N * oh * ow * L.cout;
@@ -1318,7 +1327,9 @@ int ibl_debug_time_layer(ibl_engine* e, int layer, const float* x, int N, int H,
   tc_set_bn_override(bn_override);
   for (int r = -1; r < reps && rc == IBL_OK; ++r) {       // r = -1 is a warm-up launch
     if (r == 0) cudaEventRecord(e0, nullptr);
-    if (layer == 0)
+    if (fused1)
+      rc = launch_conv1_fused_tc(x, e->w0_oihw, e->conv[0].bias, e->conv[1], N, H, W, oh_, oh_ + out_e, nullptr);
+    else if (layer == 0)
       rc = launch_conv1_1_tc(x, e->w0_oihw, e->conv[0].bias, N, H, W, oh_, oh_ + out_e, nullptr);
     else
       rc = launch_conv3x3_tc(ih, ih + in_e, e->conv[layer], N, H, W, L.cin, L.cout, L.relu, L.pool,

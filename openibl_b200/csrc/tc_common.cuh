@@ -226,8 +226,16 @@ __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_grou
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-// named barrier of the consumer warpgroup (threads 0..127 of every tensor-core kernel)
-__device__ __forceinline__ void wg_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
+// named barrier of one consumer warpgroup: id 1 for threads 0..127 of the single-consumer kernels; kernels with two
+// consumer warpgroups give each its own id so that one can run its epilogue while the other issues MMAs
+__device__ __forceinline__ void wg_sync(int id = 1) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+
+// Hand registers between the warpgroups of a warp-specialised CTA (every warp of the warpgroup executes it): the
+// producer gives up what its TMA loop does not need, the MMA warpgroups take it for their accumulators.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
 // A 128 x N fp32 accumulator held by one warpgroup as two m64 fragments: h[0] = rows 0-63, h[1] = rows 64-127.
 // In fragment h, thread t (warp w = t / 32, lane l) holds for every 8-column block i the elements
@@ -251,16 +259,16 @@ struct Acc128 {
   }
   // Row-per-thread view of 32 accumulator columns [32 ch, 32 ch + 32): thread t of the warpgroup receives row t.
   // The fragments go through `stg` (128 rows x ACC_STG_PITCH floats of shared memory); every thread of the warpgroup
-  // must call this with the same ch.
-  __device__ __forceinline__ void rows32(int ch, float* stg, uint32_t (&raw)[32]) const;
+  // must call this with the same ch and the warpgroup's named barrier `bar`.
+  __device__ __forceinline__ void rows32(int ch, float* stg, uint32_t (&raw)[32], int bar = 1) const;
 };
 constexpr int ACC_STG_PITCH = 36;                          // 144-byte rows: conflict-free 16-byte row reads
 constexpr int ACC_STG_BYTES = 128 * ACC_STG_PITCH * 4;
 
 template <int N>
-__device__ __forceinline__ void Acc128<N>::rows32(int ch, float* stg, uint32_t (&raw)[32]) const {
+__device__ __forceinline__ void Acc128<N>::rows32(int ch, float* stg, uint32_t (&raw)[32], int bar) const {
   const int t = threadIdx.x & 127, w = t >> 5, l = t & 31;
-  wg_sync();                                               // the previous chunk's reads are done
+  wg_sync(bar);                                            // the previous chunk's reads are done
 #pragma unroll
   for (int j = 0; j < 2; ++j)
 #pragma unroll
@@ -270,7 +278,7 @@ __device__ __forceinline__ void Acc128<N>::rows32(int ch, float* stg, uint32_t (
       *reinterpret_cast<float2*>(stg + r * ACC_STG_PITCH + c) = make_float2(f[0], f[1]);
       *reinterpret_cast<float2*>(stg + (r + 8) * ACC_STG_PITCH + c) = make_float2(f[2], f[3]);
     }
-  wg_sync();
+  wg_sync(bar);
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
     const float4 v = *reinterpret_cast<const float4*>(stg + t * ACC_STG_PITCH + 4 * i);

@@ -13,9 +13,13 @@
 // the activation box for tap (kh,kw) is the output patch shifted by (kh-1,kw-1) and the
 // hardware zero-fills the out-of-image part, which is exactly the conv's zero padding.
 //
-// Warp roles (160 threads, persistent over tiles):
+// Warp roles, persistent over tiles.  Box staging (BN = 64, 160 threads):
 //   warps 0-3  consumer warpgroup: wgmma main loop (two m64 halves of the 128-pixel tile), then the epilogue
 //   warp 4     TMA producer
+// Halo staging (BN = 128, 384 threads, "ping-pong"):
+//   warpgroup 0     producer (warp 0 issues the TMA loads), its registers handed to the consumers (setmaxnreg)
+//   warpgroups 1-2  consumers: consumer j takes the CTA's tiles j, j+2, j+4, ... so one runs its epilogue while the
+//                   other issues the next tile's MMAs
 // Epilogue: accumulator -> row-per-thread views (Acc128::rows32), + bias, ReLU, optional fused 2x2 max-pool
 // (warp shuffles), split into hi/lo planes (or fp32 for conv5_3), 16-byte stores.
 #include "common.cuh"
@@ -93,11 +97,12 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
   return *reinterpret_cast<uint32_t*>(&t);
 }
 
-// One accumulator tile (128 pixel rows x BN output channels, thread = pixel row) to global memory:
-// bias + ReLU + fused 2x2 max-pool + bf16 hi/lo split (or fp32), optional per-pixel sum of squares.
+// One accumulator tile (128 pixel rows x BN output channels, thread = pixel row (r, c) of the patch) to global memory:
+// bias + ReLU + fused 2x2 max-pool + bf16 hi/lo split (or fp32), optional per-pixel sum of squares.  `dr_lanes` is the
+// lane distance between a pixel and the one below it; `bar` is the warpgroup's named barrier.
 template <int BN>
 __device__ __forceinline__ void conv_epilogue_tile(const ConvTcArgs& a, const Acc128<BN>& acc, float* stg, int img, int h0,
-                                                   int w0, int n0, int nt, int r, int c, int TW) {
+                                                   int w0, int n0, int nt, int r, int c, int dr_lanes, int bar = 1) {
   const int h = h0 + r, w = w0 + c;
   bool valid;
   long long pix;
@@ -114,11 +119,11 @@ __device__ __forceinline__ void conv_epilogue_tile(const ConvTcArgs& a, const Ac
 #pragma unroll
   for (int ch = 0; ch < BN / 32; ++ch) {     // unrolled: the accumulator is indexed with constants only
     uint32_t raw[32];
-    acc.rows32(ch, stg, raw);
+    acc.rows32(ch, stg, raw, bar);
     if (a.pool) {
       // 2x2 max-pool BEFORE bias / ReLU / split (. + b and max(., 0) are monotone, so the results are the same bits)
       // as a two-step exchange: against the w-neighbour (lane ^ 1) every lane keeps one half of the 32
-      // channels and sends the other, against the h-neighbour (lane ^ TW) one half of those 16 -- 24 shuffles instead
+      // channels and sends the other, against the h-neighbour (lane ^ dr_lanes) one half of those 16 -- 24 shuffles instead
       // of 64, and each of the window's four lanes finishes 8 channels (bias, ReLU, hi/lo, ONE 16-byte store per plane)
       // instead of one lane doing all 32 while three idle.
       const bool s1 = (c & 1) != 0, s2 = (r & 1) != 0;
@@ -132,7 +137,7 @@ __device__ __forceinline__ void conv_epilogue_tile(const ConvTcArgs& a, const Ac
       float w8[8];
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
-        const float got = __shfl_xor_sync(0xffffffffu, s2 ? u[j] : u[j + 8], TW);
+        const float got = __shfl_xor_sync(0xffffffffu, s2 ? u[j] : u[j + 8], dr_lanes);
         w8[j] = fmaxf(s2 ? u[j + 8] : u[j], got);
       }
       if (valid) {
@@ -224,20 +229,27 @@ constexpr int TC_A_BYTES = TC_BM * TC_BK * 2;   // 16 KiB per plane
 // descriptor whose start is only 128-byte aligned and whose group stride is not a multiple of 1024 B reads the
 // TMA-written tile correctly (pinned on hardware by tests/test_gpu_parity.py through tc_probe.cu).
 // L2->SM traffic of the A operand drops from 9 x 32 KiB to 45 KiB per chunk; the weights get their own ring.
-constexpr int TC_HALO_W = 10, TC_HALO_H = 18;
+// An 8x16 patch (chosen where it wastes fewer rows, e.g. 120x160 maps) has an 18 x 10 halo: the same 180 rows, taps
+// (kh*18 + kw) rows in, 8-row groups 18 rows (2304 B) apart, and the second m64 half (columns 8-15 of every patch row)
+// 8 rows in.
+constexpr int TC_HALO_W = 10, TC_HALO_H = 18;   // the 16x8 patch's halo (also the fused conv1 kernel's)
+constexpr int TC_HALO_ROWS = TC_HALO_W * TC_HALO_H;
 constexpr int TC_HALO_PLANE = 23 * 1024;        // 180 rows x 128 B = 23040 B, padded to the swizzle period
 constexpr int TC_HALO_STAGE = 2 * TC_HALO_PLANE;
 
 template <int BN, int STAGES, bool HALO = false, int NA = 0>
 struct ConvTcSmem {
+  static constexpr int THREADS = HALO ? 384 : 160;
+  static constexpr int CONSUMERS = HALO ? 2 : 1;   // consumer warpgroups, each with its own epilogue staging buffer
   static constexpr int B_BYTES = BN * TC_BK * 2;
   static constexpr int STAGE_BYTES = HALO ? 2 * B_BYTES : 2 * TC_A_BYTES + 2 * B_BYTES;
   static constexpr int A_RING = HALO ? NA * TC_HALO_STAGE : 0;
-  static constexpr int BYTES = A_RING + STAGES * STAGE_BYTES + ACC_STG_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+  static constexpr int STG = CONSUMERS * ACC_STG_BYTES;
+  static constexpr int BYTES = A_RING + STAGES * STAGE_BYTES + STG + 1024 /*align slack*/ + 256 /*barriers*/;
 };
 
 template <int BN, int STAGES, bool HALO, int NA>
-__global__ void __launch_bounds__(160, 1)
+__global__ void __launch_bounds__(ConvTcSmem<BN, STAGES, HALO, NA>::THREADS, 1)
 conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tm_xhi, const __grid_constant__ CUtensorMap tm_xlo,
                   const __grid_constant__ CUtensorMap tm_whi, const __grid_constant__ CUtensorMap tm_wlo,
                   const ConvTcArgs a) {
@@ -250,27 +262,33 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tm_xhi, const __grid_const
   constexpr int A_RING = L::A_RING;           // HALO: the halo ring sits in front of the weight ring
   uint8_t* ring = smem + A_RING;
   float* stg = reinterpret_cast<float*>(ring + STAGES * STAGE_BYTES);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(ring + STAGES * STAGE_BYTES + ACC_STG_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(ring + STAGES * STAGE_BYTES + L::STG);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + STAGES;
-  uint64_t* afull_bar = bars + 2 * STAGES;    // HALO only: [NA] + [NA]
+  uint64_t* afull_bar = bars + 2 * STAGES;    // HALO only: [NA] + [NA] + the two consumers' order barriers
   uint64_t* aempty_bar = afull_bar + NA;
+  uint64_t* order_bar = aempty_bar + NA;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int worker = (int)blockIdx.x;
   const int n_workers = (int)gridDim.x;
-  if (warp == 4 && lane == 0) {
+  const int producer_warp = HALO ? 0 : 4;
+  if (warp == producer_warp && lane == 0) {
     tma_prefetch_desc(&tm_xhi);
     tma_prefetch_desc(&tm_xlo);
     tma_prefetch_desc(&tm_whi);
     tma_prefetch_desc(&tm_wlo);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 4);   // one arrival per consumer warp
+      mbar_init(&empty_bar[i], 4);   // one arrival per warp of the consuming warpgroup
     }
     for (int i = 0; i < NA; ++i) {
       mbar_init(&afull_bar[i], 1);
       mbar_init(&aempty_bar[i], 4);
+    }
+    if (HALO) {
+      mbar_init(&order_bar[0], 4);
+      mbar_init(&order_bar[1], 4);
     }
     fence_barrier_init();
     fence_proxy_async();
@@ -290,11 +308,12 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tm_xhi, const __grid_const
     w0 = (rem % a.tiles_w) * TW;
   };
 
-  if (warp == 4) {
+  if (HALO && warp < 4) setmaxnreg_dec<40>();
+  if (warp == producer_warp) {
     // ================= TMA producer: convergent warp, one elected lane issues, coordinates warp-uniform =================
     const uint32_t smem_a = warp_uniform(smem_u32(smem));
     const uint32_t ring_a = smem_a + A_RING;
-    const uint32_t bars_a = ring_a + STAGES * STAGE_BYTES + ACC_STG_BYTES;
+    const uint32_t bars_a = ring_a + STAGES * STAGE_BYTES + L::STG;
     const uint32_t full_a = bars_a, empty_a = bars_a + 8 * STAGES;
     const uint32_t afull_a = bars_a + 16 * STAGES, aempty_a = afull_a + 8 * NA;
     // the two weight planes of one tap (into `st`, planes B_BYTES apart)
@@ -336,7 +355,7 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tm_xhi, const __grid_const
           w0 = (int)warp_uniform((uint32_t)w0);
           const int c0 = (int)warp_uniform((uint32_t)(kcA * TC_BK));
           const uint32_t sa = smem_a + as_u * TC_HALO_STAGE;
-          constexpr uint32_t kHaloBytes = 2u * TC_HALO_W * TC_HALO_H * 128u;
+          constexpr uint32_t kHaloBytes = 2u * TC_HALO_ROWS * 128u;
           if (elect_one()) {
             mbar_arrive_expect_tx_a(afull_a + 8 * as_u, kHaloBytes);
             tma_load_4d_a(sa, &tm_xhi, afull_a + 8 * as_u, c0, w0 - 1, h0 - 1, img);
@@ -389,62 +408,88 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tm_xhi, const __grid_const
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
     }
-  } else {
-    // ================= consumer warpgroup: main loop + epilogue =================
-    const int m = threadIdx.x;              // accumulator row = pixel index inside the patch
-    const int r = m >> a.tw_log2, c = m & (TW - 1);
+  } else if (!HALO || warp >= 4) {
     const uint32_t smem_a = smem_u32(smem);
     const uint32_t ring_a = smem_a + A_RING;
-    int stage = 0, astage = 0;
-    uint32_t phase = 0, aphase = 0;
-    (void)ring_a; (void)astage; (void)aphase;
     auto release_w = [&](int st) {          // this warp is done reading weight slot st
       if (lane == 0) mbar_arrive(&empty_bar[st]);
     };
+    if constexpr (HALO) {
+    // ================= two consumer warpgroups (ping-pong): main loop + epilogue =================
+    setmaxnreg_inc<232>();
+    const int cw = warp / 4 - 1;            // consumer 0 / 1
+    const int bar = 1 + cw;                 // its named barrier (epilogue staging)
+    float* my_stg = stg + cw * (ACC_STG_BYTES / 4);
+    // accumulator row m -> patch pixel (r, c).  16x8: 8-row group g = pixel row g.  8x16: rows 0-63 are columns 0-7
+    // and rows 64-127 columns 8-15 of patch rows 0-7.  Either way the pixel below is 8 rows (lanes) further on.
+    const int m = threadIdx.x & 127;
+    const int r = TW == 16 ? (m >> 3) & 7 : m >> 3;
+    const int c = TW == 16 ? ((m >> 6) << 3) | (m & 7) : m & 7;
+    // K-major SW128 view of the halo tile: 8-pixel row groups one halo row (TW + 2 pixels) apart
+    const uint32_t halo_w = (uint32_t)TW + 2;
+    const uint64_t halo_desc = ((uint64_t)1 << 16) | ((uint64_t)((halo_w * 128) >> 4) << 32) | ((uint64_t)1 << 62);
+    const uint64_t a_half = (TW == 16 ? 8u : 8u * halo_w) * 128u / 16u;
+    // Consumer cw takes the CTA's tiles cw, cw + 2, ...  The producer fills both rings in tile order, so the slots
+    // (and phases) of CTA-local tile i start at running index i * kchunks (halo) and i * kiters (weights).  The order
+    // barrier lets a consumer wait on its first slots only after the other consumer has waited on all the slots of
+    // the tile before: a slot's full barrier is then at most one phase behind the awaited one, so its parity is exact.
+    for (int i = cw; worker + i * n_workers < a.total_tiles; i += 2) {
+      int img, h0, w0, nt;
+      coords(worker + i * n_workers, img, h0, w0, nt);
+      int astage = (i * kchunks) % NA, stage = (i * kiters) % STAGES;
+      uint32_t aphase = (uint32_t)((i * kchunks) / NA) & 1u, phase = (uint32_t)((i * kiters) / STAGES) & 1u;
+      if (i > 0) mbar_wait(&order_bar[cw], (uint32_t)((i - 1) >> 1) & 1u);
+      Acc128<BN> acc;
+      int prev = -1, prev_a = -1;
+      for (int kc = 0; kc < kchunks; ++kc) {
+        mbar_wait(&afull_bar[astage], aphase);
+        const uint32_t ha = smem_a + astage * TC_HALO_STAGE;
+        for (int tap = 0; tap < 9; ++tap) {
+          mbar_wait(&full_bar[stage], phase);
+          const uint32_t toff = ((uint32_t)(tap / 3) * halo_w + (uint32_t)(tap % 3)) * 128u;
+          const uint64_t a_hi = halo_desc | (uint64_t)(((ha + toff) >> 4) & 0x3fffu);
+          const uint64_t a_lo = halo_desc | (uint64_t)(((ha + TC_HALO_PLANE + toff) >> 4) & 0x3fffu);
+          const uint32_t sb = ring_a + stage * STAGE_BYTES;
+          const uint64_t b_hi = gmma_desc_kmajor_sw128(sb), b_lo = gmma_desc_kmajor_sw128(sb + B_BYTES);
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < TC_BK / 16; ++k) {
+            const uint64_t ko = (uint64_t)(k * 2);
+            acc.mma(a_lo + ko, a_lo + a_half + ko, b_hi + ko, (kc > 0 || tap > 0 || k > 0) ? 1u : 0u);
+            acc.mma(a_hi + ko, a_hi + a_half + ko, b_lo + ko, 1u);
+            acc.mma(a_hi + ko, a_hi + a_half + ko, b_hi + ko, 1u);
+          }
+          wgmma_commit();
+          if (kc == kchunks - 1 && tap == 8 && lane == 0) mbar_arrive(&order_bar[cw ^ 1]);
+          wgmma_wait<1>();                    // the previous tap's MMAs have retired: release its weight slot, and
+          if (prev >= 0) release_w(prev);     // after the first tap of a chunk the previous chunk's halo slot
+          if (prev_a >= 0) {
+            if (lane == 0) mbar_arrive(&aempty_bar[prev_a]);
+            prev_a = -1;
+          }
+          prev = stage;
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+        prev_a = astage;
+        if (++astage == NA) { astage = 0; aphase ^= 1; }
+      }
+      wgmma_wait<0>();
+      acc.fence_operands();
+      release_w(prev);
+      if (lane == 0) mbar_arrive(&aempty_bar[prev_a]);
+      conv_epilogue_tile<BN>(a, acc, my_stg, img, h0, w0, nt * BN, nt, r, c, 8, bar);
+    }
+    } else {
+    // ================= consumer warpgroup: main loop + epilogue =================
+    const int m = threadIdx.x;              // accumulator row = pixel index inside the patch
+    const int r = m >> a.tw_log2, c = m & (TW - 1);
+    int stage = 0;
+    uint32_t phase = 0;
     for (int tile = worker; tile < a.total_tiles; tile += n_workers) {
       int img, h0, w0, nt;
       coords(tile, img, h0, w0, nt);
       Acc128<BN> acc;
       int prev = -1;
-      if constexpr (HALO) {
-        // K-major SW128 view of the halo tile: 8-pixel row groups 10 rows apart; pixel rows 64-127 = groups 8-15
-        constexpr uint64_t kHaloDesc = ((uint64_t)1 << 16) | ((uint64_t)((TC_HALO_W * 128) >> 4) << 32) | ((uint64_t)1 << 62);
-        constexpr uint64_t kHalf = 8 * TC_HALO_W * 128 / 16;
-        for (int kc = 0; kc < kchunks; ++kc) {
-          mbar_wait(&afull_bar[astage], aphase);
-          const uint32_t ha = smem_a + astage * TC_HALO_STAGE;
-          for (int tap = 0; tap < 9; ++tap) {
-            mbar_wait(&full_bar[stage], phase);
-            const uint32_t toff = (uint32_t)((tap / 3) * TC_HALO_W + tap % 3) * 128u;
-            const uint64_t a_hi = kHaloDesc | (uint64_t)(((ha + toff) >> 4) & 0x3fffu);
-            const uint64_t a_lo = kHaloDesc | (uint64_t)(((ha + TC_HALO_PLANE + toff) >> 4) & 0x3fffu);
-            const uint32_t sb = ring_a + stage * STAGE_BYTES;
-            const uint64_t b_hi = gmma_desc_kmajor_sw128(sb), b_lo = gmma_desc_kmajor_sw128(sb + B_BYTES);
-            wgmma_fence();
-#pragma unroll
-            for (int k = 0; k < TC_BK / 16; ++k) {
-              const uint64_t ko = (uint64_t)(k * 2);
-              acc.mma(a_lo + ko, a_lo + kHalf + ko, b_hi + ko, (kc > 0 || tap > 0 || k > 0) ? 1u : 0u);
-              acc.mma(a_hi + ko, a_hi + kHalf + ko, b_lo + ko, 1u);
-              acc.mma(a_hi + ko, a_hi + kHalf + ko, b_hi + ko, 1u);
-            }
-            wgmma_commit();
-            if (tap < 8) {
-              wgmma_wait<1>();
-              if (prev >= 0) release_w(prev);
-              prev = stage;
-            } else {                              // the halo slot is free once all nine taps have retired
-              wgmma_wait<0>();
-              if (prev >= 0) release_w(prev);
-              release_w(stage);
-              if (lane == 0) mbar_arrive(&aempty_bar[astage]);
-              prev = -1;
-            }
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
-          }
-          if (++astage == NA) { astage = 0; aphase ^= 1; }
-        }
-      } else
       for (int kit = 0; kit < kiters; ++kit) {
         mbar_wait(&full_bar[stage], phase);
         const uint32_t sa = ring_a + stage * STAGE_BYTES;
@@ -472,6 +517,7 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tm_xhi, const __grid_const
       if (prev >= 0) release_w(prev);
       conv_epilogue_tile<BN>(a, acc, stg, img, h0, w0, nt * BN, nt, r, c, TW);
     }
+    }
   }
   __syncthreads();
 }
@@ -489,7 +535,7 @@ static int launch_tc_variant(const CUtensorMap& xhi, const CUtensorMap& xlo, con
   }
   const int sms = device_sm_count();
   const int grid = a.total_tiles < sms ? a.total_tiles : sms;
-  conv3x3_tc_kernel<BN, STAGES, HALO, NA><<<grid, 160, smem, s>>>(xhi, xlo, whi, wlo, a);
+  conv3x3_tc_kernel<BN, STAGES, HALO, NA><<<grid, ConvTcSmem<BN, STAGES, HALO, NA>::THREADS, smem, s>>>(xhi, xlo, whi, wlo, a);
   IBL_CUDA_OK(cudaGetLastError());
   return IBL_OK;
 }
@@ -521,14 +567,9 @@ int launch_conv3x3_tc(const __nv_bfloat16* x_hi, const __nv_bfloat16* x_lo, cons
   int bn = cout % 128 == 0 ? 128 : 64;
   if (g_tc_bn_override && cout % g_tc_bn_override == 0 && (g_tc_bn_override == 64 || g_tc_bn_override == 128))
     bn = g_tc_bn_override;
-  // Halo staging (16x8 patches) on the 128-wide tiles.  The choice depends on Cout only, never on the batch (the two
-  // kernels walk K in different orders).
+  // Halo staging on the 128-wide tiles.  The choice depends on Cout only, never on the batch (the two kernels walk K in
+  // different orders); the patch shape only moves pixels between accumulator rows, not the order of any pixel's sums.
   const bool halo = bn == 128;
-  if (halo) {
-    a.tw_log2 = 3;
-    a.tiles_w = cdiv(W, 8);
-    a.tiles_h = cdiv(H, 16);
-  }
   a.n_tiles = cout / bn;
   a.total_tiles = (int)((long long)N * a.tiles_h * a.tiles_w * a.n_tiles);
   a.relu = relu; a.pool = pool;
@@ -541,7 +582,7 @@ int launch_conv3x3_tc(const __nv_bfloat16* x_hi, const __nv_bfloat16* x_lo, cons
   {
     uint64_t dims[4] = {(uint64_t)cin, (uint64_t)W, (uint64_t)H, (uint64_t)N};
     uint64_t str[3] = {(uint64_t)cin * 2, (uint64_t)W * cin * 2, (uint64_t)H * W * cin * 2};
-    uint32_t box[4] = {64, (uint32_t)(halo ? TC_HALO_W : TW), (uint32_t)(halo ? TC_HALO_H : TH), 1};
+    uint32_t box[4] = {64, (uint32_t)(halo ? TW + 2 : TW), (uint32_t)(halo ? TH + 2 : TH), 1};
     IBL_RET(make_tmap(&m_xhi, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, x_hi, dims, str, box));
     IBL_RET(make_tmap(&m_xlo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, x_lo, dims, str, box));
   }

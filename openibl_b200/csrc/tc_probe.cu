@@ -6,9 +6,10 @@
 //
 //   A_halo : [rows][64] bf16 dense, loaded by TMA with the 128B swizzle (row r at byte r*128, 16-byte chunk
 //            j stored at chunk position j ^ (r & 7))
-//   view   : row m of the 128-row operand = halo row  s0 + (m / 8) * group_rows + (m % 8)
+//   view   : row m of the 128-row operand = halo row  s0 + ((m % 64) / 8) * group_rows + (m / 64) * half_rows + (m % 8)
+//            (half_rows = 8 * group_rows for a 16x8 patch, 8 for an 8x16 patch)
 //   D[m,n] = sum_k view[m,k] * B[n,k]
-// The caller compares D with the expected product for several (s0, group_rows, base_offset mode).
+// The caller compares D with the expected product for several (s0, group_rows, half_rows, base_offset mode).
 #include "common.cuh"
 #include "tc_common.cuh"
 
@@ -30,7 +31,7 @@ __device__ __forceinline__ uint64_t probe_desc(uint32_t a_addr, uint32_t sbo, in
 
 __global__ void __launch_bounds__(128, 1)
 gmma_strided_probe_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
-                          int rows, int s0, int group_rows, int base_mode, float* __restrict__ D) {
+                          int rows, int s0, int group_rows, int half_rows, int base_mode, float* __restrict__ D) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* a_sm = smem;                       // rows * 128 B (<= 32 KiB)
@@ -51,7 +52,7 @@ gmma_strided_probe_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid
   mbar_wait(&bars[0], 0);
   const uint32_t sbo = (uint32_t)group_rows * 128u;
   const uint32_t a0 = smem_u32(a_sm) + (uint32_t)s0 * 128u;
-  const uint32_t a1 = a0 + 8u * sbo;          // rows 64-127 of the view: groups 8-15
+  const uint32_t a1 = a0 + (uint32_t)half_rows * 128u;   // rows 64-127 of the view
   const uint64_t da0 = probe_desc(a0, sbo, base_mode), da1 = probe_desc(a1, sbo, base_mode);
   const uint64_t db = gmma_desc_kmajor_sw128(smem_u32(b_sm));
   Acc128<64> acc;
@@ -73,9 +74,10 @@ gmma_strided_probe_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid
 }
 
 // A: [rows][64] bf16 bits, B: [64][64] bf16 bits (device), D: [128][64] fp32
-int debug_gmma_strided(const void* A, int rows, const void* B, int s0, int group_rows, int base_mode, float* D,
-                       cudaStream_t s) {
-  IBL_REQUIRE(rows >= 8 && rows <= 256 && s0 >= 0 && group_rows >= 8 && s0 + 15 * group_rows + 8 <= rows,
+int debug_gmma_strided(const void* A, int rows, const void* B, int s0, int group_rows, int half_rows, int base_mode,
+                       float* D, cudaStream_t s) {
+  IBL_REQUIRE(rows >= 8 && rows <= 256 && s0 >= 0 && group_rows >= 8 && half_rows >= 0 &&
+                  s0 + half_rows + 7 * group_rows + 8 <= rows,
               "probe view does not fit the halo tile");
   CUtensorMap ma, mb;
   {
@@ -96,7 +98,7 @@ int debug_gmma_strided(const void* A, int rows, const void* B, int s0, int group
     IBL_CUDA_OK(cudaFuncSetAttribute(gmma_strided_probe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     attr_done.mark();
   }
-  gmma_strided_probe_kernel<<<1, 128, smem, s>>>(ma, mb, rows, s0, group_rows, base_mode, D);
+  gmma_strided_probe_kernel<<<1, 128, smem, s>>>(ma, mb, rows, s0, group_rows, half_rows, base_mode, D);
   IBL_CUDA_OK(cudaGetLastError());
   return IBL_OK;
 }

@@ -158,6 +158,8 @@ int launch_dist_guard_bf16x3(const float* q, const float* q_sq, const float2* q_
                              const float* db_sq, const float2* db_err, int n_valid, int d, const float* screened, int kc,
                              int k, long long idx_base, void* ws, float* out_dist, long long* out_idx,
                              uint64_t* launches, cudaStream_t s);
+// out3 (zeroed by the caller) = max over the n rows of {|lo|, |x - hi - lo|, |x|^2} (launch_planes_sqnorm's err, sq)
+int launch_bf16x3_colmax(const float2* err, const float* sq, int n, float* out3, cudaStream_t s);
 int pca_tc_splits(int P, int D);
 int launch_pca_partial_tc(const __nv_bfloat16* w_hi, const __nv_bfloat16* w_lo, int P,
                           const __nv_bfloat16* v_hi, const __nv_bfloat16* v_lo, int N, int D,

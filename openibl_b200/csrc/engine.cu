@@ -965,71 +965,56 @@ int ibl_l2dist_topk(ibl_engine* e, const float* q, int m, const float* db, int n
     IBL_RET(launch_planes_sqnorm(q, m, d, qh, qh + qe, e->qn.as<float>(), e->q_err.as<float2>(), s));
     IBL_RET(launch_planes_sqnorm(db, n, d, dh, dh + de, e->dbn.as<float>(), e->db_err.as<float2>(), s));
     e->launches += 2;
-    const int kc = 16;                           // candidates kept per query before exact re-scoring
     e->flag_counter = reinterpret_cast<const int*>(e->guard_ws.p);
     e->dist_path = k <= 12 ? 2 : 3;
+    int parts, kc;                               // candidate lists per query, candidates per list
     if (k <= 12) {
       // m <= 128 here: one row tile of the bf16x3 top-16 screen (tc_gemm.cu)
+      kc = 16;
       const int max_runs = dist_top16_max_runs(n_valid);
       IBL_RET(e->cand_d.ensure((size_t)max_runs * m * kc * sizeof(float)));
       IBL_RET(e->cand_i.ensure((size_t)max_runs * m * kc * sizeof(int64_t)));
-      int runs = 0;
       IBL_RET(launch_dist_top16_tc(qh, qh + qe, e->qn.as<float>(), m, dh, dh + de, e->dbn.as<float>(), n,
                                    n_valid, d, e->cand_d.as<float>(), e->cand_i.as<long long>(), max_runs,
-                                   &runs, s));
+                                   &parts, s));
       e->launches++;
-      const long long* ci = e->cand_i.as<long long>();
-      const float* cd = e->cand_d.as<float>();
-      if (runs > 1) {
-        IBL_RET(e->mrg_d.ensure((size_t)m * kc * sizeof(float)));
-        IBL_RET(e->mrg_i.ensure((size_t)m * kc * sizeof(int64_t)));
-        IBL_RET(launch_topk_merge(e->cand_d.as<float>(), e->cand_i.as<int64_t>(), runs, m, kc, kc,
-                                  e->mrg_d.as<float>(), e->mrg_i.as<int64_t>(), s));
-        e->launches++;
-        ci = e->mrg_i.as<long long>();
-        cd = e->mrg_d.as<float>();
+    } else {
+      // k > 12: dense tiles on the tensor cores, then a row select per column chunk
+      const int CHT = 32768;
+      parts = cdiv(n_valid, CHT);
+      kc = k + 8 > 128 ? 128 : k + 8;
+      IBL_REQUIRE((long long)parts * kc <= 8192, "database shard too large for one call; shard it");
+      const int chw = n_valid < CHT ? cdiv(n_valid, 4) * 4 : CHT;
+      IBL_RET(e->dist_chunk.ensure((size_t)m * chw * sizeof(float)));
+      IBL_RET(e->cand_d.ensure((size_t)parts * m * kc * sizeof(float)));
+      IBL_RET(e->cand_i.ensure((size_t)parts * m * kc * sizeof(int64_t)));
+      for (int c = 0; c < parts; ++c) {
+        const int j0 = c * CHT;
+        const int nc = (n_valid - j0 < CHT) ? (n_valid - j0) : CHT;
+        IBL_RET(launch_dist_dense_tc(qh, qh + qe, e->qn.as<float>(), m, dh + (size_t)j0 * d, dh + de + (size_t)j0 * d,
+                                     e->dbn.as<float>() + j0, nc, d, e->dist_chunk.as<float>(), chw, s));
+        IBL_RET(launch_topk_rows(e->dist_chunk.as<float>(), chw, m, nc, kc, j0,
+                                 e->cand_d.as<float>() + (size_t)c * m * kc, e->cand_i.as<int64_t>() + (size_t)c * m * kc,
+                                 false, s));
+        e->launches += 2;
       }
-      IBL_RET(launch_rescore_sort(q, e->qn.as<float>(), m, db, e->dbn.as<float>(), d, ci, kc, k, idx_base,
-                                  out_dist, reinterpret_cast<long long*>(out_idx), s));
-      e->launches++;
-      // guard: queries whose 16 survivors cannot be shown to hold the exact top-k are ranked by exact brute force
-      return launch_dist_guard_bf16x3(q, e->qn.as<float>(), qerr, m, db, e->dbn.as<float>(), dberr, n_valid, d, cd, kc,
-                                      k, idx_base, e->guard_ws.p, out_dist, reinterpret_cast<long long*>(out_idx),
-                                      &e->launches, s);
-    }
-    // k > 12: dense tiles on the tensor cores, row select, then the same exact re-scoring
-    const int CHT = 32768;
-    const int ncht = cdiv(n_valid, CHT);
-    const int kk = k + 8 > 128 ? 128 : k + 8;
-    IBL_REQUIRE((long long)ncht * kk <= 8192, "database shard too large for one call; shard it");
-    const int chw = n_valid < CHT ? cdiv(n_valid, 4) * 4 : CHT;
-    IBL_RET(e->dist_chunk.ensure((size_t)m * chw * sizeof(float)));
-    IBL_RET(e->cand_d.ensure((size_t)ncht * m * kk * sizeof(float)));
-    IBL_RET(e->cand_i.ensure((size_t)ncht * m * kk * sizeof(int64_t)));
-    for (int c = 0; c < ncht; ++c) {
-      const int j0 = c * CHT;
-      const int nc = (n_valid - j0 < CHT) ? (n_valid - j0) : CHT;
-      IBL_RET(launch_dist_dense_tc(qh, qh + qe, e->qn.as<float>(), m, dh + (size_t)j0 * d, dh + de + (size_t)j0 * d,
-                                   e->dbn.as<float>() + j0, nc, d, e->dist_chunk.as<float>(), chw, s));
-      IBL_RET(launch_topk_rows(e->dist_chunk.as<float>(), chw, m, nc, kk, j0, e->cand_d.as<float>() + (size_t)c * m * kk,
-                               e->cand_i.as<int64_t>() + (size_t)c * m * kk, false, s));
-      e->launches += 2;
     }
     const long long* ci = e->cand_i.as<long long>();
     const float* cd = e->cand_d.as<float>();
-    if (ncht > 1) {
-      IBL_RET(e->mrg_d.ensure((size_t)m * kk * sizeof(float)));
-      IBL_RET(e->mrg_i.ensure((size_t)m * kk * sizeof(int64_t)));
-      IBL_RET(launch_topk_merge(e->cand_d.as<float>(), e->cand_i.as<int64_t>(), ncht, m, kk, kk,
+    if (parts > 1) {
+      IBL_RET(e->mrg_d.ensure((size_t)m * kc * sizeof(float)));
+      IBL_RET(e->mrg_i.ensure((size_t)m * kc * sizeof(int64_t)));
+      IBL_RET(launch_topk_merge(e->cand_d.as<float>(), e->cand_i.as<int64_t>(), parts, m, kc, kc,
                                 e->mrg_d.as<float>(), e->mrg_i.as<int64_t>(), s));
       e->launches++;
       ci = e->mrg_i.as<long long>();
       cd = e->mrg_d.as<float>();
     }
-    IBL_RET(launch_rescore_sort(q, e->qn.as<float>(), m, db, e->dbn.as<float>(), d, ci, kk, k, idx_base, out_dist,
+    IBL_RET(launch_rescore_sort(q, e->qn.as<float>(), m, db, e->dbn.as<float>(), d, ci, kc, k, idx_base, out_dist,
                                 reinterpret_cast<long long*>(out_idx), s));
     e->launches++;
-    return launch_dist_guard_bf16x3(q, e->qn.as<float>(), qerr, m, db, e->dbn.as<float>(), dberr, n_valid, d, cd, kk, k,
+    // guard: queries whose kc survivors cannot be shown to hold the exact top-k are ranked by exact brute force
+    return launch_dist_guard_bf16x3(q, e->qn.as<float>(), qerr, m, db, e->dbn.as<float>(), dberr, n_valid, d, cd, kc, k,
                                     idx_base, e->guard_ws.p, out_dist, reinterpret_cast<long long*>(out_idx),
                                     &e->launches, s);
   }

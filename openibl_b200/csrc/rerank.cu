@@ -6,7 +6,7 @@
 //      (d^2, index) and the row maximum M = max_j d^2, every value an exact fp32 distance (d1_exact).  Screening runs
 //      on the tensor cores (bf16x3 dense tiles, launch_dist_dense_tc) in 32768-column chunks; per chunk the nearest
 //      kn = w + 8 screened columns (launch_topk_rows) and the KNN_FAR farthest (knn_far_select_kernel) are kept and
-//      re-scored exactly.  Two guards with the screening bound B of dist_exact.cuh decide whether the re-scored lists
+//      re-scored exactly.  Two guards with the screening bound B of ranking.cuh decide whether the re-scored lists
 //      are provably the exact answer; rows they cannot clear are ranked again by an exact scan of all N columns.
 //   2. sparse stage (launch_rerank_topk), one warp or block per row, the sets in shared memory:
 //        Kr / Kc      k-reciprocal sets of width k1+1 and round(k1/2)+1                    (rerank.py:51-57,60-64)
@@ -32,30 +32,13 @@
 #include <vector>
 
 #include "common.cuh"
-#include "dist_exact.cuh"
+#include "ranking.cuh"
 
 namespace ibl {
 
 // ------------------------------------------------------------------------------------------------------------------
 // shared helpers
 // ------------------------------------------------------------------------------------------------------------------
-
-// ascending bitonic sort of n (power of two) u64 keys in shared memory, any block size
-__device__ void rr_sort_u64(unsigned long long* buf, int n) {
-  for (int size = 2; size <= n; size <<= 1) {
-    for (int stride = size >> 1; stride > 0; stride >>= 1) {
-      __syncthreads();
-      for (int i = threadIdx.x; i < (n >> 1); i += blockDim.x) {
-        const int lo = 2 * i - (i & (stride - 1));
-        const int hi = lo + stride;
-        const bool up = ((lo & size) == 0);
-        const unsigned long long a = buf[lo], b = buf[hi];
-        if ((a > b) == up) { buf[lo] = b; buf[hi] = a; }
-      }
-    }
-  }
-  __syncthreads();
-}
 
 // key of (d^2, column): d^2 >= 0, so its bit pattern orders like the value
 __device__ __forceinline__ unsigned long long sq_key(float e, unsigned col) {
@@ -75,29 +58,6 @@ constexpr int KNN_FAR = 8;          // farthest screened columns kept per row an
 constexpr int KNN_CHT = 32768;      // columns per dense screening chunk
 constexpr int KNN_ROWS = 1024;      // rows per dense screening chunk (128 MB of screened distances)
 
-// max over the rows of {|lo|, |x - hi - lo|, |x|^2}: the column side of the bound B
-__global__ void knn_colmax_kernel(const float2* __restrict__ err, const float* __restrict__ sq, int n,
-                                  float* __restrict__ out3) {
-  float a = 0.f, b = 0.f, c = 0.f;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const float2 v = __ldg(err + i);
-    a = fmaxf(a, v.x);
-    b = fmaxf(b, v.y);
-    c = fmaxf(c, __ldg(sq + i));
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    a = fmaxf(a, __shfl_xor_sync(0xffffffffu, a, o));
-    b = fmaxf(b, __shfl_xor_sync(0xffffffffu, b, o));
-    c = fmaxf(c, __shfl_xor_sync(0xffffffffu, c, o));
-  }
-  if ((threadIdx.x & 31) == 0) {     // non-negative floats order like their bit patterns
-    atomicMax(reinterpret_cast<int*>(out3), __float_as_int(a));
-    atomicMax(reinterpret_cast<int*>(out3) + 1, __float_as_int(b));
-    atomicMax(reinterpret_cast<int*>(out3) + 2, __float_as_int(c));
-  }
-}
-
 // One block per row of a screened chunk [rows][ld], nc valid columns starting at global column j0.  Every thread
 // keeps its two largest screened values; the KNN_FAR largest thread maxima are the row's far candidates, and
 // u = max(the next thread maximum, every thread's second largest) bounds the screened value of every column that
@@ -116,22 +76,22 @@ knn_far_select_kernel(const float* __restrict__ chunk, long long ld, int nc, int
     if (i1 < 0 || v > s1) { s2 = s1; s1 = v; i1 = j; }
     else if (v > s2) s2 = v;
   }
-  keys[threadIdx.x] = i1 < 0 ? ~0ull : ((unsigned long long)(~d1_ord(s1)) << 32) | (unsigned)i1;   // largest first
+  keys[threadIdx.x] = i1 < 0 ? ~0ull : ((unsigned long long)(~ord_key(s1)) << 32) | (unsigned)i1;   // largest first
   float m2 = s2;
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) m2 = fmaxf(m2, __shfl_xor_sync(0xffffffffu, m2, o));
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m2;
-  rr_sort_u64(keys, 256);
+  block_bitonic_sort(keys, 256);
   if (threadIdx.x < KNN_FAR) {
     const unsigned long long k = keys[threadIdx.x];
-    far_s[row * KNN_FAR + threadIdx.x] = k == ~0ull ? -INFINITY : d1_unord(~(uint32_t)(k >> 32));
+    far_s[row * KNN_FAR + threadIdx.x] = k == ~0ull ? -INFINITY : unord_key(~(uint32_t)(k >> 32));
     far_i[row * KNN_FAR + threadIdx.x] = k == ~0ull ? -1 : j0 + (int)(uint32_t)(k & 0xffffffffu);
   }
   if (threadIdx.x == 0) {
     float u = -INFINITY;
     for (int i = 0; i < 8; ++i) u = fmaxf(u, red[i]);
     const unsigned long long k = keys[KNN_FAR];
-    if (k != ~0ull) u = fmaxf(u, d1_unord(~(uint32_t)(k >> 32)));
+    if (k != ~0ull) u = fmaxf(u, unord_key(~(uint32_t)(k >> 32)));
     far_u[row] = u;
   }
   (void)rows;
@@ -189,7 +149,7 @@ knn_finish_kernel(const KnnFinishArgs g) {
   // keys[c] is tied to ex[c] through the column; sort a copy of the keys only and look the distance up
   __shared__ unsigned long long sk[256];
   for (int i = threadIdx.x; i < 256; i += 128) sk[i] = keys[i];
-  rr_sort_u64(sk, 256);
+  block_bitonic_sort(sk, 256);
   for (int t = threadIdx.x; t < g.w; t += 128) {
     const unsigned long long k = sk[t];
     float e = INFINITY;
@@ -256,7 +216,7 @@ knn_exact_kernel(const KnnFinishArgs g) {
         }
         if (lane == 0) keys[256 + t] = key;
       }
-      rr_sort_u64(keys, 512);
+      block_bitonic_sort(keys, 512);
     }
     if (lane == 0) wmax[wid] = mx;
     for (int t = wid; t < g.w; t += 8) {      // the signed distance of each listed column, recomputed
@@ -354,8 +314,7 @@ int launch_knn_rowmax(const float* X, int N, int d, int row0, int n_rows, int w,
 
   IBL_RET(launch_planes_sqnorm(x, N, dp, hi, lo, sq, err, s));
   IBL_CUDA_OK(cudaMemsetAsync(cmax, 0, 32, s));   // column maxima, this chunk's and the call's listed rows
-  knn_colmax_kernel<<<std::min(64, cdiv(N, 256)), 256, 0, s>>>(err, sq, N, cmax);
-  IBL_CUDA_OK(cudaGetLastError());
+  IBL_RET(launch_bf16x3_colmax(err, sq, N, cmax, s));
   uint64_t nl = 3;
   const int kn = std::min(L.kn, N);                // near candidates per row (all columns when N <= w + 8)
   for (int r0 = 0; r0 < n_rows; r0 += L.R) {
@@ -587,19 +546,7 @@ rr_expand_kernel(const ExpandArgs g) {
       for (int t = lane; t < nc; t += 32) buf[at + t] = g.kc[(long long)c * g.wc + t];
     }
   }
-  // bitonic sort of the int buffer
-  for (int size = 2; size <= g.cap; size <<= 1) {
-    for (int stride = size >> 1; stride > 0; stride >>= 1) {
-      __syncthreads();
-      for (int t = threadIdx.x; t < (g.cap >> 1); t += 128) {
-        const int lo = 2 * t - (t & (stride - 1)), hi = lo + stride;
-        const bool up = ((lo & size) == 0);
-        const int a = buf[lo], b = buf[hi];
-        if ((a > b) == up) { buf[lo] = b; buf[hi] = a; }
-      }
-    }
-  }
-  __syncthreads();
+  block_bitonic_sort(buf, g.cap);
   // unique, in place (one thread: at most cap entries)
   if (threadIdx.x == 0) {
     int u = 0;
@@ -678,7 +625,7 @@ rr_mean_kernel(const MeanArgs g) {
       keys[base + t] = ((unsigned long long)(unsigned)g.cols[start[q] + t] << 32) | ((unsigned)q << 24) | (unsigned)t;
     base += len[q];
   }
-  rr_sort_u64(keys, g.cap);
+  block_bitonic_sort(keys, g.cap);
   if (threadIdx.x == 0) {          // compact: one sum per column, in neighbour order
     int u = 0;
     const float fk2 = (float)g.k2;
@@ -823,10 +770,10 @@ rr_topk_kernel(const TopkArgs g) {
         const float e = d1_exact(xr, g.x + (long long)(g.m + r) * g.d, g.d, lane, an, __ldg(g.sq + g.m + r));
         dn = __fdiv_rn(__fmul_rn(e, e), M);
       }
-      if (lane == 0) best[256 + t] = ((unsigned long long)d1_ord(rr_final(jj[t], dn, g.lam, g.oml)) << 32) | (unsigned)r;
+      if (lane == 0) best[256 + t] = rank_key(rr_final(jj[t], dn, g.lam, g.oml), (unsigned)r);
     }
     __syncthreads();
-    rr_sort_u64(best, 512);
+    block_bitonic_sort(best, 512);
     for (int t = threadIdx.x; t < 256; t += 256) best[256 + t] = ~0ull;
     __syncthreads();
   };
@@ -880,11 +827,7 @@ rr_topk_kernel(const TopkArgs g) {
     cnt_s = c;
   }
   score_tile();
-  for (int t = threadIdx.x; t < g.k; t += 256) {
-    const unsigned long long key = best[t];
-    g.out_dist[(long long)qi * g.k + t] = key == ~0ull ? INFINITY : d1_unord((uint32_t)(key >> 32));
-    g.out_idx[(long long)qi * g.k + t] = key == ~0ull ? -1 : (long long)(uint32_t)(key & 0xffffffffu);
-  }
+  for (int t = threadIdx.x; t < g.k; t += 256) store_ranked(best[t], 0, g.out_dist, g.out_idx, (long long)qi * g.k + t);
 }
 
 // final = fl(fl(jac * c1) + fl(q * c2)), c1 = fp32(1 - lambda), c2 = fp32(lambda): rerank.py:94 in float32 (NEP 50).

@@ -7,15 +7,11 @@
 //                     finds its merged position with one binary search in the sibling run (keys are unique, so
 //                     lower_bound on one side and on the other give a stable, collision-free scatter)
 #include "common.cuh"
+#include "ranking.cuh"
 
 namespace ibl {
 
 constexpr int SR_CHUNK = 16384;
-
-__device__ __forceinline__ uint32_t sr_ord(float f) {
-  uint32_t u = __float_as_uint(f);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
 
 // grid (chunks, m); sorts columns [c*SR_CHUNK, ...) of row r; writes u64 keys (runs) or final int64 indices
 __global__ void __launch_bounds__(1024)
@@ -27,20 +23,8 @@ sort_chunk_kernel(const float* __restrict__ dist, long long ld, int n, unsigned 
   const int len = min(SR_CHUNK, n - c0);
   const float* d = dist + r * ld + c0;
   for (int i = threadIdx.x; i < cap; i += blockDim.x)
-    sk[i] = i < len ? (((unsigned long long)sr_ord(d[i]) << 32) | (unsigned)(c0 + i)) : ~0ull;
-  for (int size = 2; size <= cap; size <<= 1) {
-    for (int stride = size >> 1; stride > 0; stride >>= 1) {
-      __syncthreads();
-      for (int i = threadIdx.x; i < (cap >> 1); i += blockDim.x) {
-        const int lo = 2 * i - (i & (stride - 1));
-        const int hi = lo + stride;
-        const bool up = ((lo & size) == 0);
-        const unsigned long long a = sk[lo], b = sk[hi];
-        if ((a > b) == up) { sk[lo] = b; sk[hi] = a; }
-      }
-    }
-  }
-  __syncthreads();
+    sk[i] = i < len ? rank_key(d[i], (unsigned)(c0 + i)) : ~0ull;
+  block_bitonic_sort(sk, cap);
   for (int i = threadIdx.x; i < len; i += blockDim.x) {
     if (idx_out) idx_out[r * n + c0 + i] = (long long)(uint32_t)(sk[i] & 0xffffffffu);
     else keys_out[r * n + c0 + i] = sk[i];

@@ -11,7 +11,7 @@
 //                             half, 128 queries x 128 database rows per tile, 5-stage TMA ring, running
 //                             top-16 per query in registers across the CTA's database range;
 //   3. dist_finish_kernel     per query: merge of the per-range candidate lists, exact fp32 re-scoring of the 16
-//                             survivors (|q|^2 + |d|^2 - 2 q.d, bit-identical to round 1's rescore_sort_kernel),
+//                             survivors (|q|^2 + |d|^2 - 2 q.d, d1_exact as in rescore_sort_kernel),
 //                             final (dist, idx) sort, and the GUARD: a database row that was NOT kept has a
 //                             screened distance >= s16 (the 16th screened distance); its exact distance is
 //                             >= s16 - B, B = d1_screen_bound: a rigorous bound of the operand rounding (the rows'
@@ -28,7 +28,7 @@
 
 #include "common.cuh"
 #include "tc_common.cuh"
-#include "dist_exact.cuh"
+#include "ranking.cuh"
 
 namespace ibl {
 
@@ -235,22 +235,7 @@ gemm_f16_top16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_con
         for (int e = 0; e < longest; ++e) {
           if (e < cnt) {
             const float2 v = d1_lds64(pend + e * 1024);
-            const float d = v.x;
-            if (d < td[15]) {
-              const int col = __float_as_int(v.y);
-              // Sorted insert without a dependency chain: the slot is counted with 16 independent compares and every
-              // entry is rewritten from the OLD values of itself and its left neighbour (descending s).
-              int pos = 0;
-#pragma unroll
-              for (int s = 0; s < 16; ++s) pos += (td[s] <= d) ? 1 : 0;
-#pragma unroll
-              for (int s = 15; s > 0; --s) {
-                const bool shift = s > pos, here = s == pos;
-                td[s] = shift ? td[s - 1] : (here ? d : td[s]);
-                ti[s] = shift ? ti[s - 1] : (here ? col : ti[s]);
-              }
-              if (pos == 0) { td[0] = d; ti[0] = col; }
-            }
+            top16_insert(td, ti, v.x, __float_as_int(v.y));
           }
         }
         paddr = pend;
@@ -263,7 +248,7 @@ gemm_f16_top16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_con
         // costs efficiency.  Ties at the gate are dropped: the guard's error bound covers them.
         if (row_ok) {
           const unsigned gv = *reinterpret_cast<volatile unsigned*>(g.gate + row);
-          if (gv != 0xFFFFFFFFu) thr = fminf(thr, d1_unord(gv));       // 0xFFFFFFFF = "no gate yet" (the memset pattern)
+          if (gv != 0xFFFFFFFFu) thr = fminf(thr, unord_key(gv));       // 0xFFFFFFFF = "no gate yet" (the memset pattern)
         }
         Acc128<D1_BN> acc;
         int prev = -1;
@@ -319,7 +304,7 @@ gemm_f16_top16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_con
         merge_pending();
         if (row_ok && td[15] < thr) {
           thr = td[15];
-          atomicMin(g.gate + row, d1_ord(thr));
+          atomicMin(g.gate + row, ord_key(thr));
         }
       }
       if (row_ok) {
@@ -349,7 +334,7 @@ struct FinishArgs {
   int* flag_count; int* flag_list; int* list_cnt;
 };
 
-// The guard's B: d1_screen_bound (dist_exact.cuh).
+// The guard's B: d1_screen_bound (ranking.cuh).
 
 __global__ void __launch_bounds__(128)
 dist_finish_kernel(const FinishArgs g) {
@@ -373,24 +358,11 @@ dist_finish_kernel(const FinishArgs g) {
       const int r = threadIdx.x >> 4, j = threadIdx.x & 15;
       const long long src = ((long long)r * g.m + row) * 16 + j;
       const int ci = g.cand_i[src];
-      if (ci >= 0) key = ((unsigned long long)d1_ord(g.cand_d[src]) << 32) | (unsigned)ci;
+      if (ci >= 0) key = rank_key(g.cand_d[src], (unsigned)ci);
     }
     skeys[threadIdx.x] = key;
   }
-  for (int size = 2; size <= 128; size <<= 1) {
-    for (int stride = size >> 1; stride > 0; stride >>= 1) {
-      __syncthreads();
-      if (threadIdx.x < 64) {
-        const int i = threadIdx.x;
-        const int lo = 2 * i - (i & (stride - 1));
-        const int hi = lo + stride;
-        const bool up = ((lo & size) == 0);
-        const unsigned long long a = skeys[lo], b = skeys[hi];
-        if ((a > b) == up) { skeys[lo] = b; skeys[hi] = a; }
-      }
-    }
-  }
-  __syncthreads();
+  block_bitonic_sort(skeys, 128);
   const float4 qa = __ldg(g.q_aux + row);
   // ---- exact fp32 re-scoring of the 16 survivors ----
   for (int c = wid; c < 128; c += 4) {
@@ -399,36 +371,14 @@ dist_finish_kernel(const FinishArgs g) {
       const unsigned long long sk = skeys[c];
       if (sk != ~0ull) {
         const long long ci = (long long)(uint32_t)(sk & 0xffffffffu);
-        const float dist = d1_exact(qrow, g.db + ci * d, d, lane, qa.x, __ldg(&g.db_aux[ci].x));
-        key = ((unsigned long long)d1_ord(dist) << 32) | (unsigned)ci;
+        key = rank_key(d1_exact(qrow, g.db + ci * d, d, lane, qa.x, __ldg(&g.db_aux[ci].x)), (unsigned)ci);
       }
     }
     if (lane == 0) keys[c] = key;
   }
-  for (int size = 2; size <= 16; size <<= 1) {          // only keys[0..15] can be valid
-    for (int stride = size >> 1; stride > 0; stride >>= 1) {
-      __syncthreads();
-      if (threadIdx.x < 8) {
-        const int i = threadIdx.x;
-        const int lo = 2 * i - (i & (stride - 1));
-        const int hi = lo + stride;
-        const bool up = ((lo & size) == 0);
-        const unsigned long long a = keys[lo], b = keys[hi];
-        if ((a > b) == up) { keys[lo] = b; keys[hi] = a; }
-      }
-    }
-  }
-  __syncthreads();
-  if ((int)threadIdx.x < g.k_out) {
-    const unsigned long long key = keys[threadIdx.x];
-    if (key == ~0ull) {
-      g.out_dist[row * g.k_out + threadIdx.x] = INFINITY;
-      g.out_idx[row * g.k_out + threadIdx.x] = -1;
-    } else {
-      g.out_dist[row * g.k_out + threadIdx.x] = d1_unord((uint32_t)(key >> 32));
-      g.out_idx[row * g.k_out + threadIdx.x] = g.idx_base + (long long)(uint32_t)(key & 0xffffffffu);
-    }
-  }
+  block_bitonic_sort(keys, 16);                          // only keys[0..15] can be valid
+  if ((int)threadIdx.x < g.k_out)
+    store_ranked(keys[threadIdx.x], g.idx_base, g.out_dist, g.out_idx, row * g.k_out + threadIdx.x);
   // ---- guard ----
   if (threadIdx.x == 0 && g.n_valid > 16) {              // with <= 16 rows everything was re-scored
     const unsigned long long s16k = skeys[15];
@@ -436,7 +386,7 @@ dist_finish_kernel(const FinishArgs g) {
     const unsigned long long ek = keys[kk - 1];
     bool flag = (s16k == ~0ull) || (ek == ~0ull);        // cannot happen with n_valid > 16; be safe
     if (!flag) {
-      const float s16 = d1_unord((uint32_t)(s16k >> 32)), e_k = d1_unord((uint32_t)(ek >> 32));
+      const float s16 = unord_key((uint32_t)(s16k >> 32)), e_k = unord_key((uint32_t)(ek >> 32));
       // fp16 operands: no lo plane, one MMA per K step; the residuals include the subnormals' rounding
       const float bound = d1_screen_bound(qa.x, 0.f, qa.z, __ldg(g.db_max2 + 2), 0.f, __ldg(g.db_max2), d, 1);
       flag = !(s16 - bound > e_k);                       // also catches NaN
@@ -523,7 +473,7 @@ dist_exact_scan_kernel(const ExactArgs g) {
           const float dist = fmaf(-2.f, v, __ldg(g.q_sq + row * g.sq_stride) + bn);
           if (lane == 0 && dist <= g.out_dist[row * g.k + g.k - 1]) {   // e_k of the re-scored list
             const int at = atomicAdd(g.list_cnt + f, 1);
-            if (at < DX_CAP) g.lists[(long long)f * DX_CAP + at] = ((unsigned long long)d1_ord(dist) << 32) | (unsigned)j;
+            if (at < DX_CAP) g.lists[(long long)f * DX_CAP + at] = rank_key(dist, (unsigned)j);
           }
         }
       }
@@ -543,27 +493,13 @@ static int dx_scan_attr() {
 
 static size_t dx_scan_smem(int d) { return (size_t)min(DX_QG, max(1, (DX_QSMEM / 4) / d)) * d * sizeof(float); }
 
-// 512 keys in shared memory, ascending (256 threads)
-__device__ __forceinline__ void dx_sort512(unsigned long long* keys) {
-  for (int size = 2; size <= 512; size <<= 1) {
-    for (int stride = size >> 1; stride > 0; stride >>= 1) {
-      __syncthreads();
-      const int i = threadIdx.x;
-      const int lo = 2 * i - (i & (stride - 1));
-      const int hi = lo + stride;
-      const bool up = ((lo & size) == 0);
-      const unsigned long long a = keys[lo], b = keys[hi];
-      if ((a > b) == up) { keys[lo] = b; keys[hi] = a; }
-    }
-  }
-  __syncthreads();
-}
-
 // one block per listed query: sort its list (or, on overflow, scan the database 256 rows at a time keeping the 256
 // best) and write the final top-k
 __global__ void __launch_bounds__(256)
 dist_exact_finish_kernel(const ExactArgs g) {
   __shared__ unsigned long long keys[512];
+  // the launch size: one compare-exchange per thread and step of the 512-key sort (unrolled, ptxas spills otherwise)
+  __builtin_assume(blockDim.x == 256);
   const int count = *g.flag_count;
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   for (int f = blockIdx.x; f < count; f += gridDim.x) {
@@ -574,7 +510,7 @@ dist_exact_finish_kernel(const ExactArgs g) {
       keys[i] = (cnt <= DX_CAP && i < cnt) ? g.lists[(long long)f * DX_CAP + i] : ~0ull;
     __syncthreads();
     if (cnt <= DX_CAP) {
-      dx_sort512(keys);
+      block_bitonic_sort(keys, 512);
     } else {
       const float* qrow = g.q + row * g.d;
       const float an = __ldg(g.q_sq + row * g.sq_stride);
@@ -583,26 +519,23 @@ dist_exact_finish_kernel(const ExactArgs g) {
           const int j = j0 + t;
           unsigned long long key = ~0ull;
           if (j < g.n_valid) {
-            const float dist = d1_exact(qrow, g.db + (long long)j * g.d, g.d, lane, an,
-                                        __ldg(g.db_sq + (long long)j * g.sq_stride));
-            key = ((unsigned long long)d1_ord(dist) << 32) | (unsigned)j;
+            key = rank_key(d1_exact(qrow, g.db + (long long)j * g.d, g.d, lane, an,
+                                    __ldg(g.db_sq + (long long)j * g.sq_stride)),
+                           (unsigned)j);
           }
           if (lane == 0) keys[256 + t] = key;
         }
-        dx_sort512(keys);
+        block_bitonic_sort(keys, 512);
       }
     }
-    if ((int)threadIdx.x < g.k) {
-      const unsigned long long key = keys[threadIdx.x];
-      g.out_dist[row * g.k + threadIdx.x] = key == ~0ull ? INFINITY : d1_unord((uint32_t)(key >> 32));
-      g.out_idx[row * g.k + threadIdx.x] = key == ~0ull ? -1 : g.idx_base + (long long)(uint32_t)(key & 0xffffffffu);
-    }
+    if ((int)threadIdx.x < g.k) store_ranked(keys[threadIdx.x], g.idx_base, g.out_dist, g.out_idx, row * g.k + threadIdx.x);
   }
 }
 
 // ---- 5. guard + exact fallback for the bf16x3 screening paths (tc_gemm.cu) -----------------------------
-// max over the database rows of (|lo|, |x - hi - lo|, |x|^2)
-__global__ void dist_guard_colmax_kernel(const float2* __restrict__ err, const float* __restrict__ sq, int n,
+// max over the database rows of (|lo|, |x - hi - lo|, |x|^2): the column side of the guard's bound after bf16x3
+// screening (here and in rerank.cu's neighbour pass)
+__global__ void bf16x3_colmax_kernel(const float2* __restrict__ err, const float* __restrict__ sq, int n,
                                          float* __restrict__ out3) {
   float a = 0.f, b = 0.f, c = 0.f;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
@@ -622,6 +555,12 @@ __global__ void dist_guard_colmax_kernel(const float2* __restrict__ err, const f
     atomicMax(reinterpret_cast<int*>(out3) + 1, __float_as_int(b));
     atomicMax(reinterpret_cast<int*>(out3) + 2, __float_as_int(c));
   }
+}
+
+int launch_bf16x3_colmax(const float2* err, const float* sq, int n, float* out3, cudaStream_t s) {
+  bf16x3_colmax_kernel<<<cdiv(n, 256) < 64 ? cdiv(n, 256) : 64, 256, 0, s>>>(err, sq, n, out3);
+  IBL_CUDA_OK(cudaGetLastError());
+  return IBL_OK;
 }
 
 // one thread per query.  screened [m][kc]: the kc smallest screened distances, ascending; a row that is not among
@@ -775,7 +714,7 @@ int launch_dist_guard_bf16x3(const float* q, const float* q_sq, const float2* q_
   int* lcnt = flist + m;
   unsigned long long* lists = reinterpret_cast<unsigned long long*>(w + guard_lists_at(m));
   IBL_CUDA_OK(cudaMemsetAsync(w, 0, 32, s));
-  dist_guard_colmax_kernel<<<cdiv(n_valid, 256) < 64 ? cdiv(n_valid, 256) : 64, 256, 0, s>>>(db_err, db_sq, n_valid, dmax3);
+  IBL_RET(launch_bf16x3_colmax(db_err, db_sq, n_valid, dmax3, s));
   dist_guard_kernel<<<cdiv(m, 128), 128, 0, s>>>(screened, kc, q_sq, q_err, dmax3, out_dist, k, m, d, n_valid, fcount,
                                                 flist, lcnt);
   ExactArgs x{};

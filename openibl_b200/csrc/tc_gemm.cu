@@ -14,6 +14,7 @@
 // round-robin to a persistent grid.  Warp roles as in tc_conv.cu.
 #include "common.cuh"
 #include "tc_common.cuh"
+#include "ranking.cuh"
 
 namespace ibl {
 
@@ -221,24 +222,13 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tm_ahi, const __grid_constant
               }
             }
           } else {  // EPI_TOP16
-            // one coalesced load of the chunk's |d|^2 terms + shuffles, chain-free sorted insert (see tc_dist1.cu)
+            // one coalesced load of the chunk's |d|^2 terms + shuffles
             const float bmine = (col0 + lane < g.n_valid) ? __ldg(g.bn + col0 + lane) : INFINITY;
 #pragma unroll
             for (int j = 0; j < 32; ++j) {
               const int col = col0 + j;
               const float d = fmaf(-2.f, __uint_as_float(raw[j]), an + __shfl_sync(0xffffffffu, bmine, j));
-              if (d < td[15]) {
-                int pos = 0;
-#pragma unroll
-                for (int s = 0; s < 16; ++s) pos += (td[s] <= d) ? 1 : 0;
-#pragma unroll
-                for (int s = 15; s > 0; --s) {
-                  const bool shift = s > pos, here = s == pos;
-                  td[s] = shift ? td[s - 1] : (here ? d : td[s]);
-                  ti[s] = shift ? ti[s - 1] : (here ? col : ti[s]);
-                }
-                if (pos == 0) { td[0] = d; ti[0] = col; }
-              }
+              top16_insert(td, ti, d, col);
             }
           }
         }
@@ -422,11 +412,6 @@ int pca_tc_splits(int P, int D) {
 // ---- exact fp32 re-scoring of a candidate list + final ordering ---------------------------------
 // one block (128 threads) per query: dist = |q|^2 + |d|^2 - 2 q.d with an fp32 dot product, then
 // (dist, idx)-ascending sort of the kc <= 128 candidates; writes the first k_out.
-__device__ __forceinline__ uint32_t f32_ord(float f) {
-  uint32_t u = __float_as_uint(f);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-
 __global__ void __launch_bounds__(128)
 rescore_sort_kernel(const float* __restrict__ q, const float* __restrict__ qn,
                     const float* __restrict__ db, const float* __restrict__ dbn, int d,
@@ -451,48 +436,13 @@ rescore_sort_kernel(const float* __restrict__ q, const float* __restrict__ qn,
     if (c < kc) {
       const long long ci = cand_i[row * kc + c];
       if (ci >= 0) {
-        const float* dp = db + ci * d;
-        float acc = 0.f;
-        for (int i = lane * 4; i < d; i += 128) {
-          const float4 a = *reinterpret_cast<const float4*>(qrow + i);
-          const float4 b = __ldg(reinterpret_cast<const float4*>(dp + i));
-          acc = fmaf(a.x, b.x, acc); acc = fmaf(a.y, b.y, acc);
-          acc = fmaf(a.z, b.z, acc); acc = fmaf(a.w, b.w, acc);
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-        const float dist = fmaf(-2.f, acc, an + __ldg(dbn + ci));
-        key = ((unsigned long long)f32_ord(dist) << 32) | (unsigned)ci;
+        key = rank_key(d1_exact(qrow, db + ci * d, d, lane, an, __ldg(dbn + ci)), (unsigned)ci);
       }
     }
     if (lane == 0) keys[c] = key;
   }
-  // bitonic sort of 128 keys, one per thread pair
-  for (int size = 2; size <= 128; size <<= 1) {
-    for (int stride = size >> 1; stride > 0; stride >>= 1) {
-      __syncthreads();
-      if (threadIdx.x < 64) {
-        const int i = threadIdx.x;
-        const int lo = 2 * i - (i & (stride - 1));
-        const int hi = lo + stride;
-        const bool up = ((lo & size) == 0);
-        const unsigned long long a = keys[lo], b = keys[hi];
-        if ((a > b) == up) { keys[lo] = b; keys[hi] = a; }
-      }
-    }
-  }
-  __syncthreads();
-  if (threadIdx.x < k_out) {
-    const unsigned long long key = keys[threadIdx.x];
-    if (key == ~0ull) {
-      out_dist[row * k_out + threadIdx.x] = INFINITY;
-      out_idx[row * k_out + threadIdx.x] = -1;
-    } else {
-      const uint32_t u = (uint32_t)(key >> 32);
-      out_dist[row * k_out + threadIdx.x] = __uint_as_float((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u);
-      out_idx[row * k_out + threadIdx.x] = idx_base + (long long)(uint32_t)(key & 0xffffffffu);
-    }
-  }
+  block_bitonic_sort(keys, 128);
+  if (threadIdx.x < k_out) store_ranked(keys[threadIdx.x], idx_base, out_dist, out_idx, row * k_out + threadIdx.x);
 }
 
 int launch_rescore_sort(const float* q, const float* qn, int m, const float* db, const float* dbn, int d,

@@ -2,36 +2,12 @@
 // reference ibl/evaluators.py:143; only the first 10 (120 with nms) ranks are read, :151-159).
 // Order is (distance, index) ascending: ties go to the lowest database index.
 #include "common.cuh"
+#include "ranking.cuh"
 
 namespace ibl {
 
-__device__ __forceinline__ uint32_t f32_orderable(float f) {
-  uint32_t u = __float_as_uint(f);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float orderable_f32(uint32_t u) {
-  return __uint_as_float((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u);
-}
-
 constexpr int TK_PER_ITER = 1024; // elements examined per block iteration (4 per thread)
 constexpr unsigned long long TK_MAX = ~0ull;
-
-// in-place ascending bitonic sort of n u64 keys in shared memory, 256 threads
-__device__ void bitonic_sort_u64(unsigned long long* buf, int n /*power of two*/) {
-  for (int size = 2; size <= n; size <<= 1) {
-    for (int stride = size >> 1; stride > 0; stride >>= 1) {
-      __syncthreads();
-      for (int i = threadIdx.x; i < (n >> 1); i += blockDim.x) {
-        const int lo = 2 * i - (i & (stride - 1));
-        const int hi = lo + stride;
-        const bool up = ((lo & size) == 0);
-        const unsigned long long a = buf[lo], b = buf[hi];
-        if ((a > b) == up) { buf[lo] = b; buf[hi] = a; }
-      }
-    }
-  }
-  __syncthreads();
-}
 
 // One block per query row.  buf[0,k) holds the best k keys found so far (after a compaction), buf[k, k+cnt)
 // the candidates appended since.  CAP = 2048 serves k <= 128, CAP = 4096 serves k <= 1024 (the reference's
@@ -57,8 +33,7 @@ topk_rows_kernel(const float* __restrict__ dist, long long ld, int n_valid, int 
     for (int u = 0; u < 4; ++u) {
       const int j = j0 + u * 256 + threadIdx.x;
       if (j < n_valid) {
-        const unsigned long long key =
-            ((unsigned long long)f32_orderable(__ldg(d + j)) << 32) | (unsigned)j;
+        const unsigned long long key = rank_key(__ldg(d + j), (unsigned)j);
         if (key < thr) {
           const int pos = atomicAdd(&cnt, 1);
           buf[k + pos] = key;
@@ -71,23 +46,14 @@ topk_rows_kernel(const float* __restrict__ dist, long long ld, int n_valid, int 
     const int c = cnt;
     __syncthreads();
     if (k + c + TK_PER_ITER > CAP) {
-      bitonic_sort_u64(buf, CAP);
+      block_bitonic_sort(buf, CAP);
       for (int i = k + threadIdx.x; i < CAP; i += blockDim.x) buf[i] = TK_MAX;
       if (threadIdx.x == 0) { cnt = 0; thr_s = buf[k - 1]; }
       __syncthreads();
     }
   }
-  bitonic_sort_u64(buf, CAP);
-  for (int i = threadIdx.x; i < k; i += blockDim.x) {
-    const unsigned long long key = buf[i];
-    if (key == TK_MAX) {
-      out_dist[row * k + i] = INFINITY;
-      out_idx[row * k + i] = -1;
-    } else {
-      out_dist[row * k + i] = orderable_f32((uint32_t)(key >> 32));
-      out_idx[row * k + i] = idx_base + (long long)(uint32_t)(key & 0xffffffffu);
-    }
-  }
+  block_bitonic_sort(buf, CAP);
+  for (int i = threadIdx.x; i < k; i += blockDim.x) store_ranked(buf[i], idx_base, out_dist, out_idx, row * k + i);
 }
 
 int launch_topk_rows(const float* dist, long long ld, int m, int n_valid, int k, int64_t idx_base,
@@ -123,7 +89,7 @@ topk_merge_kernel(const float* __restrict__ cand_dist, const long long* __restri
       const int p = i / k_in, j = i - p * k_in;
       const long long src = ((long long)p * m + row) * k_in + j;
       const long long ci = cand_idx[src];
-      if (ci >= 0) { key = f32_orderable(cand_dist[src]); idx = ci; }
+      if (ci >= 0) { key = ord_key(cand_dist[src]); idx = ci; }
     }
     skey[i] = key;
     sidx[i] = idx;
@@ -145,7 +111,7 @@ topk_merge_kernel(const float* __restrict__ cand_dist, const long long* __restri
   __syncthreads();
   for (int i = threadIdx.x; i < k_out; i += blockDim.x) {
     const bool valid = (i < cap) && sidx[i] != 0x7fffffffffffffffll;
-    out_dist[row * k_out + i] = valid ? orderable_f32(skey[i]) : INFINITY;
+    out_dist[row * k_out + i] = valid ? unord_key(skey[i]) : INFINITY;
     out_idx[row * k_out + i] = valid ? sidx[i] : -1;
   }
 }

@@ -182,6 +182,37 @@ int ibl_resize_bilinear_u8(ibl_engine* e, const uint8_t* x_nhwc, int N, int Hin,
 int ibl_extract_host_u8(ibl_engine* e, const uint8_t* x_nhwc_host, int N, int H, int W, const float* mean3,
                         const float* std3, unsigned flags, float* out_host, float* pool_host, void* stream);
 
+/* ---- input side: baseline JPEG decode on the GPU ------------------------------ */
+/* What `Image.open(f).convert('RGB')` does in Preprocessor.__getitem__ (ibl/utils/data/preprocessor.py:31-42) for
+ * baseline JPEGs, bit-identical to Pillow's libjpeg(-turbo) decode with its defaults: accurate integer IDCT
+ * (JDCT_ISLOW), "fancy" triangular chroma upsampling, integer YCbCr->RGB.  Supported: SOF0/SOF1, 8-bit, Huffman, one
+ * interleaved scan, 1 component (grayscale, replicated to RGB) or 3 YCbCr components with luma sampling 1x1, 2x1 or
+ * 2x2 and chroma 1x1; DRI/RSTn; APPn/COM skipped.  Everything else is IBL_ERR_UNSUPPORTED with `reason` set. */
+typedef struct ibl_jpeg_info {
+  int width, height;
+  int components;            /* 1 or 3 */
+  int h_samp, v_samp;        /* luma sampling factors (chroma is 1x1) */
+  int restart_interval;      /* MCUs per restart interval, 0 = none */
+  int intervals;             /* entropy-coded segments (restart intervals) */
+  int mcus;                  /* MCUs in the scan */
+  uint64_t entropy_bytes;    /* entropy-coded bytes after removing the stuffed 0x00 after 0xFF */
+  char reason[120];          /* why the file was rejected ("" when accepted) */
+} ibl_jpeg_info;
+/* Host-only parse of one in-memory file (no device, no engine): headers, Huffman and quantisation tables, restart
+ * segmentation.  IBL_OK for a file ibl_jpeg_decode_u8 decodes; IBL_ERR_UNSUPPORTED for progressive, arithmetic,
+ * 12-bit, CMYK/YCCK, RGB-coded, other sampling, multi-scan, and for files that are cut short, have no EOI or carry a
+ * bad segment length. */
+int ibl_jpeg_parse(const uint8_t* data, size_t len, ibl_jpeg_info* out);
+/* Decode N in-memory JPEG files (HOST pointers files[i], lens[i] bytes) into native-size uint8 HWC RGB at
+ * out_u8 + out_offsets[i] (device buffer, HOST offsets; image i needs height*width*3 bytes).  status[i] (HOST) is
+ * IBL_OK or the ibl_jpeg_parse result; rejected images are not written.  One pinned H2D copy of the destuffed entropy
+ * data and tables, then kernels on `stream`; no synchronisation of this call's work.  err_dev[i] (DEVICE int32) is
+ * set to 0 when the call is enqueued and becomes nonzero if image i's entropy data turns out to be corrupt (an
+ * invalid Huffman code, or a restart interval that ends before its last MCU); every bit read is clamped to its
+ * interval, so a corrupt stream never reads or writes out of bounds. */
+int ibl_jpeg_decode_u8(ibl_engine* e, const uint8_t* const* files, const size_t* lens, int N, uint8_t* out_u8,
+                       const uint64_t* out_offsets, int* status, int* err_dev, void* stream);
+
 /* ---- stage (iii-b): distance + ranking ------------------------------------- */
 /* pairwise_distance(features) with query = gallery = None (evaluators.py:106-114):
  * out[i,j] = 2|x_i|^2 - 2 x_i.x_j, x [n,d], out [n,n]. */

@@ -6,7 +6,7 @@ from __future__ import annotations
 
 import ctypes
 import os
-from ctypes import POINTER, c_char_p, c_double, c_float, c_int, c_int64, c_uint, c_uint64, c_void_p
+from ctypes import POINTER, Structure, c_char, c_char_p, c_double, c_float, c_int, c_int64, c_size_t, c_uint, c_uint64, c_void_p
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libiblb200.so")
@@ -18,6 +18,15 @@ OUT_VLAD, OUT_PCA, OUT_POOL = 0x1, 0x2, 0x4
 CONV_SIMT_FP32, CONV_TC_BF16X3 = 0, 1
 
 _P = c_void_p
+
+
+class JpegInfo(Structure):
+    """ibl_jpeg_info (include/iblb200.h)."""
+    _fields_ = [("width", c_int), ("height", c_int), ("components", c_int), ("h_samp", c_int), ("v_samp", c_int),
+                ("restart_interval", c_int), ("intervals", c_int), ("mcus", c_int), ("entropy_bytes", c_uint64),
+                ("reason", c_char * 120)]
+
+
 # name -> (restype, argtypes); mirrors include/iblb200.h one to one
 SIGNATURES = {
     "ibl_abi_version": (c_int, []),
@@ -50,6 +59,8 @@ SIGNATURES = {
     "ibl_preprocess_u8": (c_int, [_P, _P, c_int, c_int, c_int, _P, _P, _P, _P]),
     "ibl_resize_bilinear_u8": (c_int, [_P, _P, c_int, c_int, c_int, c_int, c_int, _P, _P, c_int, _P, _P, c_int, _P, _P]),
     "ibl_extract_host_u8": (c_int, [_P, _P, c_int, c_int, c_int, _P, _P, c_uint, _P, _P, _P]),
+    "ibl_jpeg_parse": (c_int, [c_char_p, c_size_t, POINTER(JpegInfo)]),
+    "ibl_jpeg_decode_u8": (c_int, [_P, _P, _P, c_int, _P, _P, _P, _P, _P]),
     "ibl_l2dist_dense": (c_int, [_P, _P, c_int, _P, c_int, c_int, _P, _P]),
     "ibl_l2dist_self": (c_int, [_P, _P, c_int, c_int, _P, _P]),
     "ibl_l2dist_topk": (c_int, [_P, _P, c_int, _P, c_int, c_int, c_int, c_int, c_int64, _P, _P, _P]),
@@ -101,6 +112,18 @@ def load(build_if_missing: bool = True) -> ctypes.CDLL:
         fn.argtypes = args
     _lib = lib
     return lib
+
+
+def jpeg_parse(data: bytes) -> dict:
+    """ibl_jpeg_parse on one in-memory file; runs on the host, no device needed."""
+    lib = load()
+    info = JpegInfo()
+    data = bytes(data)
+    st = lib.ibl_jpeg_parse(data, len(data), ctypes.byref(info))
+    return {"ok": st == IBL_OK, "status": st, "width": info.width, "height": info.height,
+            "components": info.components, "h_samp": info.h_samp, "v_samp": info.v_samp,
+            "restart_interval": info.restart_interval, "intervals": info.intervals, "mcus": info.mcus,
+            "entropy_bytes": info.entropy_bytes, "reason": info.reason.decode()}
 
 
 def check(status: int, where: str) -> None:

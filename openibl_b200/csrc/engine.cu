@@ -84,6 +84,7 @@ struct ibl_engine {
   DevBuf q_err, db_err, guard_ws;        // guard of the bf16x3 screening paths: per-row error norms, workspace
   DevBuf knn_ws;                         // neighbour pass of the re-ranking (rerank.cu)
   const int* knn_flag_counter = nullptr; // its count of rows sent to the exact scan (null: no call yet)
+  JpegWs* jpeg_ws = nullptr;             // JPEG decode: pinned staging blob, tables, coefficients, planes (jpeg.cu)
   RerankWs* rr_ws = nullptr;             // sparse stage of the re-ranking: CSR matrices, inverted index, pair buffers
   const int* flag_counter = nullptr;     // guard counter of the last ibl_l2dist_topk call (null: no guard on its path)
   int dist_path = -1;                    // ranking path of the last ibl_l2dist_topk call (ibl_debug_dist_path)
@@ -277,6 +278,7 @@ int ibl_engine_destroy(ibl_engine* e) {
   for (DevBuf* b : bufs) b->release();
   e->knn_ws.release();
   rerank_ws_destroy(e->rr_ws);
+  jpeg_ws_destroy(e->jpeg_ws);
   delete e;
   return IBL_OK;
 }
@@ -798,6 +800,16 @@ int ibl_resize_bilinear_u8(ibl_engine* e, const uint8_t* x_nhwc, int N, int Hin,
   }
   return launch_resize_bilinear_u8(x_nhwc, N, Hin, Win, Hout, Wout, bounds_h, kk_h, ksize_h, bounds_v, kk_v, ksize_v, tmp,
                                    out_nhwc, S(stream), &e->launches);
+}
+
+// Image.open(f).convert('RGB') of Preprocessor.__getitem__ (ibl/utils/data/preprocessor.py:31-42) for baseline JPEGs,
+// bit-exact with Pillow's libjpeg decode (jpeg.cu).
+int ibl_jpeg_decode_u8(ibl_engine* e, const uint8_t* const* files, const size_t* lens, int N, uint8_t* out_u8,
+                       const uint64_t* out_offsets, int* status, int* err_dev, void* stream) {
+  IBL_REQUIRE(e && files && lens && out_offsets && status && err_dev, "null argument");
+  IBL_REQUIRE(N >= 1, "empty batch");
+  DeviceGuard g(e->device);
+  return jpeg_decode_u8(&e->jpeg_ws, files, lens, N, out_u8, out_offsets, status, err_dev, S(stream), &e->launches);
 }
 
 int ibl_extract_host_u8(ibl_engine* e, const uint8_t* x_nhwc_host, int N, int H, int W, const float* mean3,

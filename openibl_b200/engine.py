@@ -336,6 +336,53 @@ class Engine:
               "ibl_resize_bilinear_u8")
         return out
 
+    @staticmethod
+    def jpeg_parse(data: bytes) -> dict:
+        """Host-only header parse of one in-memory JPEG (no device needed): size, components, sampling, restart
+        layout; `ok` is False with `reason` set for files the device decoder does not take."""
+        return _cabi.jpeg_parse(data)
+
+    def decode_jpeg_async(self, files: Sequence[bytes]):
+        """In-memory JPEG files -> ([device uint8 [H,W,3] or None], device int32 error words [N]).  None marks a file
+        the parser rejected (progressive, CMYK, ...); nothing is synchronised, so a corrupt entropy stream shows
+        only in its error word (nonzero) once the stream has run."""
+        n = len(files)
+        if n == 0:
+            return [], torch.zeros(0, dtype=torch.int32, device=torch.device("cuda", self.device))
+        infos = [_cabi.jpeg_parse(f) for f in files]
+        offsets = (c_uint64 * n)()
+        total = 0
+        for i, inf in enumerate(infos):
+            offsets[i] = total
+            if inf["ok"]:
+                total += inf["height"] * inf["width"] * 3
+        dev = torch.device("cuda", self.device)
+        out = torch.empty(max(total, 1), dtype=torch.uint8, device=dev)
+        err = torch.empty(n, dtype=torch.int32, device=dev)
+        ptrs = (ctypes.c_char_p * n)(*[bytes(f) for f in files])
+        lens = (ctypes.c_size_t * n)(*[len(f) for f in files])
+        status = (c_int * n)()
+        check(self.lib.ibl_jpeg_decode_u8(self.h, ptrs, lens, n, _ptr(out), offsets, status, _ptr(err),
+                                          _stream(self.device)), "ibl_jpeg_decode_u8")
+        imgs = []
+        for i, inf in enumerate(infos):
+            if status[i] != _cabi.IBL_OK:
+                imgs.append(None)
+                continue
+            h, w = inf["height"], inf["width"]
+            imgs.append(out[offsets[i]: offsets[i] + h * w * 3].view(h, w, 3))
+        return imgs, err
+
+    def decode_jpeg(self, files: Sequence[bytes]):
+        """In-memory JPEG files -> list of device uint8 [H,W,3], bit-identical to
+        np.asarray(Image.open(f).convert('RGB')); None for a file the device decoder does not take.  Waits for the
+        stream and raises RuntimeError if an entropy stream is corrupt."""
+        imgs, err = self.decode_jpeg_async(files)
+        bad = torch.nonzero(err).flatten().tolist()
+        if bad:
+            raise RuntimeError(f"corrupt JPEG entropy data in file(s) {bad} of the batch")
+        return imgs
+
     def argsort_rows(self, dist: torch.Tensor) -> torch.Tensor:
         """torch.argsort(dist, dim=1) on the engine's own sort kernels: [m,n] fp32 -> [m,n] int64, ties by index."""
         dist = _require_cuda(dist, "distance matrix")

@@ -20,6 +20,7 @@ import torch
 import torch.distributed as dist
 
 from .engine import Engine
+from .utils.data.gpu_jpeg import check_decode_errors, decode_batch, is_encoded_batch
 from .utils.data.sampler import slice_bounds
 
 __all__ = ["extract_cnn_feature", "extract_features", "pairwise_distance", "spatial_nms",
@@ -41,8 +42,12 @@ def _to_torch(x):
 
 
 def extract_cnn_feature(model, inputs, vlad=True, gpu=None):
-    """evaluators.py:22-34: forward, pick vlad/pooled output, L2 (idempotent for vlad)."""
+    """evaluators.py:22-34: forward, pick vlad/pooled output, L2 (idempotent for vlad).
+    A batch of file bytes (get_transformer_test(..., device_decode=True)) is decoded and transformed on the GPU
+    first (utils/data/gpu_jpeg.py)."""
     model.eval()
+    if is_encoded_batch(inputs):
+        inputs = decode_batch(inputs, device=gpu)
     inputs = _to_torch(inputs).cuda(gpu, non_blocking=True)
     with torch.no_grad():
         outputs = model(inputs)
@@ -61,10 +66,13 @@ def _extract_local(model, data_loader, print_freq=10, vlad=True, pca=None, gpu=N
     if pca is not None:
         pca.load(gpu=gpu)
     feats, names = [], []
+    decode_errors = []                   # device JPEG decode: error words, checked once before returning
     end = time.time()
     bt_sum = 0.0
     with torch.no_grad():
         for i, (imgs, fnames, _, _, _) in enumerate(data_loader):
+            if is_encoded_batch(imgs):   # file bytes: decode on the GPU, corrupt-file check deferred to the end
+                imgs = decode_batch(imgs, device=gpu, pending=decode_errors)
             out = extract_cnn_feature(model, imgs, vlad, gpu=gpu)
             if pca is not None:
                 out = pca.infer(out)
@@ -76,6 +84,7 @@ def _extract_local(model, data_loader, print_freq=10, vlad=True, pca=None, gpu=N
             if (i + 1) % print_freq == 0 and rank == 0:
                 print("Extract Features: [{}/{}]\tTime {:.3f} ({:.3f})".format(
                     i + 1, len(data_loader), bt, bt_sum / (i + 1)))
+    check_decode_errors(decode_errors)
     if feats:
         return torch.cat(feats), names
     return torch.empty(0, 0, device=torch.device("cuda", torch.cuda.current_device() if gpu is None else gpu)), names

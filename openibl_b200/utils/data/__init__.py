@@ -30,7 +30,12 @@ def get_transformer_train(height, width):
                       T.Normalize(mean=_MEAN, std=_STD)])
 
 
-def get_transformer_test(height, width, tokyo=False):
+def get_transformer_test(height, width, tokyo=False, device_decode=False):
+    """device_decode=True: `Preprocessor` yields the file's bytes and `extract_cnn_feature` runs this same transform
+    on the GPU (gpu_jpeg.decode_to_tensor), bit for bit."""
+    if device_decode:
+        from .gpu_jpeg import DeviceDecode
+        return DeviceDecode(height, width, tokyo)
     import torchvision.transforms as T
     return T.Compose([T.Resize(max(height, width) if tokyo else (height, width)), T.ToTensor(),
                       T.Normalize(mean=_MEAN, std=_STD)])

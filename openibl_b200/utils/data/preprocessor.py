@@ -3,6 +3,8 @@ import os.path as osp
 
 from torch.utils.data import Dataset
 
+from .gpu_jpeg import DeviceDecode
+
 
 class Preprocessor(Dataset):
     def __init__(self, dataset, root=None, transform=None):
@@ -21,6 +23,9 @@ class Preprocessor(Dataset):
         from PIL import Image
         fname, pid, x, y = self.dataset[index]
         fpath = fname if self.root is None else osp.join(self.root, fname)
+        if isinstance(self.transform, DeviceDecode):     # decode + transform happen on the GPU (gpu_jpeg.py)
+            with open(fpath, "rb") as f:
+                return self.transform(f.read(), fname), fname, pid, x, y
         img = Image.open(fpath).convert("RGB")
         if self.transform is not None:
             img = self.transform(img)

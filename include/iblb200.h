@@ -320,6 +320,9 @@ int ibl_debug_umma_strided(ibl_engine* e, const void* A, int rows, const void* B
  * patch: view row m is row s0 + ((m%64)/8)*group_rows + (m/64)*half_rows + (m%8)), base_offset 0. */
 int ibl_debug_umma_halo_view(ibl_engine* e, const void* A, int rows, const void* B, int s0, int group_rows,
                              int half_rows, float* D, void* stream);
+/* The fused conv1_1 + ReLU + conv1_2 + ReLU + 2x2 max-pool kernel of the forward alone, weights from the engine
+ * (ibl_engine_set_vgg16): x NCHW [N,3,H,W] fp32, y_hi / y_lo the bf16 hi/lo planes [N,H/2,W/2,64] (device). */
+int ibl_debug_conv1_fused(ibl_engine* e, const float* x, int N, int H, int W, void* y_hi, void* y_lo, void* stream);
 /* Average device time (ms) of one backbone layer over `reps` launches, weights from the engine
  * (tools/bench_layers.py).  layer 0 = the tensor-core conv1_1 (x NCHW [N,3,H,W]); 1..12 = conv1_2..conv5_3
  * (x NHWC [N,H,W,Cin] fp32), where bn_override forces the N tile (64/128) when it divides Cout, 0 = default;

@@ -1299,6 +1299,17 @@ int ibl_debug_umma_halo_view(ibl_engine* e, const void* A, int rows, const void*
   return debug_gmma_strided(A, rows, B, s0, group_rows, half_rows, 0, D, S(stream));
 }
 
+// The fused conv1_1 + ReLU + conv1_2 + ReLU + 2x2 pool kernel alone (test hook), weights from the engine: x NCHW
+// [N,3,H,W] fp32, y_hi / y_lo the bf16 planes [N,H/2,W/2,64] the forward hands to conv2_1.
+int ibl_debug_conv1_fused(ibl_engine* e, const float* x, int N, int H, int W, void* y_hi, void* y_lo, void* stream) {
+  IBL_REQUIRE(e && x && y_hi && y_lo && N >= 1 && H >= 2 && W >= 2, "bad argument");
+  if (!e->vgg_ready) { set_last_error("ibl_engine_set_vgg16 was not called"); return IBL_ERR_NOT_READY; }
+  DeviceGuard g(e->device);
+  e->launches += 1;
+  return launch_conv1_fused_tc(x, e->w0_oihw, e->conv[0].bias, e->conv[1], N, H, W, static_cast<__nv_bfloat16*>(y_hi),
+                               static_cast<__nv_bfloat16*>(y_lo), S(stream));
+}
+
 // Timing hooks (tools/bench_layers.py): average device time of one backbone layer over `reps`
 // back-to-back launches, weights taken from the engine (ibl_engine_set_vgg16).  layer 0 = the tensor-core conv1_1
 // (x is NCHW [N,3,H,W]); layers 1..12 take x NHWC [N,H,W,Cin] fp32 (converted to planes once).

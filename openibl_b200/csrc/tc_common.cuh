@@ -210,6 +210,16 @@ __device__ __forceinline__ uint64_t gmma_desc_kmajor_sw128(uint32_t smem_addr) {
   d |= (uint64_t)1 << 62;                           // layout type: SWIZZLE_128B
   return d;
 }
+// K-major operand, 64-byte swizzle: rows of 64 bytes (32 bf16, a K = 32 operand without padding), 16-byte chunk j of
+// row r stored at chunk position j ^ ((r >> 1) & 3), 8-row atoms 512 bytes apart.  +2 steps 16 elements along K.
+__device__ __forceinline__ uint64_t gmma_desc_kmajor_sw64(uint32_t smem_addr) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr >> 4) & 0x3fffu);
+  d |= (uint64_t)1 << 16;
+  d |= (uint64_t)(512u >> 4) << 32;
+  d |= (uint64_t)2 << 62;                           // layout type: SWIZZLE_64B
+  return d;
+}
 // MN-major operand, 128-byte swizzle: rows (K index) of 64 elements = 128 B, 8-row atoms 1024 B apart (SBO); further
 // 64-element blocks along M/N are `lbo_bytes` apart (LBO).  16 K rows (one k16 step) are 2048 bytes.
 __device__ __forceinline__ uint64_t gmma_desc_mnmajor_sw128(uint32_t smem_addr, uint32_t lbo_bytes) {

@@ -601,17 +601,20 @@ int launch_conv3x3_tc(const __nv_bfloat16* x_hi, const __nv_bfloat16* x_lo, cons
 // conv1_1 + conv1_2 (+ ReLU + 2x2 max-pool) in ONE kernel  (vgg.py:40-42 slots 0 and 2)
 //
 // conv1_1's output -- 64 channels at full resolution, 2.5 GB per batch of 32 as hi/lo planes -- is the largest tensor
-// of the network and would be written to HBM by one kernel only to be read back by the next.  Here a CTA owns a 16 x 8
-// patch of conv1_2 outputs and RECOMPUTES the conv1_1 activations it needs, the (16+2) x (8+2) = 180-pixel halo,
-// straight into the shared-memory halo tile that conv1_2's nine tap views read (the HALO staging above):
+// of the network and would be written to HBM by one kernel only to be read back by the next.  Here a CTA owns 16 x 8
+// patches of conv1_2 outputs and RECOMPUTES the conv1_1 activations each needs, the (16+2) x (8+2) = 180-pixel halo,
+// straight into the shared-memory halo tile that conv1_2's nine tap views read (the HALO staging above).
 //
-//   builders (warps 5-8)   im2col of the 3-channel input for the 180 halo pixels: K = 27 -> 32, bf16 hi/lo, K-major
-//                          SW128 rows (two 128-row M tiles)                                    [as conv1_1_tc_kernel]
-//   consumer (warps 0-3)   C1: 2 M tiles x 2 K steps x 3 wgmma (N = 64) -> bias, ReLU, ZERO outside the image
-//                          (conv1_2's padding), hi/lo -> halo tile;  C2: 9 taps x 4 K steps x 3 wgmma -> bias, ReLU,
-//                          2x2 max-pool, hi/lo planes -> HBM                                   [conv_epilogue_tile]
-//   producer (warp 4)      TMA ring of conv1_2's weight taps (16 KiB each)
-// The builders fill the operand of the next tile while the consumer runs C1/C2 of the current one.
+//   producer (warpgroup 0)     warp 0: TMA ring of conv1_2's weight taps (16 KiB each); the warpgroup's registers go
+//                              to the consumers (setmaxnreg)
+//   consumers (warpgroups 1-2) consumer j takes the CTA's tiles j, j + 2, ... and, per tile:
+//     A1  im2col of the 3-channel input for the 180 halo pixels: K = 27 -> 32, bf16 hi/lo, 64-byte K-major SW64 rows,
+//         192 rows = 3 m64 tiles, built in the consumer's own halo buffer (free until C1's epilogue fills it)
+//     C1  conv1_1: 3 M tiles x 2 K steps x 3 wgmma (N = 64) -> bias, ReLU, ZERO outside the image (conv1_2's padding),
+//         hi/lo straight from the accumulator fragment into the halo tile's swizzled rows
+//     C2  conv1_2: 9 taps x 4 K steps x 3 wgmma (N = 64) over the halo's tap views -> bias, ReLU, 2x2 max-pool, hi/lo
+//         planes -> HBM                                                                       [conv_epilogue_tile]
+// so one consumer's C2 MMAs run while the other does its C2 epilogue, its next tile's A1, C1 and C1 epilogue.
 // =====================================================================================================================
 struct Conv1FusedArgs {
   const float* x;       // [N,3,H,W]
@@ -620,43 +623,49 @@ struct Conv1FusedArgs {
   ConvTcArgs c2;        // conv1_2: N,H,W, cin = cout = 64, tw_log2 = 3, tiles, relu, pool, bias, y_hi / y_lo
 };
 
-constexpr int F1_W1 = 16384;                         // conv1_1 filters: hi 8 KiB | lo 8 KiB
-constexpr int F1_A1_PLANE = 256 * 128;               // 256 halo rows x 128 B (K = 32 uses the first 64 B of a row)
-constexpr int F1_A1 = 2 * F1_A1_PLANE;               // hi | lo
+constexpr int F1_A1_ROWS = 192;                      // the 180 halo pixels in three m64 tiles
+constexpr int F1_A1_PLANE = F1_A1_ROWS * 64;         // 64-byte rows: K = 32
+constexpr int F1_W1_PLANE = 64 * 64;                 // conv1_1 filters: 64 rows x 64 B per plane
 constexpr int F1_W2_STAGE = 2 * 64 * TC_BK * 2;      // one tap of conv1_2: W_hi 8 KiB | W_lo 8 KiB
-constexpr int F1_W2_STAGES = 3;
-constexpr int F1_OFF_A1 = F1_W1;
-constexpr int F1_OFF_HALO = F1_OFF_A1 + F1_A1;       // 80 KiB, 1024-aligned
-constexpr int F1_OFF_W2 = F1_OFF_HALO + TC_HALO_STAGE;
+constexpr int F1_W2_STAGES = 4;
+// [halo 0 | halo 1] [W1 hi | W1 lo] [4 weight taps] [staging 0 | staging 1] [barriers, bias1]
+constexpr int F1_OFF_W1 = 2 * TC_HALO_STAGE;         // 92 KiB
+constexpr int F1_OFF_W2 = F1_OFF_W1 + 2 * F1_W1_PLANE;
 constexpr int F1_OFF_STG = F1_OFF_W2 + F1_W2_STAGES * F1_W2_STAGE;
-constexpr int F1_OFF_BAR = F1_OFF_STG + ACC_STG_BYTES;
+constexpr int F1_OFF_BAR = F1_OFF_STG + 2 * ACC_STG_BYTES;
 constexpr int F1_SMEM = F1_OFF_BAR + 512 + 1024;
+static_assert(2 * F1_A1_PLANE <= TC_HALO_STAGE, "A1 (hi | lo) is built inside the consumer's halo buffer");
+static_assert(TC_HALO_STAGE % 1024 == 0 && F1_OFF_W1 % 512 == 0 && F1_OFF_W2 % 1024 == 0, "swizzle atom alignment");
 static_assert(F1_SMEM <= 232448, "shared-memory budget of the fused conv1 kernel");
 
-__global__ void __launch_bounds__(288, 1)
+// d[0:32] += A . B^T as m64n64k16 (A, B descriptors): the columns 0-63 of an N = 128 fragment d[64] (fused conv1 kernel)
+__device__ __forceinline__ void wgmma_n64_into_n128(float (&d)[64], uint64_t a, uint64_t b) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a), "l"(b));
+}
+
+__global__ void __launch_bounds__(384, 1)
 conv1_fused_tc_kernel(const __grid_constant__ CUtensorMap tm_whi, const __grid_constant__ CUtensorMap tm_wlo,
                       const Conv1FusedArgs fa) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const ConvTcArgs& a = fa.c2;
-  uint8_t* w1_hi = smem;
-  uint8_t* w1_lo = smem + 8192;
-  uint8_t* a1 = smem + F1_OFF_A1;
-  uint8_t* halo = smem + F1_OFF_HALO;
+  uint8_t* w1 = smem + F1_OFF_W1;
   uint8_t* w2 = smem + F1_OFF_W2;
   float* stg = reinterpret_cast<float*>(smem + F1_OFF_STG);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + F1_OFF_BAR);
-  uint64_t* w_full = bars;                 // [3] producer
-  uint64_t* w_empty = bars + 3;            // [3] 4 consumer warps
-  uint64_t* a1_full = bars + 6;            // 4 builder warps
-  uint64_t* a1_empty = bars + 7;           // 4 consumer warps
-  float* bias1_s = reinterpret_cast<float*>(bars + 8);   // [64]
+  uint64_t* w_full = bars;                           // [4] producer
+  uint64_t* w_empty = bars + F1_W2_STAGES;           // [4] 4 warps of the consumer of the tile
+  uint64_t* order_bar = bars + 2 * F1_W2_STAGES;     // [2] 4 warps of the other consumer
+  float* bias1_s = reinterpret_cast<float*>(bars + 16);   // [64]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // one-time: zero A1 (the K >= 32 half of every row stays zero), lay out conv1_1's filters
-  for (int i = threadIdx.x; i < F1_A1 / 16; i += blockDim.x) reinterpret_cast<uint4*>(a1)[i] = make_uint4(0, 0, 0, 0);
-  for (int i = threadIdx.x; i < 64 * 8; i += blockDim.x) {   // (row n, chunk j): 8 k-values each, k = tap*3 + c
-    const int n = i >> 3, j = i & 7;
+  // one-time: conv1_1's filters as K-major SW64 rows, k = tap*3 + c (zero for k >= 27)
+  for (int i = threadIdx.x; i < 64 * 4; i += blockDim.x) {   // (row n, 16-byte chunk j): 8 k-values each
+    const int n = i >> 2, j = i & 3;
     uint32_t hi[4], lo[4];
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
@@ -672,20 +681,20 @@ conv1_fused_tc_kernel(const __grid_constant__ CUtensorMap tm_whi, const __grid_c
       hi[e] = *reinterpret_cast<uint32_t*>(&hh);
       lo[e] = pack_bf16x2(v[0] - __bfloat162float(h0), v[1] - __bfloat162float(h1));
     }
-    const int pos = n * 128 + ((j ^ (n & 7)) * 16);
-    *reinterpret_cast<uint4*>(w1_hi + pos) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-    *reinterpret_cast<uint4*>(w1_lo + pos) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+    const int pos = n * 64 + ((j ^ ((n >> 1) & 3)) * 16);
+    *reinterpret_cast<uint4*>(w1 + pos) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+    *reinterpret_cast<uint4*>(w1 + F1_W1_PLANE + pos) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
   }
   if (threadIdx.x < 64) bias1_s[threadIdx.x] = fa.bias1[threadIdx.x];
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tm_whi);
     tma_prefetch_desc(&tm_wlo);
     for (int i = 0; i < F1_W2_STAGES; ++i) { mbar_init(&w_full[i], 1); mbar_init(&w_empty[i], 4); }
-    mbar_init(a1_full, 4);
-    mbar_init(a1_empty, 4);
+    mbar_init(&order_bar[0], 4);
+    mbar_init(&order_bar[1], 4);
     fence_barrier_init();
   }
-  fence_proxy_async();        // generic-proxy writes of the filters and the zero fill -> visible to the tensor core
+  fence_proxy_async();        // generic-proxy writes of the filters -> visible to the tensor core
   __syncthreads();
   const int tiles_per_img = a.tiles_h * a.tiles_w;
   auto coords = [&](int tile, int& img, int& h0, int& w0) {
@@ -694,9 +703,9 @@ conv1_fused_tc_kernel(const __grid_constant__ CUtensorMap tm_whi, const __grid_c
     h0 = (rem / a.tiles_w) * 16;
     w0 = (rem % a.tiles_w) * 8;
   };
-  const long long HW = (long long)a.H * a.W;
 
-  if (warp == 4) {
+  if (warp < 4) setmaxnreg_dec<40>();
+  if (warp == 0) {
     // ================= TMA producer: conv1_2 weight taps (convergent warp, one elected lane issues) =================
     int stage = 0; uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < a.total_tiles; tile += gridDim.x) {
@@ -712,156 +721,181 @@ conv1_fused_tc_kernel(const __grid_constant__ CUtensorMap tm_whi, const __grid_c
         if (++stage == F1_W2_STAGES) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp < 4) {
-    // ================= consumer warpgroup: C1 -> halo tile, C2 -> conv1_2 epilogue =================
-    const int t = threadIdx.x;
-    const int r = t >> 3, c = t & 7;                  // 8-wide, 16-tall patch
-    const uint64_t b1h = gmma_desc_kmajor_sw128(smem_u32(w1_hi)), b1l = gmma_desc_kmajor_sw128(smem_u32(w1_lo));
+  } else if (warp >= 4) {
+    // ================= two consumer warpgroups (ping-pong): A1 -> C1 -> halo tile, C2 -> conv1_2 epilogue =================
+    setmaxnreg_inc<232>();
+    const int cw = warp / 4 - 1;                      // consumer 0 / 1
+    const int bar = 1 + cw;                           // its named barrier
+    float* my_stg = stg + cw * (ACC_STG_BYTES / 4);
+    uint8_t* halo = smem + cw * TC_HALO_STAGE;        // this consumer's halo tile; A1 hi | lo at its start until C1 retires
+    const int t = threadIdx.x & 127;                  // thread inside the warpgroup
+    const int r = t >> 3, c = t & 7;                  // C2 accumulator row t = pixel (r, c) of the 8-wide, 16-tall patch
+    const uint32_t ha = smem_u32(halo);
+    const uint64_t b1h = gmma_desc_kmajor_sw64(smem_u32(w1)), b1l = gmma_desc_kmajor_sw64(smem_u32(w1) + F1_W1_PLANE);
+    const uint64_t a1h = gmma_desc_kmajor_sw64(ha), a1l = gmma_desc_kmajor_sw64(ha + F1_A1_PLANE);
+    constexpr uint64_t kA1Tile = 64 * 64 / 16;         // the next m64 tile of A1: +4 KiB
     constexpr uint64_t kHaloDesc = ((uint64_t)1 << 16) | ((uint64_t)((TC_HALO_W * 128) >> 4) << 32) | ((uint64_t)1 << 62);
     constexpr uint64_t kHaloHalf = 8 * TC_HALO_W * 128 / 16;   // pixel rows 64-127 of a tap view: groups 8-15
-    const uint32_t ha = smem_u32(halo);
-    int stage = 0; uint32_t phase = 0;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < a.total_tiles; tile += gridDim.x, ++it) {
+    const long long HW = (long long)a.H * a.W;
+    // Consumer cw takes the CTA's tiles cw, cw + 2, ...  The producer fills the weight ring in tile order, so the taps of
+    // CTA-local tile i start at running index 9 i.  The order barrier lets a consumer wait on its first tap only after
+    // the other consumer has waited on all the taps of the tile before: a slot's full barrier is then at most one phase
+    // behind the awaited one, so its parity is exact.
+    for (int i = cw; blockIdx.x + i * gridDim.x < a.total_tiles; i += 2) {
       int img, h0, w0;
-      coords(tile, img, h0, w0);
-      mbar_wait(a1_full, it & 1);
-#pragma unroll 1
-      for (int mt = 0; mt < 2; ++mt) {
-        const uint32_t sa = smem_u32(a1) + mt * 16384;
-        const uint64_t ah = gmma_desc_kmajor_sw128(sa), al = gmma_desc_kmajor_sw128(sa + F1_A1_PLANE);
-        constexpr uint64_t kHalf = 64 * 128 / 16;
-        Acc128<64> c1;
-        wgmma_fence();
+      coords(blockIdx.x + i * gridDim.x, img, h0, w0);
+      // the per-row index math below is recomputed for every tile: hoisted out of the loop it would hold ~20 registers
+      // through the C2 main loop and epilogue
+      int tl = t;
+      asm volatile("" : "+r"(tl));
+      // ---- A1: rows t and t + 128 (halo pixels; rows >= 180 are zero).  The previous tile's C2 has retired: every warp
+      // passed its wgmma_wait<0> before the named barriers of that tile's epilogue.
 #pragma unroll
-        for (int k = 0; k < 2; ++k) {                   // K = 32: two 16-wide steps
-          const uint64_t ko = (uint64_t)(k * 2);
-          c1.mma(al + ko, al + kHalf + ko, b1h + ko, k > 0 ? 1u : 0u);
-          c1.mma(ah + ko, ah + kHalf + ko, b1l + ko, 1u);
-          c1.mma(ah + ko, ah + kHalf + ko, b1h + ko, 1u);
+      for (int q = 0; q < 2; ++q) {
+        const int p = q * 128 + tl;
+        if (p < F1_A1_ROWS) {
+          float v[32];
+#pragma unroll
+          for (int k = 0; k < 32; ++k) v[k] = 0.f;
+          const int hl = p / TC_HALO_W, wl = p - hl * TC_HALO_W;
+          const int ph = h0 - 1 + hl, pw = w0 - 1 + wl;
+          if (p < TC_HALO_ROWS && ph >= 0 && ph < a.H && pw >= 0 && pw < a.W && img < a.N) {
+            const float* xb = fa.x + (long long)img * 3 * HW;
+#pragma unroll
+            for (int tap = 0; tap < 9; ++tap) {
+              const int ih = ph + tap / 3 - 1, iw = pw + tap % 3 - 1;
+              if (ih >= 0 && ih < a.H && iw >= 0 && iw < a.W) {
+                const long long o = (long long)ih * a.W + iw;
+#pragma unroll
+                for (int ci = 0; ci < 3; ++ci) v[tap * 3 + ci] = __ldg(xb + ci * HW + o);
+              }
+            }
+          }
+          uint8_t* rh = halo + p * 64;
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            uint32_t hi[4], lo[4];
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+              const float x0 = v[8 * j + 2 * e], x1 = v[8 * j + 2 * e + 1];
+              const __nv_bfloat16 h0b = __float2bfloat16_rn(x0), h1b = __float2bfloat16_rn(x1);
+              __nv_bfloat162 hv(h0b, h1b);
+              hi[e] = *reinterpret_cast<uint32_t*>(&hv);
+              lo[e] = pack_bf16x2(x0 - __bfloat162float(h0b), x1 - __bfloat162float(h1b));
+            }
+            const int pos = (j ^ ((p >> 1) & 3)) * 16;
+            *reinterpret_cast<uint4*>(rh + pos) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+            *reinterpret_cast<uint4*>(rh + F1_A1_PLANE + pos) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+          }
         }
-        wgmma_commit();
-        wgmma_wait<0>();
-        c1.fence_operands();
-        if (mt == 1 && lane == 0) mbar_arrive(a1_empty);   // the builders may refill A1
-        // epilogue 1: bias, ReLU, image mask, hi/lo -> halo row p (the previous tile's C2 has retired)
-        const int p = mt * 128 + t;
-        const int hl = p / TC_HALO_W, wl = p - hl * TC_HALO_W;
-        const int ph = h0 - 1 + hl, pw = w0 - 1 + wl;
-        const bool inside = p < TC_HALO_W * TC_HALO_H && ph >= 0 && ph < a.H && pw >= 0 && pw < a.W && img < a.N;
+      }
+      fence_proxy_async();                             // generic-proxy writes of A1 -> visible to the tensor core
+      wg_sync(bar);
+      // ---- C1: conv1_1 on the 192 A1 rows
+      float c1[3][32];
+      wgmma_fence();
 #pragma unroll
-        for (int ch = 0; ch < 2; ++ch) {
-          uint32_t raw[32];
-          c1.rows32(ch, stg, raw);
-          if (p < TC_HALO_W * TC_HALO_H) {
-            uint32_t hi[16], lo[16];
+      for (int k = 0; k < 2; ++k) {                    // K = 32: two 16-wide steps
+        const uint64_t ko = (uint64_t)(k * 2);
 #pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              float x0 = fmaxf(__uint_as_float(raw[2 * j]) + bias1_s[ch * 32 + 2 * j], 0.f);
-              float x1 = fmaxf(__uint_as_float(raw[2 * j + 1]) + bias1_s[ch * 32 + 2 * j + 1], 0.f);
+        for (int f = 0; f < 3; ++f) {
+          const uint64_t fo = f * kA1Tile + ko;
+          Wgmma<64, false, 0, 0>::mma(c1[f], a1l + fo, b1h + ko, k > 0 ? 1u : 0u);
+          Wgmma<64, false, 0, 0>::mma(c1[f], a1h + fo, b1l + ko, 1u);
+          Wgmma<64, false, 0, 0>::mma(c1[f], a1h + fo, b1h + ko, 1u);
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+#pragma unroll
+      for (int f = 0; f < 3; ++f)
+#pragma unroll
+        for (int j = 0; j < 32; ++j) asm volatile("" : "+f"(c1[f][j])::"memory");
+      wg_sync(bar);                                    // no warp reads A1 any more: the halo rows may overwrite it
+      // ---- C1 epilogue: bias, ReLU, image mask, hi/lo -> halo row p, from the fragment.  Thread 32 w + l holds
+      // rows 16 w + l/4 (+ 8) of each m64 tile, channel pairs 8 j + 2 (l % 4): one 4-byte store per plane and pair,
+      // eight distinct rows x four lanes per 16-byte chunk position -> conflict-free.
+#pragma unroll
+      for (int f = 0; f < 3; ++f) {
+#pragma unroll
+        for (int hf = 0; hf < 2; ++hf) {
+          const int p = 64 * f + (tl & ~31) / 2 + ((tl & 31) >> 2) + 8 * hf;
+          if (p < TC_HALO_ROWS) {
+            const int hl = p / TC_HALO_W, wl = p - hl * TC_HALO_W;
+            const int ph = h0 - 1 + hl, pw = w0 - 1 + wl;
+            const bool inside = ph >= 0 && ph < a.H && pw >= 0 && pw < a.W && img < a.N;
+            uint8_t* rh = halo + p * 128 + (tl & 3) * 4;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+              const int ch = 8 * j + 2 * (tl & 3);
+              float x0 = fmaxf(c1[f][4 * j + 2 * hf] + bias1_s[ch], 0.f);
+              float x1 = fmaxf(c1[f][4 * j + 2 * hf + 1] + bias1_s[ch + 1], 0.f);
               if (!inside) { x0 = 0.f; x1 = 0.f; }       // conv1_2 pads its INPUT with zeros
               const __nv_bfloat16 h0b = __float2bfloat16_rn(x0), h1b = __float2bfloat16_rn(x1);
               __nv_bfloat162 hv(h0b, h1b);
-              hi[j] = *reinterpret_cast<uint32_t*>(&hv);
-              lo[j] = pack_bf16x2(x0 - __bfloat162float(h0b), x1 - __bfloat162float(h1b));
-            }
-            uint8_t* rh = halo + p * 128;
-            uint8_t* rl = rh + TC_HALO_PLANE;
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const int pos = ((ch * 4 + j) ^ (p & 7)) * 16;
-              *reinterpret_cast<uint4*>(rh + pos) = make_uint4(hi[4 * j], hi[4 * j + 1], hi[4 * j + 2], hi[4 * j + 3]);
-              *reinterpret_cast<uint4*>(rl + pos) = make_uint4(lo[4 * j], lo[4 * j + 1], lo[4 * j + 2], lo[4 * j + 3]);
+              const int pos = (j ^ (p & 7)) * 16;
+              *reinterpret_cast<uint32_t*>(rh + pos) = *reinterpret_cast<uint32_t*>(&hv);
+              *reinterpret_cast<uint32_t*>(rh + TC_HALO_PLANE + pos) =
+                  pack_bf16x2(x0 - __bfloat162float(h0b), x1 - __bfloat162float(h1b));
             }
           }
         }
       }
-      fence_proxy_async();                               // generic-proxy writes of the halo -> visible to the tensor core
-      wg_sync();                                         // every halo row is written
-      // C2: conv1_2 over the nine tap views of the halo tile
-      Acc128<64> acc;
+      fence_proxy_async();                             // generic-proxy writes of the halo -> visible to the tensor core
+      wg_sync(bar);                                    // every halo row is written
+      // ---- C2: conv1_2 over the nine tap views of the halo tile
+      int stage = (i * 9) % F1_W2_STAGES;
+      uint32_t phase = (uint32_t)((i * 9) / F1_W2_STAGES) & 1u;
+      if (i > 0) mbar_wait(&order_bar[cw], (uint32_t)((i - 1) >> 1) & 1u);
+      // A tap's weight stage is W_hi (64 rows) then W_lo (64 rows): one K-major N = 128 operand.  Per k16 step and m64
+      // half, A_hi . [W_hi; W_lo] is one m64n128k16 (A_hi W_hi in columns 0-63, A_hi W_lo in 64-127) and A_lo . W_hi one
+      // m64n64k16 into the first 32 registers of the same fragment (columns 0-63): 10 KiB of shared-memory operands
+      // instead of 12 KiB for the three N = 64 products.  The epilogue adds the two column halves.
+      float d[2][64];
+#pragma unroll
+      for (int hm = 0; hm < 2; ++hm)
+#pragma unroll
+        for (int j = 0; j < 64; ++j) d[hm][j] = 0.f;   // the first MMA ignores it, but its live range starts here, not before C1
       int prev = -1;
       for (int tap = 0; tap < 9; ++tap) {
         mbar_wait(&w_full[stage], phase);
         const uint32_t toff = (uint32_t)((tap / 3) * TC_HALO_W + tap % 3) * 128u;
         const uint64_t a_hi = kHaloDesc | (uint64_t)(((ha + toff) >> 4) & 0x3fffu);
         const uint64_t a_lo = kHaloDesc | (uint64_t)(((ha + TC_HALO_PLANE + toff) >> 4) & 0x3fffu);
-        const uint32_t sb = smem_u32(w2 + stage * F1_W2_STAGE);
-        const uint64_t b_hi = gmma_desc_kmajor_sw128(sb), b_lo = gmma_desc_kmajor_sw128(sb + F1_W2_STAGE / 2);
+        const uint64_t b_w = gmma_desc_kmajor_sw128(smem_u32(w2 + stage * F1_W2_STAGE));
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < TC_BK / 16; ++k) {
           const uint64_t ko = (uint64_t)(k * 2);
-          acc.mma(a_lo + ko, a_lo + kHaloHalf + ko, b_hi + ko, (tap > 0 || k > 0) ? 1u : 0u);
-          acc.mma(a_hi + ko, a_hi + kHaloHalf + ko, b_lo + ko, 1u);
-          acc.mma(a_hi + ko, a_hi + kHaloHalf + ko, b_hi + ko, 1u);
+#pragma unroll
+          for (int hm = 0; hm < 2; ++hm) {
+            const uint64_t ho = hm ? kHaloHalf : 0;
+            Wgmma<128, false, 0, 0>::mma(d[hm], a_hi + ho + ko, b_w + ko, (tap > 0 || k > 0) ? 1u : 0u);
+            wgmma_n64_into_n128(d[hm], a_lo + ho + ko, b_w + ko);
+          }
         }
         wgmma_commit();
+        if (tap == 8 && lane == 0) mbar_arrive(&order_bar[cw ^ 1]);
         wgmma_wait<1>();
         if (prev >= 0 && lane == 0) mbar_arrive(&w_empty[prev]);
         prev = stage;
         if (++stage == F1_W2_STAGES) { stage = 0; phase ^= 1; }
       }
       wgmma_wait<0>();
-      acc.fence_operands();
+#pragma unroll
+      for (int hm = 0; hm < 2; ++hm)
+#pragma unroll
+        for (int j = 0; j < 64; ++j) asm volatile("" : "+f"(d[hm][j])::"memory");
       if (lane == 0) mbar_arrive(&w_empty[prev]);
-      conv_epilogue_tile<64>(a, acc, stg, img, h0, w0, 0, 0, r, c, 8);
-    }
-  } else {
-    // ================= builders: im2col rows of conv1_1 for the 180 halo pixels =================
-    const int bw = warp - 5;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < a.total_tiles; tile += gridDim.x, ++it) {
-      int img, h0, w0;
-      coords(tile, img, h0, w0);
-      float v[2][32];
+      Acc128<64> acc;
 #pragma unroll
-      for (int mt = 0; mt < 2; ++mt) {
+      for (int hm = 0; hm < 2; ++hm)
 #pragma unroll
-        for (int k = 0; k < 32; ++k) v[mt][k] = 0.f;
-        const int p = mt * 128 + bw * 32 + lane;
-        const int hl = p / TC_HALO_W, wl = p - hl * TC_HALO_W;
-        const int ph = h0 - 1 + hl, pw = w0 - 1 + wl;
-        if (p < TC_HALO_W * TC_HALO_H && ph >= 0 && ph < a.H && pw >= 0 && pw < a.W && img < a.N) {
-          const float* xb = fa.x + (long long)img * 3 * HW;
-#pragma unroll
-          for (int tap = 0; tap < 9; ++tap) {
-            const int ih = ph + tap / 3 - 1, iw = pw + tap % 3 - 1;
-            if (ih >= 0 && ih < a.H && iw >= 0 && iw < a.W) {
-              const long long o = (long long)ih * a.W + iw;
-#pragma unroll
-              for (int c = 0; c < 3; ++c) v[mt][tap * 3 + c] = __ldg(xb + c * HW + o);
-            }
-          }
-        }
-      }
-      mbar_wait(a1_empty, (it & 1) ^ 1);                // C1 of the previous tile has consumed A1
-#pragma unroll
-      for (int mt = 0; mt < 2; ++mt) {
-        const int p = mt * 128 + bw * 32 + lane;
-        uint8_t* rh = a1 + p * 128;
-        uint8_t* rl = rh + F1_A1_PLANE;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          uint32_t hi[4], lo[4];
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const float x0 = v[mt][8 * j + 2 * e], x1 = v[mt][8 * j + 2 * e + 1];
-            const __nv_bfloat16 h0b = __float2bfloat16_rn(x0), h1b = __float2bfloat16_rn(x1);
-            __nv_bfloat162 hv(h0b, h1b);
-            hi[e] = *reinterpret_cast<uint32_t*>(&hv);
-            lo[e] = pack_bf16x2(x0 - __bfloat162float(h0b), x1 - __bfloat162float(h1b));
-          }
-          const int pos = (j ^ (p & 7)) * 16;
-          *reinterpret_cast<uint4*>(rh + pos) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-          *reinterpret_cast<uint4*>(rl + pos) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-        }
-      }
-      fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(a1_full);
+        for (int j = 0; j < 32; ++j) acc.h[hm][j] = d[hm][j] + d[hm][32 + j];
+      conv_epilogue_tile<64>(a, acc, my_stg, img, h0, w0, 0, 0, r, c, 8, bar);
     }
   }
+  __syncthreads();
 }
 
 // x [N,3,H,W] fp32 -> conv1_1 -> ReLU -> conv1_2 -> ReLU -> 2x2 max-pool as hi/lo planes [N,H/2,W/2,64]
@@ -894,7 +928,7 @@ int launch_conv1_fused_tc(const float* x_nchw, const float* w1_oihw, const float
   }
   const int sms = device_sm_count();
   const int grid = a.total_tiles < sms ? a.total_tiles : sms;
-  conv1_fused_tc_kernel<<<grid, 288, F1_SMEM, s>>>(m_whi, m_wlo, fa);
+  conv1_fused_tc_kernel<<<grid, 384, F1_SMEM, s>>>(m_whi, m_wlo, fa);
   IBL_CUDA_OK(cudaGetLastError());
   return IBL_OK;
 }

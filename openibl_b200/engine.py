@@ -638,3 +638,16 @@ class Engine:
                                          int(pool), int(mode), int(bn), _ptr(y), _stream(self.device)),
               "ibl_debug_conv3x3")
         return y
+
+    def debug_conv1_fused(self, x_nchw):
+        """The fused conv1_1 + ReLU + conv1_2 + ReLU + 2x2 max-pool kernel alone on the engine's weights: the bf16
+        hi / lo planes [N, H/2, W/2, 64] it hands to conv2_1."""
+        x = _require_cuda(x_nchw, "x")
+        N, C, H, W = x.shape
+        if C != 3:
+            raise ValueError(f"conv1 input must have 3 channels, got {C}")
+        hi = torch.empty(N, H // 2, W // 2, 64, dtype=torch.bfloat16, device=x.device)
+        lo = torch.empty_like(hi)
+        check(self.lib.ibl_debug_conv1_fused(self.h, _ptr(x), N, H, W, _ptr(hi), _ptr(lo), _stream(self.device)),
+              "ibl_debug_conv1_fused")
+        return hi, lo

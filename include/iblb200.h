@@ -213,6 +213,26 @@ int ibl_jpeg_parse(const uint8_t* data, size_t len, ibl_jpeg_info* out);
 int ibl_jpeg_decode_u8(ibl_engine* e, const uint8_t* const* files, const size_t* lens, int N, uint8_t* out_u8,
                        const uint64_t* out_offsets, int* status, int* err_dev, void* stream);
 
+/* ---- input side: the training transform's colour jitter on the GPU ------------ */
+/* T.ColorJitter(0.7, 0.7, 0.7, 0.5), the first step of the reference's training transform
+ * (ibl/utils/data/__init__.py:29-35), bit-identical to torchvision's PIL path: ColorJitter.forward applies, in the
+ * drawn order, F.adjust_brightness / adjust_contrast / adjust_saturation (Pillow's ImageEnhance.Brightness / Contrast /
+ * Color, i.e. Image.blend with a black, mean-of-L or L degenerate image) and F.adjust_hue (Image.convert('HSV'), hue
+ * shifted by uint8(int32(hue * 255)), convert('RGB')).  `order` is ColorJitter.get_params' fn_idx; a NaN factor is one
+ * that get_params returned as None, and its step is skipped.  Brightness, contrast and saturation factors must be
+ * >= 0, hue in [-0.5, 0.5]. */
+typedef struct ibl_color_jitter_params {
+  int order[4];                                   /* permutation of 0 brightness, 1 contrast, 2 saturation, 3 hue */
+  float brightness, contrast, saturation, hue;
+} ibl_color_jitter_params;
+/* Jitters N uint8 HWC RGB images in place: image i is H[i]*W[i]*3 bytes at buf + out_offsets[i] (device buffer, HOST
+ * offsets, sizes and params; the layout ibl_jpeg_decode_u8 writes).  One H2D copy of the per-image descriptors, then
+ * at most two kernels on `stream` whatever the sizes (the steps before contrast, which also sum each image's L; then
+ * contrast with that mean and the remaining steps); no host synchronisation.  Calls may come from different streams:
+ * each call's descriptor copy is ordered on the device after the previous call's kernels. */
+int ibl_color_jitter_u8(ibl_engine* e, uint8_t* buf, const uint64_t* out_offsets, const int* H, const int* W,
+                        const ibl_color_jitter_params* params, int N, void* stream);
+
 /* ---- stage (iii-b): distance + ranking ------------------------------------- */
 /* pairwise_distance(features) with query = gallery = None (evaluators.py:106-114):
  * out[i,j] = 2|x_i|^2 - 2 x_i.x_j, x [n,d], out [n,n]. */

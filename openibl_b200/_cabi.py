@@ -27,6 +27,12 @@ class JpegInfo(Structure):
                 ("reason", c_char * 120)]
 
 
+class ColorJitterParams(Structure):
+    """ibl_color_jitter_params (include/iblb200.h)."""
+    _fields_ = [("order", c_int * 4), ("brightness", c_float), ("contrast", c_float), ("saturation", c_float),
+                ("hue", c_float)]
+
+
 # name -> (restype, argtypes); mirrors include/iblb200.h one to one
 SIGNATURES = {
     "ibl_abi_version": (c_int, []),
@@ -61,6 +67,7 @@ SIGNATURES = {
     "ibl_extract_host_u8": (c_int, [_P, _P, c_int, c_int, c_int, _P, _P, c_uint, _P, _P, _P]),
     "ibl_jpeg_parse": (c_int, [c_char_p, c_size_t, POINTER(JpegInfo)]),
     "ibl_jpeg_decode_u8": (c_int, [_P, _P, _P, c_int, _P, _P, _P, _P, _P]),
+    "ibl_color_jitter_u8": (c_int, [_P, _P, _P, _P, _P, POINTER(ColorJitterParams), c_int, _P]),
     "ibl_l2dist_dense": (c_int, [_P, _P, c_int, _P, c_int, c_int, _P, _P]),
     "ibl_l2dist_self": (c_int, [_P, _P, c_int, c_int, _P, _P]),
     "ibl_l2dist_topk": (c_int, [_P, _P, c_int, _P, c_int, c_int, c_int, c_int, c_int64, _P, _P, _P]),

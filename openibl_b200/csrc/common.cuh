@@ -115,6 +115,11 @@ struct JpegWs;   // opaque per-engine workspace: pinned staging blob, device tab
 void jpeg_ws_destroy(JpegWs* ws);
 int jpeg_decode_u8(JpegWs** ws, const uint8_t* const* files, const size_t* lens, int N, uint8_t* out_u8,
                    const uint64_t* out_offsets, int* status, int* err_dev, cudaStream_t s, uint64_t* launches);
+// color_jitter.cu  (T.ColorJitter, bit-exact with torchvision's PIL path)
+struct JitterWs;   // opaque per-engine workspace: pinned staging of descriptors, device copy, L sums
+void jitter_ws_destroy(JitterWs* ws);
+int color_jitter_u8(JitterWs** ws, uint8_t* buf, const uint64_t* out_offsets, const int* H, const int* W,
+                    const ibl_color_jitter_params* params, int N, cudaStream_t s, uint64_t* launches);
 // tc_conv_bwd.cu  (dgrad filter re-layout, wgmma wgrad, ReLU mask, pool backward, conv1_1 wgrad)
 int launch_repack_weights_dgrad(const float* w_tck, int cout, int cin, __nv_bfloat16* w_hi, __nv_bfloat16* w_lo,
                                 cudaStream_t s);

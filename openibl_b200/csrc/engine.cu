@@ -85,6 +85,7 @@ struct ibl_engine {
   DevBuf knn_ws;                         // neighbour pass of the re-ranking (rerank.cu)
   const int* knn_flag_counter = nullptr; // its count of rows sent to the exact scan (null: no call yet)
   JpegWs* jpeg_ws = nullptr;             // JPEG decode: pinned staging blob, tables, coefficients, planes (jpeg.cu)
+  JitterWs* jitter_ws = nullptr;         // colour jitter: pinned staging of per-image descriptors, L sums (color_jitter.cu)
   RerankWs* rr_ws = nullptr;             // sparse stage of the re-ranking: CSR matrices, inverted index, pair buffers
   const int* flag_counter = nullptr;     // guard counter of the last ibl_l2dist_topk call (null: no guard on its path)
   int dist_path = -1;                    // ranking path of the last ibl_l2dist_topk call (ibl_debug_dist_path)
@@ -279,6 +280,7 @@ int ibl_engine_destroy(ibl_engine* e) {
   e->knn_ws.release();
   rerank_ws_destroy(e->rr_ws);
   jpeg_ws_destroy(e->jpeg_ws);
+  jitter_ws_destroy(e->jitter_ws);
   delete e;
   return IBL_OK;
 }
@@ -810,6 +812,16 @@ int ibl_jpeg_decode_u8(ibl_engine* e, const uint8_t* const* files, const size_t*
   IBL_REQUIRE(N >= 1, "empty batch");
   DeviceGuard g(e->device);
   return jpeg_decode_u8(&e->jpeg_ws, files, lens, N, out_u8, out_offsets, status, err_dev, S(stream), &e->launches);
+}
+
+// T.ColorJitter of the reference's training transform (ibl/utils/data/__init__.py:29-35) on decoded uint8 HWC images,
+// in place, bit-exact with torchvision's PIL path (color_jitter.cu).
+int ibl_color_jitter_u8(ibl_engine* e, uint8_t* buf, const uint64_t* out_offsets, const int* H, const int* W,
+                        const ibl_color_jitter_params* params, int N, void* stream) {
+  IBL_REQUIRE(e && buf && out_offsets && H && W && params, "null argument");
+  IBL_REQUIRE(N >= 1, "empty batch");
+  DeviceGuard g(e->device);
+  return color_jitter_u8(&e->jitter_ws, buf, out_offsets, H, W, params, N, S(stream), &e->launches);
 }
 
 int ibl_extract_host_u8(ibl_engine* e, const uint8_t* x_nhwc_host, int N, int H, int W, const float* mean3,

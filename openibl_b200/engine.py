@@ -342,20 +342,26 @@ class Engine:
         layout; `ok` is False with `reason` set for files the device decoder does not take."""
         return _cabi.jpeg_parse(data)
 
-    def decode_jpeg_async(self, files: Sequence[bytes]):
+    def decode_jpeg_async(self, files: Sequence[bytes], fallback=None):
         """In-memory JPEG files -> ([device uint8 [H,W,3] or None], device int32 error words [N]).  None marks a file
         the parser rejected (progressive, CMYK, ...); nothing is synchronised, so a corrupt entropy stream shows
-        only in its error word (nonzero) once the stream has run."""
+        only in its error word (nonzero) once the stream has run.
+
+        With `fallback` (bytes -> host uint8 [H,W,3] array), rejected files are decoded by it instead and copied into
+        the same device buffer, so every returned image is a view into one allocation (what color_jitter_u8 takes)."""
         n = len(files)
         if n == 0:
             return [], torch.zeros(0, dtype=torch.int32, device=torch.device("cuda", self.device))
         infos = [_cabi.jpeg_parse(f) for f in files]
+        host = {i: fallback(f) for i, (f, inf) in enumerate(zip(files, infos)) if fallback and not inf["ok"]}
         offsets = (c_uint64 * n)()
         total = 0
         for i, inf in enumerate(infos):
             offsets[i] = total
             if inf["ok"]:
                 total += inf["height"] * inf["width"] * 3
+            elif i in host:
+                total += host[i].size
         dev = torch.device("cuda", self.device)
         out = torch.empty(max(total, 1), dtype=torch.uint8, device=dev)
         err = torch.empty(n, dtype=torch.int32, device=dev)
@@ -366,11 +372,15 @@ class Engine:
                                           _stream(self.device)), "ibl_jpeg_decode_u8")
         imgs = []
         for i, inf in enumerate(infos):
-            if status[i] != _cabi.IBL_OK:
+            if i in host:
+                im = out[offsets[i]: offsets[i] + host[i].size].view(host[i].shape)
+                im.copy_(torch.from_numpy(host[i]))
+                imgs.append(im)
+            elif status[i] != _cabi.IBL_OK:
                 imgs.append(None)
-                continue
-            h, w = inf["height"], inf["width"]
-            imgs.append(out[offsets[i]: offsets[i] + h * w * 3].view(h, w, 3))
+            else:
+                h, w = inf["height"], inf["width"]
+                imgs.append(out[offsets[i]: offsets[i] + h * w * 3].view(h, w, 3))
         return imgs, err
 
     def decode_jpeg(self, files: Sequence[bytes]):
@@ -382,6 +392,47 @@ class Engine:
         if bad:
             raise RuntimeError(f"corrupt JPEG entropy data in file(s) {bad} of the batch")
         return imgs
+
+    def color_jitter_u8(self, images: Sequence[torch.Tensor], params: Sequence) -> None:
+        """T.ColorJitter on device uint8 [H,W,3] images, in place, bit-identical to torchvision on the PIL images.
+
+        params[i] is (order, brightness, contrast, saturation, hue) as ColorJitter.get_params returns them; a factor
+        of None skips its step.  Factors cross the C ABI as fp32, which is what get_params draws (and what Pillow's
+        blend takes).  Like the C ABI, the images must be non-overlapping views into one device buffer on this
+        engine's device, as decode_jpeg_async returns them; the batch is one call of at most two launches."""
+        n = len(images)
+        if n != len(params):
+            raise ValueError(f"{n} images but {len(params)} parameter sets")
+        if n == 0:
+            return
+        ims = []
+        for i, im in enumerate(images):
+            _require_cuda(im, f"images[{i}]", dtype=torch.uint8)
+            if im.dim() != 3 or im.shape[2] != 3 or not im.is_contiguous() or im.numel() == 0:
+                raise ValueError(f"images[{i}] must be a non-empty contiguous uint8 [H,W,3] tensor, got {tuple(im.shape)}")
+            ims.append(im)
+        nan = float("nan")
+        p = (_cabi.ColorJitterParams * n)()
+        for i, (order, b, c, s, h) in enumerate(params):
+            p[i].order[:] = [int(k) for k in order]
+            p[i].brightness, p[i].contrast, p[i].saturation, p[i].hue = [nan if v is None else float(v)
+                                                                          for v in (b, c, s, h)]
+        if any(im.device.index != self.device for im in ims):
+            raise ValueError(f"images must be on cuda:{self.device}, the engine's device")
+        base = ims[0].untyped_storage().data_ptr()
+        if any(im.untyped_storage().data_ptr() != base for im in ims):
+            raise ValueError("images must be views into one device buffer (decode_jpeg_async(..., fallback=...))")
+        sizes = [im.numel() for im in ims]
+        offs = [im.data_ptr() - base for im in ims]
+        spans = sorted(zip(offs, sizes))
+        if any(o0 + s0 > o1 for (o0, s0), (o1, _) in zip(spans, spans[1:])):
+            raise ValueError("images overlap in memory")
+        buf = c_void_p(base)
+        off_a = (c_uint64 * n)(*offs)
+        h_a = (c_int * n)(*[im.shape[0] for im in ims])
+        w_a = (c_int * n)(*[im.shape[1] for im in ims])
+        check(self.lib.ibl_color_jitter_u8(self.h, buf, off_a, h_a, w_a, p, n, _stream(self.device)),
+              "ibl_color_jitter_u8")
 
     def argsort_rows(self, dist: torch.Tensor) -> torch.Tensor:
         """torch.argsort(dist, dim=1) on the engine's own sort kernels: [m,n] fp32 -> [m,n] int64, ties by index."""

@@ -17,6 +17,7 @@ import time
 import torch
 import torch.nn.functional as F
 
+from .utils.data.gpu_jpeg import decode_tuples, is_encoded_batch
 from .utils.meters import AverageMeter
 
 
@@ -60,7 +61,10 @@ class Trainer(object):
                     losses.val, losses.avg))
 
     def _parse_data(self, inputs):
-        """trainers.py:64-68: the collated tuple positions -> [B, N, C, H, W] on the device."""
+        """trainers.py:64-68: the collated tuple positions -> [B, N, C, H, W] on the device (file bytes from a
+        `get_transformer_train(..., device_decode=True)` loader are decoded and transformed there)."""
+        if is_encoded_batch(inputs[0][0]):
+            return decode_tuples(inputs, self.gpu)
         imgs = torch.stack([item[0] for item in inputs]).permute(1, 0, 2, 3, 4)
         return imgs.cuda(self.gpu)
 
@@ -123,7 +127,10 @@ class SFRSTrainer(object):
 
     def _parse_data(self, inputs):
         """trainers.py:228-233: tuple = (anchor, positive, neg_num negatives, difficult positives...)."""
-        imgs = torch.stack([item[0] for item in inputs]).permute(1, 0, 2, 3, 4)
+        if is_encoded_batch(inputs[0][0]):
+            imgs = decode_tuples(inputs, self.gpu)
+        else:
+            imgs = torch.stack([item[0] for item in inputs]).permute(1, 0, 2, 3, 4)
         easy = imgs[:, : self.neg_num + 2]
         diff = torch.cat((imgs[:, :1], imgs[:, self.neg_num + 2:]), dim=1)
         return easy.cuda(self.gpu), diff.cuda(self.gpu)

@@ -24,10 +24,15 @@ class IterLoader:
             return next(self.iter)
 
 
-def get_transformer_train(height, width):
+def get_transformer_train(height, width, device_decode=False):
+    """device_decode=True: `Preprocessor` yields the file's bytes with the ColorJitter parameters drawn for it, and the
+    trainers' `_parse_data` runs this same transform on the GPU (gpu_jpeg.decode_tuples), bit for bit."""
     import torchvision.transforms as T
-    return T.Compose([T.ColorJitter(0.7, 0.7, 0.7, 0.5), T.Resize((height, width)), T.ToTensor(),
-                      T.Normalize(mean=_MEAN, std=_STD)])
+    jitter = T.ColorJitter(0.7, 0.7, 0.7, 0.5)
+    if device_decode:
+        from .gpu_jpeg import DeviceJitterDecode
+        return DeviceJitterDecode(height, width, jitter)
+    return T.Compose([jitter, T.Resize((height, width)), T.ToTensor(), T.Normalize(mean=_MEAN, std=_STD)])
 
 
 def get_transformer_test(height, width, tokyo=False, device_decode=False):

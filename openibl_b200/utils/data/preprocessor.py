@@ -23,7 +23,7 @@ class Preprocessor(Dataset):
         from PIL import Image
         fname, pid, x, y = self.dataset[index]
         fpath = fname if self.root is None else osp.join(self.root, fname)
-        if isinstance(self.transform, DeviceDecode):     # decode + transform happen on the GPU (gpu_jpeg.py)
+        if isinstance(self.transform, DeviceDecode):     # decode + transform (+ jitter) happen on the GPU (gpu_jpeg.py)
             with open(fpath, "rb") as f:
                 return self.transform(f.read(), fname), fname, pid, x, y
         img = Image.open(fpath).convert("RGB")

@@ -79,7 +79,8 @@ int ibl_engine_launch_count(ibl_engine* e, uint64_t* count);
 int ibl_engine_set_vgg16(ibl_engine* e, const float* const* weights13,
                          const float* const* biases13, void* stream);
 /* NetVLAD parameters: conv_w [K,C] (net_vlad.conv.weight squeezed), centroids [K,C]
- * (netvlad.py:28-29). */
+ * (netvlad.py:28-29).  1 <= K <= 64: IBL_ERR_BAD_ARG for K < 1, IBL_ERR_UNSUPPORTED for K > 64.
+ * The tensor-core path pads K < 64 to 64 clusters (same cost as K = 64). */
 int ibl_engine_set_netvlad(ibl_engine* e, const float* conv_w, const float* centroids,
                            int K, int C, void* stream);
 /* PCA-whitening layer: W [P,D] (pca_layer.weight squeezed == PCA.load weight,
@@ -116,7 +117,8 @@ int ibl_vgg16_layer_backward(ibl_engine* e, int layer, const float* x, const flo
 
 /* ---- stage (ii): NetVLAD --------------------------------------------------- */
 /* NetVLAD.forward (netvlad.py:44-61) + EmbedNet normalisation (netvlad.py:78-80), fused.
- * feat is [N,S,C] if nhwc != 0 else [N,C,S].  conv_w/centroids [K,C] are read directly.
+ * feat is [N,S,C] if nhwc != 0 else [N,C,S].  conv_w/centroids [K,C] are read directly;
+ * 1 <= K <= 64 (IBL_ERR_BAD_ARG for K < 1, IBL_ERR_UNSUPPORTED for K > 64).
  * vlad_raw [N,K,C] (un-normalised, what NetVLAD.forward returns; may be NULL)
  * vlad_norm [N,K*C] (intra-norm + flatten + L2; may be NULL). */
 int ibl_netvlad_forward(ibl_engine* e, const float* feat, int nhwc, int N, int C, int S,
@@ -124,7 +126,8 @@ int ibl_netvlad_forward(ibl_engine* e, const float* feat, int nhwc, int N, int C
                         int normalize_input, float* vlad_raw, float* vlad_norm, void* stream);
 /* Backward of NetVLAD.forward (what autograd derives for netvlad.py:44-61; SURVEY 8 row a11, used by the SFRS
  * training step, netvlad.py:139-146).  grad_vlad [N,K,C] -> grad_feat (same layout as feat), grad_conv_w [K,C],
- * grad_centroids [K,C] (both summed over the batch).  fp32 CUDA cores; the soft-assignment is recomputed. */
+ * grad_centroids [K,C] (both summed over the batch).  fp32 CUDA cores; the soft-assignment is recomputed.
+ * 1 <= K <= 64 (IBL_ERR_BAD_ARG for K < 1, IBL_ERR_UNSUPPORTED for K > 64). */
 int ibl_netvlad_backward(ibl_engine* e, const float* feat, int nhwc, int N, int C, int S,
                          const float* conv_w, const float* centroids, int K, int normalize_input,
                          const float* grad_vlad, float* grad_feat, float* grad_conv_w,

@@ -39,6 +39,21 @@ void set_last_error(const std::string& s);
 
 static inline int cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
 
+// NetVLAD cluster counts the kernels serve: 1..64.  The tensor-core kernel pads K < 64 to 64 clusters; more than 64
+// would need a different shared-memory plan there and a two-block softmax in the CUDA-core kernels.
+constexpr int NETVLAD_MAX_K = 64;
+static inline int check_netvlad_clusters(int K) {
+  if (K < 1) {
+    set_last_error("bad argument: NetVLAD num_clusters must be in 1..64, got " + std::to_string(K));
+    return IBL_ERR_BAD_ARG;
+  }
+  if (K > NETVLAD_MAX_K) {
+    set_last_error("unsupported: NetVLAD num_clusters must be in 1..64, got " + std::to_string(K));
+    return IBL_ERR_UNSUPPORTED;
+  }
+  return IBL_OK;
+}
+
 // "Done once" flag per CUDA device: function attributes (cudaFuncSetAttribute) and device properties belong
 // to a device, and one process may drive several GPUs (one engine each).  done()/mark() look at the calling
 // thread's current device; setting an attribute twice from two threads is harmless, launching before it
@@ -141,7 +156,7 @@ int debug_gmma_strided(const void* A, int rows, const void* B, int s0, int group
 // tc_netvlad.cu
 int debug_gemm_tn(const float* A, const float* B, float* C, cudaStream_t s);
 int netvlad_tc_units(int B, int S);
-int launch_netvlad_tc(const __nv_bfloat16* x_hi, const __nv_bfloat16* x_lo, int B, int S,
+int launch_netvlad_tc(const __nv_bfloat16* x_hi, const __nv_bfloat16* x_lo, int B, int S, int K,
                       const __nv_bfloat16* w_hi, const __nv_bfloat16* w_lo, const float* ssq, int ssq_parts,
                       const float* cent, bool normalize_input, float* part, float* asum_part, int* ticket,
                       float* vlad_raw, float* vlad_norm, cudaStream_t s);
@@ -194,11 +209,11 @@ int launch_netvlad(const float* feat, bool nhwc, int N, int C, int S, const floa
                    float* invnorm, float* asum, float* vlad_raw, float* vlad_norm,
                    cudaStream_t s, uint64_t* launches);
 int launch_vlad_normalize(const float* raw, int N, int K, int C, float* out, cudaStream_t s);
-int launch_netvlad_assign(const float* feat, bool nhwc, int N, int C, int S, const float* conv_w,
+int launch_netvlad_assign(const float* feat, bool nhwc, int N, int C, int S, const float* conv_w, int K,
                           bool normalize_input, float* assign, float* invnorm, cudaStream_t s);
 // netvlad_bwd.cu
 int launch_netvlad_backward(const float* x, bool nhwc, int N, int C, int S, const float* conv_w,
-                            const float* centroids, const float* g, bool normalize_input, float* assign,
+                            const float* centroids, int K, const float* g, bool normalize_input, float* assign,
                             float* invnorm, float* dz, float* part, int splits, float* dx, float* dW,
                             float* dcent, cudaStream_t s, uint64_t* launches);
 

@@ -89,7 +89,7 @@ struct ibl_engine {
   RerankWs* rr_ws = nullptr;             // sparse stage of the re-ranking: CSR matrices, inverted index, pair buffers
   const int* flag_counter = nullptr;     // guard counter of the last ibl_l2dist_topk call (null: no guard on its path)
   int dist_path = -1;                    // ranking path of the last ibl_l2dist_topk call (ibl_debug_dist_path)
-  DevBuf ssq, nv_part, nv_asum, nvw_pl;  // fused NetVLAD: |x|^2 partials, unit partials, W planes [64,512]
+  DevBuf ssq, nv_part, nv_asum, nvw_pl;  // fused NetVLAD: |x|^2 partials, unit partials, W planes [64,512] (rows K.. zero)
   DevBuf nv_ticket;                      // [images] arrival counters of the fused NetVLAD kernel (zero between launches)
   const float* nvw_pl_src = nullptr;
   cudaStream_t copy_stream = nullptr;   // H2D staging of ibl_extract_host overlaps compute
@@ -335,21 +335,28 @@ int ibl_engine_set_vgg16(ibl_engine* e, const float* const* w13, const float* co
   return IBL_OK;
 }
 
+// conv_w [K,512] -> bf16 hi/lo planes [64,512] each (hi at pl, lo at pl + 64*512) with rows K..63 zero: the layout of
+// the tensor-core NetVLAD kernel for every 1 <= K <= 64
+static int netvlad_weight_planes(const float* conv_w, int K, __nv_bfloat16* pl, cudaStream_t s) {
+  const size_t n64 = (size_t)NETVLAD_MAX_K * 512;
+  if (K < NETVLAD_MAX_K) IBL_CUDA_OK(cudaMemsetAsync(pl, 0, n64 * 4, s));
+  return launch_f32_to_planes(conv_w, (size_t)K * 512, pl, pl + n64, s);
+}
+
 int ibl_engine_set_netvlad(ibl_engine* e, const float* conv_w, const float* centroids, int K, int C,
                            void* stream) {
+  IBL_RET(check_netvlad_clusters(K));
   IBL_REQUIRE(e && conv_w && centroids, "null argument");
-  IBL_REQUIRE(K == 64, "NetVLAD kernels are built for K=64 clusters");
   IBL_REQUIRE(C >= 4 && C % 4 == 0, "NetVLAD dim must be a positive multiple of 4");
   e->nv_w = conv_w;
   e->nv_c = centroids;
   e->nv_K = K;
   e->nv_C = C;
   e->nvw_pl_src = nullptr;
-  if (K == 64 && C == 512) {
+  if (C == 512) {
     DeviceGuard g(e->device);
-    const size_t n = (size_t)K * C;
-    IBL_RET(e->nvw_pl.ensure(n * 4));
-    IBL_RET(launch_f32_to_planes(conv_w, n, e->nvw_pl.as<__nv_bfloat16>(), e->nvw_pl.as<__nv_bfloat16>() + n, S(stream)));
+    IBL_RET(e->nvw_pl.ensure((size_t)NETVLAD_MAX_K * 512 * 4));
+    IBL_RET(netvlad_weight_planes(conv_w, K, e->nvw_pl.as<__nv_bfloat16>(), S(stream)));
     e->launches++;
     e->nvw_pl_src = conv_w;
   }
@@ -510,26 +517,26 @@ int ibl_vgg16_layer_backward(ibl_engine* e, int layer, const float* x, const flo
 int ibl_netvlad_forward(ibl_engine* e, const float* feat, int nhwc, int N, int C, int S_, const float* conv_w,
                         const float* centroids, int K, int normalize_input, float* vlad_raw,
                         float* vlad_norm, void* stream) {
+  IBL_RET(check_netvlad_clusters(K));
   IBL_REQUIRE(e && feat && conv_w && centroids, "null argument");
   IBL_REQUIRE(N >= 1 && C >= 1 && S_ >= 1, "empty NetVLAD input");
-  IBL_REQUIRE(K == 64, "NetVLAD kernels are built for K=64 clusters");
   IBL_REQUIRE(vlad_raw || vlad_norm, "no output requested");
   DeviceGuard g(e->device);
-  if (nhwc && C == 512 && K == 64 && e->gemm_mode == IBL_CONV_TC_BF16X3) {
+  if (nhwc && C == 512 && e->gemm_mode == IBL_CONV_TC_BF16X3) {
     cudaStream_t s = S(stream);
-    const size_t ne = (size_t)N * S_ * C, nw = (size_t)K * C;
+    const size_t ne = (size_t)N * S_ * C, nw = (size_t)NETVLAD_MAX_K * C;
     IBL_RET(e->v_pl.ensure(ne * 4));
     IBL_RET(e->q_pl.ensure(nw * 4));
     IBL_RET(e->ssq.ensure((size_t)N * S_ * sizeof(float)));
     __nv_bfloat16 *xh = e->v_pl.as<__nv_bfloat16>(), *wh = e->q_pl.as<__nv_bfloat16>();
     IBL_RET(launch_f32_to_planes(feat, ne, xh, xh + ne, s));
-    IBL_RET(launch_f32_to_planes(conv_w, nw, wh, wh + nw, s));
+    IBL_RET(netvlad_weight_planes(conv_w, K, wh, s));
     IBL_RET(launch_row_sqnorm(feat, N * S_, C, e->ssq.as<float>(), s));
     const int G = netvlad_tc_units(N, S_);
     IBL_RET(e->nv_part.ensure((size_t)N * G * 64 * 512 * sizeof(float)));
     IBL_RET(e->nv_asum.ensure((size_t)N * G * 64 * sizeof(float)));
     IBL_RET(ensure_tickets(e, N, s));
-    IBL_RET(launch_netvlad_tc(xh, xh + ne, N, S_, wh, wh + nw, e->ssq.as<float>(), 1, centroids,
+    IBL_RET(launch_netvlad_tc(xh, xh + ne, N, S_, K, wh, wh + nw, e->ssq.as<float>(), 1, centroids,
                               normalize_input != 0, e->nv_part.as<float>(), e->nv_asum.as<float>(),
                               e->nv_ticket.as<int>(), vlad_raw, vlad_norm, s));
     e->launches += 4;
@@ -550,17 +557,17 @@ int ibl_netvlad_forward(ibl_engine* e, const float* feat, int nhwc, int N, int C
 int ibl_netvlad_backward(ibl_engine* e, const float* feat, int nhwc, int N, int C, int S_, const float* conv_w,
                          const float* centroids, int K, int normalize_input, const float* grad_vlad,
                          float* grad_feat, float* grad_conv_w, float* grad_centroids, void* stream) {
+  IBL_RET(check_netvlad_clusters(K));
   IBL_REQUIRE(e && feat && conv_w && centroids && grad_vlad && grad_feat && grad_conv_w && grad_centroids,
               "null argument");
   IBL_REQUIRE(N >= 1 && C >= 64 && S_ >= 1, "empty NetVLAD input");
-  IBL_REQUIRE(K == 64, "NetVLAD kernels are built for K=64 clusters");
   DeviceGuard g(e->device);
   const int splits = 64;
   IBL_RET(e->nv_assign.ensure((size_t)N * S_ * K * sizeof(float)));
   IBL_RET(e->nv_inv.ensure((size_t)N * S_ * sizeof(float)));
   IBL_RET(e->nv_raw.ensure((size_t)N * S_ * K * sizeof(float)));                 // dz
   IBL_RET(e->nv_part.ensure((size_t)splits * K * C * sizeof(float)));            // dW partials
-  return launch_netvlad_backward(feat, nhwc != 0, N, C, S_, conv_w, centroids, grad_vlad, normalize_input != 0,
+  return launch_netvlad_backward(feat, nhwc != 0, N, C, S_, conv_w, centroids, K, grad_vlad, normalize_input != 0,
                                  e->nv_assign.as<float>(), e->nv_inv.as<float>(), e->nv_raw.as<float>(),
                                  e->nv_part.as<float>(), splits, grad_feat, grad_conv_w, grad_centroids, S(stream),
                                  &e->launches);
@@ -642,7 +649,7 @@ int ibl_extract(ibl_engine* e, const float* x, int N, int H, int W, unsigned fla
       vdst = e->vlad.as<float>();
     }
     const bool fused = e->conv_mode == IBL_CONV_TC_BF16X3 && e->gemm_mode == IBL_CONV_TC_BF16X3 &&
-                       e->nvw_pl_src == e->nv_w && K == 64 && C == 512;
+                       e->nvw_pl_src == e->nv_w && C == 512;
     if (fused) {
       // conv5_3 -> hi/lo planes + |x|^2 partials -> one tensor-core NetVLAD kernel (+ finalize)
       FeatPlanes fp;
@@ -655,8 +662,8 @@ int ibl_extract(ibl_engine* e, const float* x, int N, int H, int W, unsigned fla
       IBL_RET(e->nv_part.ensure((size_t)nb * G * 64 * 512 * sizeof(float)));
       IBL_RET(e->nv_asum.ensure((size_t)nb * G * 64 * sizeof(float)));
       IBL_RET(ensure_tickets(e, nb, S(stream)));
-      const size_t nw = (size_t)64 * 512;
-      IBL_RET(launch_netvlad_tc(fp.hi, fp.lo, nb, Sp, e->nvw_pl.as<__nv_bfloat16>(), e->nvw_pl.as<__nv_bfloat16>() + nw,
+      const size_t nw = (size_t)NETVLAD_MAX_K * 512;
+      IBL_RET(launch_netvlad_tc(fp.hi, fp.lo, nb, Sp, K, e->nvw_pl.as<__nv_bfloat16>(), e->nvw_pl.as<__nv_bfloat16>() + nw,
                                 e->ssq.as<float>(), fp.ssq_parts, e->nv_c, true, e->nv_part.as<float>(),
                                 e->nv_asum.as<float>(), e->nv_ticket.as<int>(), nullptr, vdst, S(stream)));
       e->launches += 1;                     // ONE launch: partials, centroid term, intra-norm and L2 inside the kernel

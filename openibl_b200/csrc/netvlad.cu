@@ -7,11 +7,14 @@
 //
 // The reference materialises a [N,K,C,S] residual tensor (157 MB / image); here the two
 // contractions are tiled GEMMs and nothing larger than [N,S,K] is written.
+//
+// The blocks are 64 clusters wide.  K < 64 clusters run on the same blocks: clusters K..63 get zero weights and are
+// left out of the softmax, so their assignment is 0; assign and the outputs are stored at a stride of K.
 #include "common.cuh"
 
 namespace ibl {
 
-constexpr int NV_K = 64;  // clusters handled per block (the reference uses K=64)
+constexpr int NV_K = 64;  // clusters handled per block: the most the kernels serve (the reference default)
 
 // element (n,s,c) of the feature map for both supported layouts
 struct FeatView {
@@ -25,8 +28,8 @@ struct FeatView {
 // ---- kernel A: per-pixel inverse norm + soft-assignment -----------------------------------
 // block = 32 pixels x 64 clusters, 256 threads: thread (p = t%32, kg = t/32) owns 8 logits.
 __global__ void __launch_bounds__(256)
-netvlad_assign_kernel(FeatView f, bool nhwc, int C, int S, const float* __restrict__ w /*[64][C]*/,
-                      int normalize_input, float* __restrict__ assign /*[N,S,64]*/,
+netvlad_assign_kernel(FeatView f, bool nhwc, int C, int S, const float* __restrict__ w /*[K][C]*/, int K,
+                      int normalize_input, float* __restrict__ assign /*[N,S,K]*/,
                       float* __restrict__ invnorm /*[N,S]*/) {
   __shared__ float xs[32][65];
   __shared__ float wsm[NV_K][65];
@@ -51,7 +54,7 @@ netvlad_assign_kernel(FeatView f, bool nhwc, int C, int S, const float* __restri
     }
     for (int e = t; e < NV_K * 64; e += 256) {
       const int k = e >> 6, cc = e & 63;
-      wsm[k][cc] = (c0 + cc < C) ? __ldg(w + (long long)k * C + c0 + cc) : 0.f;
+      wsm[k][cc] = (k < K && c0 + cc < C) ? __ldg(w + (long long)k * C + c0 + cc) : 0.f;
     }
     __syncthreads();
 #pragma unroll 8
@@ -70,12 +73,14 @@ netvlad_assign_kernel(FeatView f, bool nhwc, int C, int S, const float* __restri
   for (int j = 0; j < 8; ++j) zs[p][kg * 8 + j] = acc[j] * inv;
   __syncthreads();
 
-  // softmax over the 64 clusters: warp w handles pixels 4w..4w+3, two clusters per lane
+  // softmax over the K clusters: warp w handles pixels 4w..4w+3, two clusters per lane
   const int lane = t & 31, wid = t >> 5;
   for (int q = 0; q < 4; ++q) {
     const int pp = wid * 4 + q;
     const int s = s0 + pp;
     float z0 = zs[pp][lane], z1 = zs[pp][lane + 32];
+    if (lane >= K) z0 = -INFINITY;
+    if (lane + 32 >= K) z1 = -INFINITY;
     float m = fmaxf(z0, z1);
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
@@ -84,9 +89,9 @@ netvlad_assign_kernel(FeatView f, bool nhwc, int C, int S, const float* __restri
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
     if (s < S) {
-      float* ap = assign + (n * S + s) * (long long)NV_K;
-      ap[lane] = e0 / sum;
-      ap[lane + 32] = e1 / sum;
+      float* ap = assign + (n * S + s) * (long long)K;
+      if (lane < K) ap[lane] = e0 / sum;
+      if (lane + 32 < K) ap[lane + 32] = e1 / sum;
       if (lane == 0) invnorm[n * S + s] = inv_s[pp];
     }
   }
@@ -95,9 +100,9 @@ netvlad_assign_kernel(FeatView f, bool nhwc, int C, int S, const float* __restri
 // ---- kernel B: vlad[k,c] = sum_s a[s,k] (x[s,c] inv[s]) - cent[k,c] asum[k] -----------------
 // block = 64 clusters x 64 channels, 256 threads, 4x4 per thread, S in chunks of 16.
 __global__ void __launch_bounds__(256)
-netvlad_aggregate_kernel(FeatView f, bool nhwc, int C, int S, const float* __restrict__ assign,
+netvlad_aggregate_kernel(FeatView f, bool nhwc, int C, int S, int K, const float* __restrict__ assign,
                          const float* __restrict__ invnorm, const float* __restrict__ cent,
-                         float* __restrict__ raw /*[N,64,C]*/) {
+                         float* __restrict__ raw /*[N,K,C]*/) {
   __shared__ __align__(16) float As[16][NV_K];
   __shared__ __align__(16) float Bs[16][64];
   const int t = threadIdx.x;
@@ -116,7 +121,7 @@ netvlad_aggregate_kernel(FeatView f, bool nhwc, int C, int S, const float* __res
     for (int e = t; e < 16 * 64; e += 256) {
       const int ss = e >> 6, k = e & 63;
       const int s = sb + ss;
-      As[ss][k] = (s < S) ? __ldg(assign + (n * S + s) * (long long)NV_K + k) : 0.f;
+      As[ss][k] = (s < S && k < K) ? __ldg(assign + (n * S + s) * (long long)K + k) : 0.f;
     }
     for (int e = t; e < 16 * 64; e += 256) {
       int ss, cc;
@@ -145,10 +150,11 @@ netvlad_aggregate_kernel(FeatView f, bool nhwc, int C, int S, const float* __res
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     const int k = tm * 4 + i;
+    if (k >= K) break;
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const int c = c0 + tn * 4 + j;
-      if (c < C) raw[(n * NV_K + k) * (long long)C + c] = acc[i][j] - __ldg(cent + (long long)k * C + c) * asum[i];
+      if (c < C) raw[(n * K + k) * (long long)C + c] = acc[i][j] - __ldg(cent + (long long)k * C + c) * asum[i];
     }
   }
 }
@@ -201,16 +207,16 @@ int launch_netvlad(const float* feat, bool nhwc, int N, int C, int S, const floa
                    float* invnorm, float* asum, float* vlad_raw, float* vlad_norm,
                    cudaStream_t s, uint64_t* launches) {
   (void)asum;
-  IBL_REQUIRE(K == NV_K, "NetVLAD kernels are built for K=64 clusters");
+  IBL_REQUIRE(K >= 1 && K <= NV_K, "NetVLAD kernels serve 1..64 clusters");
   FeatView f;
   f.p = feat;
   f.sN = (long long)S * C;
   if (nhwc) { f.sS = C; f.sC = 1; } else { f.sS = 1; f.sC = S; }
   dim3 ga((unsigned)cdiv(S, 32), (unsigned)N);
-  netvlad_assign_kernel<<<ga, 256, 0, s>>>(f, nhwc, C, S, conv_w, normalize_input ? 1 : 0, assign, invnorm);
+  netvlad_assign_kernel<<<ga, 256, 0, s>>>(f, nhwc, C, S, conv_w, K, normalize_input ? 1 : 0, assign, invnorm);
   IBL_CUDA_OK(cudaGetLastError());
   dim3 gb((unsigned)cdiv(C, 64), (unsigned)N);
-  netvlad_aggregate_kernel<<<gb, 256, 0, s>>>(f, nhwc, C, S, assign, invnorm, centroids, vlad_raw);
+  netvlad_aggregate_kernel<<<gb, 256, 0, s>>>(f, nhwc, C, S, K, assign, invnorm, centroids, vlad_raw);
   IBL_CUDA_OK(cudaGetLastError());
   *launches += 2;
   if (vlad_norm) {
@@ -224,14 +230,15 @@ int launch_netvlad(const float* feat, bool nhwc, int N, int C, int S, const floa
 
 namespace ibl {
 // soft-assignment + inverse norms only (shared with the backward pass, netvlad_bwd.cu)
-int launch_netvlad_assign(const float* feat, bool nhwc, int N, int C, int S, const float* conv_w,
+int launch_netvlad_assign(const float* feat, bool nhwc, int N, int C, int S, const float* conv_w, int K,
                           bool normalize_input, float* assign, float* invnorm, cudaStream_t s) {
+  IBL_REQUIRE(K >= 1 && K <= NV_K, "NetVLAD kernels serve 1..64 clusters");
   FeatView f;
   f.p = feat;
   f.sN = (long long)S * C;
   if (nhwc) { f.sS = C; f.sC = 1; } else { f.sS = 1; f.sC = S; }
   dim3 ga((unsigned)cdiv(S, 32), (unsigned)N);
-  netvlad_assign_kernel<<<ga, 256, 0, s>>>(f, nhwc, C, S, conv_w, normalize_input ? 1 : 0, assign, invnorm);
+  netvlad_assign_kernel<<<ga, 256, 0, s>>>(f, nhwc, C, S, conv_w, K, normalize_input ? 1 : 0, assign, invnorm);
   IBL_CUDA_OK(cudaGetLastError());
   return IBL_OK;
 }

@@ -12,11 +12,14 @@
 //
 // The soft-assignment a and 1/|x| are recomputed with the forward's assign kernel instead of being
 // saved (the reference's autograd keeps the [N,K,C,S] residual tensor alive for backward).
+//
+// The blocks are 64 clusters wide; for K < 64 clusters K..63 load zeros (a, dz, g, W, cent), so they add nothing, and
+// every [.., K] / [K, C] tensor is read and written at a stride of K.
 #include "common.cuh"
 
 namespace ibl {
 
-constexpr int NB_K = 64;
+constexpr int NB_K = 64;   // clusters per block: the most the kernels serve
 
 struct FeatV {
   const float* p;
@@ -27,9 +30,9 @@ struct FeatV {
 // ---- dz[n,s,k] and asum[n,k] --------------------------------------------------------------------
 // block = 32 pixels x 64 clusters (256 threads: thread (p = t%32, kg = t/32) owns 8 clusters)
 __global__ void __launch_bounds__(256)
-nv_bwd_dz_kernel(FeatV f, bool nhwc, int C, int S, const float* __restrict__ g /*[N,64,C]*/,
-                 const float* __restrict__ cent, const float* __restrict__ assign /*[N,S,64]*/,
-                 const float* __restrict__ invnorm /*[N,S]*/, float* __restrict__ dz /*[N,S,64]*/) {
+nv_bwd_dz_kernel(FeatV f, bool nhwc, int C, int S, int K, const float* __restrict__ g /*[N,K,C]*/,
+                 const float* __restrict__ cent, const float* __restrict__ assign /*[N,S,K]*/,
+                 const float* __restrict__ invnorm /*[N,S]*/, float* __restrict__ dz /*[N,S,K]*/) {
   __shared__ float xs[32][65];
   __shared__ float gs[NB_K][65];
   __shared__ float ps[32][65];
@@ -37,12 +40,13 @@ nv_bwd_dz_kernel(FeatV f, bool nhwc, int C, int S, const float* __restrict__ g /
   const int t = threadIdx.x, p = t & 31, kg = t >> 5;
   const long long n = blockIdx.y;
   const int s0 = blockIdx.x * 32;
-  const float* gn = g + n * NB_K * (long long)C;
+  const float* gn = g + n * K * (long long)C;
   // gc[k] = g[k,:].cent[k,:]  (4 threads per cluster)
   {
     const int k = t >> 2, part = t & 3;
     float acc = 0.f;
-    for (int c = part; c < C; c += 4) acc = fmaf(__ldg(gn + (long long)k * C + c), __ldg(cent + (long long)k * C + c), acc);
+    if (k < K)
+      for (int c = part; c < C; c += 4) acc = fmaf(__ldg(gn + (long long)k * C + c), __ldg(cent + (long long)k * C + c), acc);
     acc += __shfl_xor_sync(0xffffffffu, acc, 1);
     acc += __shfl_xor_sync(0xffffffffu, acc, 2);
     if (part == 0) gc[k] = acc;
@@ -60,7 +64,7 @@ nv_bwd_dz_kernel(FeatV f, bool nhwc, int C, int S, const float* __restrict__ g /
     }
     for (int e = t; e < NB_K * 64; e += 256) {
       const int k = e >> 6, cc = e & 63;
-      gs[k][cc] = (c0 + cc < C) ? __ldg(gn + (long long)k * C + c0 + cc) : 0.f;
+      gs[k][cc] = (k < K && c0 + cc < C) ? __ldg(gn + (long long)k * C + c0 + cc) : 0.f;
     }
     __syncthreads();
 #pragma unroll 8
@@ -78,22 +82,22 @@ nv_bwd_dz_kernel(FeatV f, bool nhwc, int C, int S, const float* __restrict__ g /
   for (int q = 0; q < 4; ++q) {
     const int pp = wid * 4 + q, s = s0 + pp;
     if (s >= S) continue;                         // warp-uniform
-    const float* ap = assign + (n * S + s) * (long long)NB_K;
-    const float a0 = __ldg(ap + lane), a1 = __ldg(ap + lane + 32);
+    const float* ap = assign + (n * S + s) * (long long)K;
+    const float a0 = lane < K ? __ldg(ap + lane) : 0.f, a1 = lane + 32 < K ? __ldg(ap + lane + 32) : 0.f;
     const float d0 = ps[pp][lane], d1 = ps[pp][lane + 32];
     float tsum = a0 * d0 + a1 * d1;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) tsum += __shfl_xor_sync(0xffffffffu, tsum, o);
-    float* o = dz + (n * S + s) * (long long)NB_K;
-    o[lane] = a0 * (d0 - tsum);
-    o[lane + 32] = a1 * (d1 - tsum);
+    float* o = dz + (n * S + s) * (long long)K;
+    if (lane < K) o[lane] = a0 * (d0 - tsum);
+    if (lane + 32 < K) o[lane + 32] = a1 * (d1 - tsum);
   }
 }
 
 // ---- dx: one block per 32 pixels, all channels kept in shared memory ---------------------------------
 // dx^[s,c] = sum_k a[s,k] g[k,c] + dz[s,k] W[k,c];  dx = inv (dx^ - x^ (x^.dx^))
 __global__ void __launch_bounds__(256)
-nv_bwd_dx_kernel(FeatV f, bool nhwc, int C, int S, const float* __restrict__ g, const float* __restrict__ w,
+nv_bwd_dx_kernel(FeatV f, bool nhwc, int C, int S, int K, const float* __restrict__ g, const float* __restrict__ w,
                  const float* __restrict__ assign, const float* __restrict__ dz,
                  const float* __restrict__ invnorm, int normalize_input, float* __restrict__ dx,
                  long long dN, long long dS, long long dC) {
@@ -110,15 +114,15 @@ nv_bwd_dx_kernel(FeatV f, bool nhwc, int C, int S, const float* __restrict__ g, 
   const int ldx = C + 1;
   for (int e = t; e < 32 * 64; e += 256) {
     const int pp = e >> 6, k = e & 63, s = s0 + pp;
-    a_t[pp * 65 + k] = (s < S) ? __ldg(assign + (n * S + s) * (long long)NB_K + k) : 0.f;
-    z_t[pp * 65 + k] = (s < S) ? __ldg(dz + (n * S + s) * (long long)NB_K + k) : 0.f;
+    a_t[pp * 65 + k] = (s < S && k < K) ? __ldg(assign + (n * S + s) * (long long)K + k) : 0.f;
+    z_t[pp * 65 + k] = (s < S && k < K) ? __ldg(dz + (n * S + s) * (long long)K + k) : 0.f;
   }
-  const float* gn = g + n * NB_K * (long long)C;
+  const float* gn = g + n * K * (long long)C;
   for (int c0 = 0; c0 < C; c0 += 64) {
     __syncthreads();
     for (int e = t; e < NB_K * 64; e += 256) {
       const int k = e >> 6, cc = e & 63;
-      const bool ok = c0 + cc < C;
+      const bool ok = k < K && c0 + cc < C;
       g_t[k * 65 + cc] = ok ? __ldg(gn + (long long)k * C + c0 + cc) : 0.f;
       w_t[k * 65 + cc] = ok ? __ldg(w + (long long)k * C + c0 + cc) : 0.f;
     }
@@ -168,7 +172,7 @@ nv_bwd_dx_kernel(FeatV f, bool nhwc, int C, int S, const float* __restrict__ g, 
 // ---- dW partials: part[z][k][c] = sum over the z-th slice of (n,s) of dz[n,s,k] x^[n,s,c] ------------
 // block = 64 clusters x 64 channels, 4x4 per thread; grid (C/64, splits)
 __global__ void __launch_bounds__(256)
-nv_bwd_dw_kernel(FeatV f, bool nhwc, int C, int S, int N, const float* __restrict__ dz,
+nv_bwd_dw_kernel(FeatV f, bool nhwc, int C, int S, int N, int K, const float* __restrict__ dz,
                  const float* __restrict__ invnorm, int rows_per_split, float* __restrict__ part) {
   __shared__ __align__(16) float As[16][NB_K];
   __shared__ __align__(16) float Bs[16][64];
@@ -186,7 +190,7 @@ nv_bwd_dw_kernel(FeatV f, bool nhwc, int C, int S, int N, const float* __restric
     for (int e = t; e < 16 * 64; e += 256) {
       const int rr = e >> 6, k = e & 63;
       const long long r = rb + rr;
-      As[rr][k] = (r < r1) ? __ldg(dz + r * NB_K + k) : 0.f;
+      As[rr][k] = (r < r1 && k < K) ? __ldg(dz + r * K + k) : 0.f;
     }
     for (int e = t; e < 16 * 64; e += 256) {
       int rr, cc;
@@ -213,27 +217,27 @@ nv_bwd_dw_kernel(FeatV f, bool nhwc, int C, int S, int N, const float* __restric
     }
     __syncthreads();
   }
-  float* o = part + (long long)blockIdx.y * NB_K * C;
+  float* o = part + (long long)blockIdx.y * K * C;
 #pragma unroll
   for (int i = 0; i < 4; ++i)
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const int c = c0 + tn * 4 + j;
-      if (c < C) o[(long long)(tm * 4 + i) * C + c] = acc[i][j];
+      if (tm * 4 + i < K && c < C) o[(long long)(tm * 4 + i) * C + c] = acc[i][j];
     }
 }
 
 // dW[k,c] = sum_z part[z][k][c];  dcent[k,c] = - sum_n g[n,k,c] asum[n,k],  asum[n,k] = sum_s a[n,s,k]
 __global__ void __launch_bounds__(256)
-nv_bwd_reduce_kernel(const float* __restrict__ part, int splits, int C, int N, int S,
+nv_bwd_reduce_kernel(const float* __restrict__ part, int splits, int C, int N, int S, int K,
                      const float* __restrict__ g, const float* __restrict__ assign,
                      float* __restrict__ dW, float* __restrict__ dcent) {
   __shared__ float asum_s[8];
-  const int k = blockIdx.x;      // one block per cluster
+  const int k = blockIdx.x;      // one block per cluster, K blocks
   // dW row
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     float v = 0.f;
-    for (int z = 0; z < splits; ++z) v += part[((long long)z * NB_K + k) * C + c];
+    for (int z = 0; z < splits; ++z) v += part[((long long)z * K + k) * C + c];
     dW[(long long)k * C + c] = v;
   }
   // dcent row: accumulate over images; asum[n,k] by a block reduction per image
@@ -241,7 +245,7 @@ nv_bwd_reduce_kernel(const float* __restrict__ part, int splits, int C, int N, i
   for (int c = threadIdx.x; c < C; c += blockDim.x) dc[c] = 0.f;
   for (int n = 0; n < N; ++n) {
     float a = 0.f;
-    for (int s = threadIdx.x; s < S; s += blockDim.x) a += __ldg(assign + ((long long)n * S + s) * NB_K + k);
+    for (int s = threadIdx.x; s < S; s += blockDim.x) a += __ldg(assign + ((long long)n * S + s) * K + k);
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
     __syncthreads();
@@ -249,24 +253,25 @@ nv_bwd_reduce_kernel(const float* __restrict__ part, int splits, int C, int N, i
     __syncthreads();
     float tot = 0.f;
     for (int i = 0; i < (int)(blockDim.x >> 5); ++i) tot += asum_s[i];
-    const float* gn = g + ((long long)n * NB_K + k) * C;
+    const float* gn = g + ((long long)n * K + k) * C;
     for (int c = threadIdx.x; c < C; c += blockDim.x) dc[c] -= __ldg(gn + c) * tot;
   }
 }
 
 int launch_netvlad_backward(const float* x, bool nhwc, int N, int C, int S, const float* conv_w,
-                            const float* centroids, const float* g, bool normalize_input, float* assign,
+                            const float* centroids, int K, const float* g, bool normalize_input, float* assign,
                             float* invnorm, float* dz, float* part, int splits, float* dx, float* dW,
                             float* dcent, cudaStream_t s, uint64_t* launches) {
   IBL_REQUIRE(C % 4 == 0 && C <= 2048, "NetVLAD backward: C must be a multiple of 4 and <= 2048");
+  IBL_REQUIRE(K >= 1 && K <= NB_K, "NetVLAD backward kernels serve 1..64 clusters");
   // recompute a and 1/|x| with the forward kernels (raw vlad goes to `part` as scratch and is discarded)
   FeatV f;
   f.p = x;
   f.sN = (long long)S * C;
   if (nhwc) { f.sS = C; f.sC = 1; } else { f.sS = 1; f.sC = S; }
-  IBL_RET(launch_netvlad_assign(x, nhwc, N, C, S, conv_w, normalize_input, assign, invnorm, s));
+  IBL_RET(launch_netvlad_assign(x, nhwc, N, C, S, conv_w, K, normalize_input, assign, invnorm, s));
   dim3 g1((unsigned)cdiv(S, 32), (unsigned)N);
-  nv_bwd_dz_kernel<<<g1, 256, 0, s>>>(f, nhwc, C, S, g, centroids, assign, invnorm, dz);
+  nv_bwd_dz_kernel<<<g1, 256, 0, s>>>(f, nhwc, C, S, K, g, centroids, assign, invnorm, dz);
   IBL_CUDA_OK(cudaGetLastError());
   const size_t smem = (size_t)(2 * 32 * 65 + 2 * 64 * 65 + 32 * (C + 1)) * sizeof(float);
   static DeviceOnce attr_done;   // the attribute is per device
@@ -275,17 +280,17 @@ int launch_netvlad_backward(const float* x, bool nhwc, int N, int C, int S, cons
     attr_done.mark();
   }
   const long long dN = (long long)S * C, dS = nhwc ? C : 1, dC = nhwc ? 1 : S;
-  nv_bwd_dx_kernel<<<g1, 256, smem, s>>>(f, nhwc, C, S, g, conv_w, assign, dz, invnorm, normalize_input ? 1 : 0, dx,
+  nv_bwd_dx_kernel<<<g1, 256, smem, s>>>(f, nhwc, C, S, K, g, conv_w, assign, dz, invnorm, normalize_input ? 1 : 0, dx,
                                          dN, dS, dC);
   IBL_CUDA_OK(cudaGetLastError());
   const long long R = (long long)N * S;
   int rows_per_split = (int)((R + splits - 1) / splits);
   rows_per_split = ((rows_per_split + 15) / 16) * 16;
   const int nsplit = (int)((R + rows_per_split - 1) / rows_per_split);
-  nv_bwd_dw_kernel<<<dim3((unsigned)cdiv(C, 64), (unsigned)nsplit), 256, 0, s>>>(f, nhwc, C, S, N, dz, invnorm,
+  nv_bwd_dw_kernel<<<dim3((unsigned)cdiv(C, 64), (unsigned)nsplit), 256, 0, s>>>(f, nhwc, C, S, N, K, dz, invnorm,
                                                                                   rows_per_split, part);
   IBL_CUDA_OK(cudaGetLastError());
-  nv_bwd_reduce_kernel<<<NB_K, 256, 0, s>>>(part, nsplit, C, N, S, g, assign, dW, dcent);
+  nv_bwd_reduce_kernel<<<K, 256, 0, s>>>(part, nsplit, C, N, S, K, g, assign, dW, dcent);
   IBL_CUDA_OK(cudaGetLastError());
   *launches += 5;
   return IBL_OK;

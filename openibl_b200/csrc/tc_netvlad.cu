@@ -105,6 +105,10 @@ int debug_gemm_tn(const float* A, const float* B, float* C, cudaStream_t s) {
 //                                       tiles, and a' = a/|x| written to shared memory by the softmax)
 //   vlad[k,c] = V[c,k] - cent[k,c] * sum_s a[s,k]
 //
+// K <= 64 clusters run on the K = 64 layout: rows K..63 of the W planes are zero and their logits are set to -inf
+// before the softmax, so their a, a', sum_s a and V columns are exactly 0.  The partials keep 64 rows; only the
+// finalisation knows K (it reads centroid rows k < K and writes [B][K][512]).
+//
 // One work unit = (image, every G-th 128-pixel tile); a unit accumulates V (512 x 64 fp32, too large for the
 // registers of one warpgroup) in its own partial slice in global memory, which stays in L2: every element is
 // read-modified-written by the same thread, tile after tile, in tile order.  ONE LAUNCH: the unit that arrives last for an image
@@ -121,14 +125,15 @@ int debug_gemm_tn(const float* A, const float* B, float* C, cudaStream_t s) {
 // =====================================================================================================
 struct NvTcArgs {
   int B, S, G, T;                 // images, pixels per image, units per image, 128-pixel tiles per image
+  int K;                          // clusters, 1..64
   int ssq_parts;                  // number of partial |x|^2 planes to add
   const float* ssq;               // [ssq_parts][B*S]
   int normalize_input;
   float* part;                    // [B*G][64][512]   partial V^T (k-major rows, c contiguous)
   float* asum_part;               // [B*G][64]
-  const float* cent;              // [64][512] centroids
-  float* vlad_raw;                // [B][64][512] un-normalised VLAD (nullable)
-  float* vlad_norm;               // [B][64*512] intra-normalised + L2-normalised descriptor (nullable)
+  const float* cent;              // [K][512] centroids
+  float* vlad_raw;                // [B][K][512] un-normalised VLAD (nullable)
+  float* vlad_norm;               // [B][K*512] intra-normalised + L2-normalised descriptor (nullable)
   int* ticket;                    // [B] zero on entry; the unit that takes ticket G-1 finalises the image and resets it
 };
 
@@ -154,9 +159,11 @@ struct NvIter {
 //   vlad[k,c] = sum_g part[b,g,k,c] - cent[k,c] * sum_g asum[b,g,k]   (partials added in index order: deterministic)
 //   intra-normalise every cluster row (netvlad.py:78), flatten k-major, global L2 (:79-80).
 // Warp q owns rows q*16 .. q*16+15, lane L the channels L, L+32, ...; every thread rescales exactly the elements it
-// wrote itself, so the second pass needs no fence.  `sm` is the 260-float asum scratch of the kernel.
+// wrote itself, so the second pass needs no fence.  `sm` is the 260-float asum scratch of the kernel.  Rows k >= K are
+// zero in the partials: they are neither read from the centroids nor written, and add nothing to the norms.
 __device__ __forceinline__ void nv_finalize_image(const NvTcArgs& a, int b, int q, int lane, float* sm) {
   const int tid = q * 32 + lane;
+  const int K = a.K;
   const long long ub = (long long)b * a.G;
   if (tid < 64) {
     float s = 0.f;
@@ -175,7 +182,9 @@ __device__ __forceinline__ void nv_finalize_image(const NvTcArgs& a, int b, int 
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         v[u][j] = make_float4(0.f, 0.f, 0.f, 0.f);
-        cz[u][j] = __ldg(reinterpret_cast<const float4*>(a.cent + (q * 16 + r + u) * 512 + 4 * lane + 128 * j));
+        cz[u][j] = q * 16 + r + u < K
+                       ? __ldg(reinterpret_cast<const float4*>(a.cent + (q * 16 + r + u) * 512 + 4 * lane + 128 * j))
+                       : make_float4(0.f, 0.f, 0.f, 0.f);
       }
 #pragma unroll
     for (int g = 0; g < 4; ++g) {                      // G <= 4 (netvlad_tc_units); partials added in index order
@@ -210,13 +219,13 @@ __device__ __forceinline__ void nv_finalize_image(const NvTcArgs& a, int b, int 
       for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
       const float inv = 1.f / fmaxf(sqrtf(ss), 1e-12f);
       float s2 = 0.f;
-      const long long row = ((long long)b * 64 + k) * 512 + 4 * lane;
+      const long long row = ((long long)b * K + k) * 512 + 4 * lane;
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
-        if (a.vlad_raw) *reinterpret_cast<float4*>(a.vlad_raw + row + 128 * j) = v[u][j];
+        if (a.vlad_raw && k < K) *reinterpret_cast<float4*>(a.vlad_raw + row + 128 * j) = v[u][j];
         const float4 w = make_float4(v[u][j].x * inv, v[u][j].y * inv, v[u][j].z * inv, v[u][j].w * inv);
         s2 = fmaf(w.x, w.x, s2); s2 = fmaf(w.y, w.y, s2); s2 = fmaf(w.z, w.z, s2); s2 = fmaf(w.w, w.w, s2);
-        if (a.vlad_norm) *reinterpret_cast<float4*>(a.vlad_norm + row + 128 * j) = w;
+        if (a.vlad_norm && k < K) *reinterpret_cast<float4*>(a.vlad_norm + row + 128 * j) = w;
       }
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) s2 += __shfl_xor_sync(0xffffffffu, s2, o);
@@ -229,13 +238,24 @@ __device__ __forceinline__ void nv_finalize_image(const NvTcArgs& a, int b, int 
   const float ginv = 1.f / fmaxf(sqrtf((sm[128] + sm[129]) + (sm[130] + sm[131])), 1e-12f);
 #pragma unroll 1
   for (int r8 = 0; r8 < 2; ++r8) {                   // 8 rows = 32 independent 16-byte loads per thread in flight
-    float4* o = reinterpret_cast<float4*>(a.vlad_norm + ((long long)b * 64 + q * 16 + r8 * 8) * 512 + 4 * lane);
-    float4 t[32];
+    const int k0 = q * 16 + r8 * 8;
+    float4* o = reinterpret_cast<float4*>(a.vlad_norm + ((long long)b * K + k0) * 512 + 4 * lane);
+    if (k0 + 8 <= K) {                               // warp-uniform: 8 whole rows
+      float4 t[32];
 #pragma unroll
-    for (int i = 0; i < 32; ++i) t[i] = o[(i >> 2) * 128 + 32 * (i & 3)];
+      for (int i = 0; i < 32; ++i) t[i] = o[(i >> 2) * 128 + 32 * (i & 3)];
 #pragma unroll
-    for (int i = 0; i < 32; ++i)
-      o[(i >> 2) * 128 + 32 * (i & 3)] = make_float4(t[i].x * ginv, t[i].y * ginv, t[i].z * ginv, t[i].w * ginv);
+      for (int i = 0; i < 32; ++i)
+        o[(i >> 2) * 128 + 32 * (i & 3)] = make_float4(t[i].x * ginv, t[i].y * ginv, t[i].z * ginv, t[i].w * ginv);
+    } else {                                         // the 8-row block that K < 64 cuts: its rows below K only
+#pragma unroll 1
+      for (int r = 0; k0 + r < K; ++r)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const float4 t = o[r * 128 + 32 * j];
+          o[r * 128 + 32 * j] = make_float4(t.x * ginv, t.y * ginv, t.z * ginv, t.w * ginv);
+        }
+    }
   }
 }
 
@@ -377,6 +397,11 @@ netvlad_tc_kernel(const __grid_constant__ CUtensorMap tm_xhi, const __grid_const
             for (int j = 0; j < 32; ++j) z[h * 32 + j] = __uint_as_float(r0[j]) * inv;
           }
           wg_sync();                                 // every row has read its logits before a' overwrites them
+        }
+        if (a.K < 64) {                              // padded clusters: assignment exactly 0
+#pragma unroll
+          for (int j = 0; j < 64; ++j)
+            if (j >= a.K) z[j] = -INFINITY;
         }
         float m = z[0];
 #pragma unroll
@@ -531,11 +556,13 @@ int netvlad_tc_units(int B, int S) {
   return T < 4 ? T : 4;
 }
 
-// x planes [B,S,512] (hi, lo), w planes [64,512] (hi, lo), ssq [parts][B*S], cent [64,512] fp32
-int launch_netvlad_tc(const __nv_bfloat16* x_hi, const __nv_bfloat16* x_lo, int B, int S,
+// x planes [B,S,512] (hi, lo), w planes [64,512] (hi, lo; rows K..63 zero), ssq [parts][B*S], cent [K,512] fp32,
+// vlad_raw [B,K,512], vlad_norm [B,K*512]; part / asum_part are sized for 64 clusters whatever K is
+int launch_netvlad_tc(const __nv_bfloat16* x_hi, const __nv_bfloat16* x_lo, int B, int S, int K,
                       const __nv_bfloat16* w_hi, const __nv_bfloat16* w_lo, const float* ssq, int ssq_parts,
                       const float* cent, bool normalize_input, float* part, float* asum_part, int* ticket,
                       float* vlad_raw, float* vlad_norm, cudaStream_t s) {
+  IBL_REQUIRE(K >= 1 && K <= 64, "the tensor-core NetVLAD kernel serves 1..64 clusters");
   CUtensorMap mx_hi, mx_lo, mw_hi, mw_lo;
   {
     uint64_t dims[3] = {512, (uint64_t)S, (uint64_t)B};
@@ -552,7 +579,7 @@ int launch_netvlad_tc(const __nv_bfloat16* x_hi, const __nv_bfloat16* x_lo, int 
     IBL_RET(make_tmap(&mw_lo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, w_lo, dims, str, box));
   }
   NvTcArgs a{};
-  a.B = B; a.S = S; a.T = cdiv(S, 128); a.G = netvlad_tc_units(B, S);
+  a.B = B; a.S = S; a.K = K; a.T = cdiv(S, 128); a.G = netvlad_tc_units(B, S);
   a.ssq = ssq; a.ssq_parts = ssq_parts; a.normalize_input = normalize_input ? 1 : 0;
   a.part = part; a.asum_part = asum_part;
   a.cent = cent; a.vlad_raw = vlad_raw; a.vlad_norm = vlad_norm; a.ticket = ticket;

@@ -8,10 +8,10 @@ bytes.  Shapes follow the reference:
   * VGG16 trunk conv1_1..conv5_3: 13 convs 3x3, state-dict slots
     {0,2,5,7,10,12,14,17,19,21,24,26,28} (reference ibl/models/vgg.py:40-42),
     kaiming-normal fan_out weights, zero bias (vgg.py:72-77).
-  * NetVLAD K=64, C=512: centroids ~ U[0,1) (netvlad.py:29); conv weight
+  * NetVLAD K=64 (any 1..64 on request), C=512: centroids ~ U[0,1) (netvlad.py:29); conv weight
     default Conv2d init; the "sharp" variant mimics _init_params
     (netvlad.py:34-42) with alpha from the top-2 dot gap.
-  * PCA layer Conv2d(32768, 4096, 1) default init (netvlad.py:89).
+  * PCA layer Conv2d(K*512, 4096, 1) default init (netvlad.py:89).
 """
 from __future__ import annotations
 
@@ -76,7 +76,8 @@ def make_netvlad_params(seed: int = 0, num_clusters: int = 64, dim: int = 512, s
     dots = assign @ desc.numpy().T
     dots.sort(0)
     dots = dots[::-1, :]
-    alpha = float(-np.log(0.01) / np.mean(dots[0, :] - dots[1, :]))
+    # one cluster has no runner-up to set alpha by; its assignment is 1 whatever alpha is
+    alpha = float(-np.log(0.01) / np.mean(dots[0, :] - dots[1, :])) if num_clusters > 1 else 100.0
     conv_w = torch.from_numpy((alpha * assign).astype(np.float32)).reshape(num_clusters, dim, 1, 1)
     return {"centroids": torch.from_numpy(clsts_n.copy()), "conv_weight": conv_w, "alpha": alpha}
 
@@ -93,17 +94,18 @@ def make_pca_params(seed: int = 0, in_dim: int = 32768, out_dim: int = 4096):
 
 
 def make_state_dict(seed: int = 0, sharp: bool = False, with_pca: bool = True,
-                    pca_dim: int = 4096, bias_scale: float = 0.0):
+                    pca_dim: int = 4096, bias_scale: float = 0.0, num_clusters: int = 64):
     """Full EmbedNet / EmbedNetPCA state dict with the reference's key names
-    (SURVEY 8b: base_model.base.N.*, net_vlad.*, pca_layer.*)."""
+    (SURVEY 8b: base_model.base.N.*, net_vlad.*, pca_layer.*) for a NetVLAD layer of
+    `num_clusters` clusters; the PCA layer's input is num_clusters * 512."""
     sd = OrderedDict()
     for k, v in make_vgg_weights(seed, bias_scale).items():
         sd["base_model." + k] = v
-    nv = make_netvlad_params(seed, sharp=sharp)
+    nv = make_netvlad_params(seed, num_clusters=num_clusters, sharp=sharp)
     sd["net_vlad.centroids"] = nv["centroids"]
     sd["net_vlad.conv.weight"] = nv["conv_weight"]
     if with_pca:
-        p = make_pca_params(seed, 32768, pca_dim)
+        p = make_pca_params(seed, num_clusters * 512, pca_dim)
         sd["pca_layer.weight"] = p["weight"]
         sd["pca_layer.bias"] = p["bias"]
     return sd

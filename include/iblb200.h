@@ -185,7 +185,7 @@ int ibl_resize_bilinear_u8(ibl_engine* e, const uint8_t* x_nhwc, int N, int Hin,
 int ibl_extract_host_u8(ibl_engine* e, const uint8_t* x_nhwc_host, int N, int H, int W, const float* mean3,
                         const float* std3, unsigned flags, float* out_host, float* pool_host, void* stream);
 
-/* ---- input side: baseline JPEG decode on the GPU ------------------------------ */
+/* ---- input side: baseline and progressive JPEG decode on the GPU -------------- */
 /* What `Image.open(f).convert('RGB')` does in Preprocessor.__getitem__ (ibl/utils/data/preprocessor.py:31-42) for
  * baseline JPEGs, bit-identical to Pillow's libjpeg(-turbo) decode with its defaults: accurate integer IDCT
  * (JDCT_ISLOW), "fancy" triangular chroma upsampling, integer YCbCr->RGB.  Supported: SOF0/SOF1, 8-bit, Huffman, one
@@ -202,7 +202,8 @@ typedef struct ibl_jpeg_info {
   char reason[120];          /* why the file was rejected ("" when accepted) */
 } ibl_jpeg_info;
 /* Host-only parse of one in-memory file (no device, no engine): headers, Huffman and quantisation tables, restart
- * segmentation.  IBL_OK for a file ibl_jpeg_decode_u8 decodes; IBL_ERR_UNSUPPORTED for progressive, arithmetic,
+ * segmentation.  IBL_OK for a file ibl_jpeg_decode_u8 decodes; IBL_ERR_UNSUPPORTED (reason "progressive") for
+ * progressive files, which ibl_jpeg_parse_progressive / ibl_jpeg_decode_progressive_u8 take, and for arithmetic,
  * 12-bit, CMYK/YCCK, RGB-coded, other sampling, multi-scan, and for files that are cut short, have no EOI or carry a
  * bad segment length. */
 int ibl_jpeg_parse(const uint8_t* data, size_t len, ibl_jpeg_info* out);
@@ -215,6 +216,31 @@ int ibl_jpeg_parse(const uint8_t* data, size_t len, ibl_jpeg_info* out);
  * interval, so a corrupt stream never reads or writes out of bounds. */
 int ibl_jpeg_decode_u8(ibl_engine* e, const uint8_t* const* files, const size_t* lens, int N, uint8_t* out_u8,
                        const uint64_t* out_offsets, int* status, int* err_dev, void* stream);
+/* Progressive JPEGs (SOF2, 8-bit, Huffman), bit-identical to Pillow like the baseline decoder: the same components,
+ * sampling, DRI/RSTn and APPn/COM rules, any scan script libjpeg accepts without a warning (DC first / refinement,
+ * interleaved or not; AC first / refinement of one component; DHT and DRI between scans).  Rejected with a reason:
+ * jdphuff.c's progression range checks, an AC scan with more than one component or before the component's DC scan, a
+ * refinement whose Ah is not the previous Al, and files libjpeg would block-smooth (the DC or one of zig-zag
+ * coefficients 1..9 of a component not fully refined after the last scan).  ibl_jpeg_parse keeps rejecting progressive
+ * files; this parse rejects sequential ones. */
+typedef struct ibl_jpeg_scan {
+  int components;            /* components in the scan */
+  int comp[3];               /* their frame indices */
+  int ss, se, ah, al;        /* spectral band and successive-approximation bits */
+  int restart_interval;      /* DRI in force for the scan */
+  int intervals;             /* its entropy-coded segments */
+} ibl_jpeg_scan;
+/* Host-only parse of one progressive file.  `out` as ibl_jpeg_parse, with restart_interval the last one in force and
+ * intervals / entropy_bytes summed over the scans; *n_scans (if not null) is the number of scans, and the first
+ * max_scans of them are written to `scans` (may be null). */
+int ibl_jpeg_parse_progressive(const uint8_t* data, size_t len, ibl_jpeg_info* out, int* n_scans,
+                               ibl_jpeg_scan* scans, int max_scans);
+/* ibl_jpeg_decode_u8's contract for progressive files (status[i] is the ibl_jpeg_parse_progressive result).  Every
+ * scan of every image is decoded on the device, the scans of one image in file order; err_dev[i] becomes nonzero for
+ * an invalid Huffman code, a restart interval that ends before its last block, or an end-of-band run past its end. */
+int ibl_jpeg_decode_progressive_u8(ibl_engine* e, const uint8_t* const* files, const size_t* lens, int N,
+                                   uint8_t* out_u8, const uint64_t* out_offsets, int* status, int* err_dev,
+                                   void* stream);
 
 /* ---- input side: the training transform's colour jitter on the GPU ------------ */
 /* T.ColorJitter(0.7, 0.7, 0.7, 0.5), the first step of the reference's training transform

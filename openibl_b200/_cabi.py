@@ -27,6 +27,12 @@ class JpegInfo(Structure):
                 ("reason", c_char * 120)]
 
 
+class JpegScan(Structure):
+    """ibl_jpeg_scan (include/iblb200.h)."""
+    _fields_ = [("components", c_int), ("comp", c_int * 3), ("ss", c_int), ("se", c_int), ("ah", c_int), ("al", c_int),
+                ("restart_interval", c_int), ("intervals", c_int)]
+
+
 class ColorJitterParams(Structure):
     """ibl_color_jitter_params (include/iblb200.h)."""
     _fields_ = [("order", c_int * 4), ("brightness", c_float), ("contrast", c_float), ("saturation", c_float),
@@ -67,6 +73,9 @@ SIGNATURES = {
     "ibl_extract_host_u8": (c_int, [_P, _P, c_int, c_int, c_int, _P, _P, c_uint, _P, _P, _P]),
     "ibl_jpeg_parse": (c_int, [c_char_p, c_size_t, POINTER(JpegInfo)]),
     "ibl_jpeg_decode_u8": (c_int, [_P, _P, _P, c_int, _P, _P, _P, _P, _P]),
+    "ibl_jpeg_parse_progressive": (c_int, [c_char_p, c_size_t, POINTER(JpegInfo), POINTER(c_int), POINTER(JpegScan),
+                                           c_int]),
+    "ibl_jpeg_decode_progressive_u8": (c_int, [_P, _P, _P, c_int, _P, _P, _P, _P, _P]),
     "ibl_color_jitter_u8": (c_int, [_P, _P, _P, _P, _P, POINTER(ColorJitterParams), c_int, _P]),
     "ibl_l2dist_dense": (c_int, [_P, _P, c_int, _P, c_int, c_int, _P, _P]),
     "ibl_l2dist_self": (c_int, [_P, _P, c_int, c_int, _P, _P]),
@@ -132,6 +141,26 @@ def jpeg_parse(data: bytes) -> dict:
             "components": info.components, "h_samp": info.h_samp, "v_samp": info.v_samp,
             "restart_interval": info.restart_interval, "intervals": info.intervals, "mcus": info.mcus,
             "entropy_bytes": info.entropy_bytes, "reason": info.reason.decode()}
+
+
+def jpeg_parse_progressive(data: bytes) -> dict:
+    """ibl_jpeg_parse_progressive on one in-memory file (host only): jpeg_parse's fields plus `scans`, the scan
+    script as a list of dicts (components, ss, se, ah, al, restart_interval, intervals)."""
+    lib = load()
+    info = JpegInfo()
+    data = bytes(data)
+    n = c_int(0)
+    st = lib.ibl_jpeg_parse_progressive(data, len(data), ctypes.byref(info), ctypes.byref(n), None, 0)
+    scans = (JpegScan * max(n.value, 1))()
+    if n.value:
+        lib.ibl_jpeg_parse_progressive(data, len(data), ctypes.byref(info), ctypes.byref(n), scans, n.value)
+    return {"ok": st == IBL_OK, "status": st, "width": info.width, "height": info.height,
+            "components": info.components, "h_samp": info.h_samp, "v_samp": info.v_samp,
+            "restart_interval": info.restart_interval, "intervals": info.intervals, "mcus": info.mcus,
+            "entropy_bytes": info.entropy_bytes, "reason": info.reason.decode(),
+            "scans": [{"components": tuple(s.comp[:s.components]), "ss": s.ss, "se": s.se, "ah": s.ah, "al": s.al,
+                       "restart_interval": s.restart_interval, "intervals": s.intervals}
+                      for s in scans[:n.value]]}
 
 
 def check(status: int, where: str) -> None:

@@ -125,11 +125,14 @@ int launch_argsort_rows(const float* dist, long long ld, int m, int n, long long
 int launch_resize_bilinear_u8(const uint8_t* x, int N, int Hin, int Win, int Hout, int Wout, const int* bounds_h,
                               const int* kk_h, int ksize_h, const int* bounds_v, const int* kk_v, int ksize_v,
                               uint8_t* tmp, uint8_t* out, cudaStream_t s, uint64_t* launches);
-// jpeg.cu  (baseline JPEG decode, bit-exact with libjpeg's defaults; the parser is host code)
+// jpeg.cu  (baseline and progressive JPEG decode, bit-exact with libjpeg's defaults; the parser is host code)
 struct JpegWs;   // opaque per-engine workspace: pinned staging blob, device tables, coefficients, planes
 void jpeg_ws_destroy(JpegWs* ws);
 int jpeg_decode_u8(JpegWs** ws, const uint8_t* const* files, const size_t* lens, int N, uint8_t* out_u8,
                    const uint64_t* out_offsets, int* status, int* err_dev, cudaStream_t s, uint64_t* launches);
+int jpeg_decode_progressive_u8(JpegWs** ws, const uint8_t* const* files, const size_t* lens, int N, uint8_t* out_u8,
+                               const uint64_t* out_offsets, int* status, int* err_dev, cudaStream_t s,
+                               uint64_t* launches);
 // color_jitter.cu  (T.ColorJitter, bit-exact with torchvision's PIL path)
 struct JitterWs;   // opaque per-engine workspace: pinned staging of descriptors, device copy, L sums
 void jitter_ws_destroy(JitterWs* ws);

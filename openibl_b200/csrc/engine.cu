@@ -85,6 +85,7 @@ struct ibl_engine {
   DevBuf knn_ws;                         // neighbour pass of the re-ranking (rerank.cu)
   const int* knn_flag_counter = nullptr; // its count of rows sent to the exact scan (null: no call yet)
   JpegWs* jpeg_ws = nullptr;             // JPEG decode: pinned staging blob, tables, coefficients, planes (jpeg.cu)
+  JpegWs* jpeg_prog_ws = nullptr;        // the same for progressive JPEGs
   JitterWs* jitter_ws = nullptr;         // colour jitter: pinned staging of per-image descriptors, L sums (color_jitter.cu)
   RerankWs* rr_ws = nullptr;             // sparse stage of the re-ranking: CSR matrices, inverted index, pair buffers
   const int* flag_counter = nullptr;     // guard counter of the last ibl_l2dist_topk call (null: no guard on its path)
@@ -280,6 +281,7 @@ int ibl_engine_destroy(ibl_engine* e) {
   e->knn_ws.release();
   rerank_ws_destroy(e->rr_ws);
   jpeg_ws_destroy(e->jpeg_ws);
+  jpeg_ws_destroy(e->jpeg_prog_ws);
   jitter_ws_destroy(e->jitter_ws);
   delete e;
   return IBL_OK;
@@ -819,6 +821,17 @@ int ibl_jpeg_decode_u8(ibl_engine* e, const uint8_t* const* files, const size_t*
   IBL_REQUIRE(N >= 1, "empty batch");
   DeviceGuard g(e->device);
   return jpeg_decode_u8(&e->jpeg_ws, files, lens, N, out_u8, out_offsets, status, err_dev, S(stream), &e->launches);
+}
+
+// The same for progressive JPEGs (SOF2), whose scans the device decodes one at a time per image (jpeg.cu).
+int ibl_jpeg_decode_progressive_u8(ibl_engine* e, const uint8_t* const* files, const size_t* lens, int N,
+                                   uint8_t* out_u8, const uint64_t* out_offsets, int* status, int* err_dev,
+                                   void* stream) {
+  IBL_REQUIRE(e && files && lens && out_offsets && status && err_dev, "null argument");
+  IBL_REQUIRE(N >= 1, "empty batch");
+  DeviceGuard g(e->device);
+  return jpeg_decode_progressive_u8(&e->jpeg_prog_ws, files, lens, N, out_u8, out_offsets, status, err_dev, S(stream),
+                                    &e->launches);
 }
 
 // T.ColorJitter of the reference's training transform (ibl/utils/data/__init__.py:29-35) on decoded uint8 HWC images,

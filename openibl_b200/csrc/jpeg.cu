@@ -30,6 +30,10 @@
 //   6. jpeg_color_kernel    fancy upsampling (h2v1 / h2v2, edge replication) + YCbCr->RGB, uint8 HWC out.
 // Every bit fetch reads at most 5 bytes from a position inside its interval, and every interval is followed by 8 zero
 // bytes in the staging buffer: no input, however corrupt, reads or writes outside the buffers.
+//
+// Progressive files (SOF2): `parse_jpeg(..., progressive=true)` records the scan script, and the jpeg_prog_*_kernel
+// family decodes the scans of every image in file order into the same coefficient buffer (frame MCU order), after
+// which steps 5 and 6 run unchanged.
 #include <string.h>
 
 #include <algorithm>
@@ -50,6 +54,7 @@ constexpr int kFixThreads = 512;
 constexpr int kDcThreads = 256;
 constexpr uint64_t kInvalid = 1ull << 63;
 constexpr int kPad = 8;               // zero bytes after every interval
+constexpr int kProgWarps = 4;         // warps per block of the sequential progressive scan kernels
 
 // jpeg_natural_order (jutils.c): zig-zag index -> natural (row-major) index
 __constant__ uint8_t c_natural[64] = {
@@ -475,7 +480,269 @@ __global__ void jpeg_color_kernel(Batch b) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// progressive scans (jdphuff.c), into the same natural-order [blocks][64] buffer in frame MCU order
+
+enum ScanKind { kDcFirst = 0, kDcRefine = 1, kAcFirst = 2, kAcRefine = 3 };
+
+struct ScanDev {
+  int img;                          // ImgDev index
+  int ncomp;                        // components in the scan; 1 = non-interleaved (one block per MCU)
+  int ss, se, al;
+  int bpm;                          // blocks per scan MCU
+  int mcus_x;                       // scan MCUs per row (the component's width in blocks when non-interleaved)
+  int hs, vs, comp_first;           // non-interleaved: the component's sampling and first block in the frame MCU
+  int8_t blk_slot[6];               // interleaved: scan component (table, DC predictor) of every block of the MCU
+  int8_t blk_off[6];                // interleaved: the block's index within the frame MCU
+};
+
+struct ProgIvDev {
+  uint64_t byte_base;               // first byte in the entropy arena
+  uint32_t nbits;
+  int scan;                         // ScanDev index; its Huffman tables are tabs[3 * scan + slot]
+  int first_mcu, n_mcus;
+};
+
+struct ProgBatch {
+  const ImgDev* img;
+  const ScanDev* scan;
+  const ProgIvDev* iv;
+  const HuffTab* tabs;
+  const uint8_t* bytes;
+  int16_t* coef;
+  int* err;
+  const int* err_slot;
+};
+
+// frame block (MCU order, the layout jpeg_idct_kernel reads) of block k of scan MCU m
+__device__ inline uint64_t frame_block(const ImgDev& im, const ScanDev& sc, int m, int k) {
+  if (sc.ncomp > 1) return (uint64_t)m * im.bpm + sc.blk_off[k];
+  const int by = m / sc.mcus_x, bx = m - by * sc.mcus_x;
+  return (uint64_t)((by / sc.vs) * im.mcus_x + bx / sc.hs) * im.bpm + sc.comp_first + (by % sc.vs) * sc.hs + bx % sc.hs;
+}
+
+__device__ inline void prog_error(const ProgBatch& b, const ScanDev& sc, int code) {
+  atomicOr(b.err + b.err_slot[sc.img], code);
+}
+
+// The sequential scan kernels give every interval a warp of its own and decode it on lane 0: intervals of different
+// images or scans follow different paths, and one warp each keeps them from serialising each other.
+//
+// Error codes (the image's error word): 1 an invalid Huffman code, 2 an interval that ends before its last block, 4
+// an EOBRUN that runs past the end of its interval.  Every read starts below the interval's last bit, so it fetches at
+// most 4 bytes past it, inside the 8 zero bytes that follow every interval.
+
+// DC first (decode_mcu_DC_first): one thread per interval, the DC difference prefix-summed per scan component from the
+// interval's start, stored as (JCOEF)(sum << Al).
+__device__ int dc_first(const ProgBatch& b, const ProgIvDev& iv) {
+  const ScanDev& sc = b.scan[iv.scan];
+  const ImgDev& im = b.img[sc.img];
+  const HuffTab* tabs = b.tabs + 3 * iv.scan;
+  const uint8_t* d = b.bytes + iv.byte_base;
+  int16_t* coef = b.coef + im.coef_block * 64;
+  int last[3] = {0, 0, 0};
+  uint32_t pos = 0;
+  for (int m = iv.first_mcu; m < iv.first_mcu + iv.n_mcus; ++m)
+    for (int k = 0; k < sc.bpm; ++k) {
+      if (pos >= iv.nbits) return 2;
+      const uint32_t bits = peek32(d, pos);
+      const int slot = sc.ncomp > 1 ? sc.blk_slot[k] : 0;
+      int len;
+      const int s = huff_decode(tabs[slot], bits, &len);
+      if (s < 0) return 1;
+      last[slot] += s ? extend((bits << len) >> (32 - s), s) : 0;
+      pos += len + s;
+      coef[frame_block(im, sc, m, k) * 64] = (int16_t)((uint32_t)last[slot] << sc.al);
+    }
+  return 0;
+}
+
+__global__ void jpeg_prog_dc_first_kernel(ProgBatch b, int i0, int i1) {
+  const int i = i0 + (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+  if (i >= i1 || (threadIdx.x & 31)) return;
+  const ProgIvDev iv = b.iv[i];
+  if (const int e = dc_first(b, iv)) prog_error(b, b.scan[iv.scan], e);
+}
+
+// DC refinement (decode_mcu_DC_refine): block t of an interval is its bit t, OR-ed in as 1 << Al.  One CUDA block per
+// interval, fully parallel.
+__global__ void jpeg_prog_dc_refine_kernel(ProgBatch b, int i0) {
+  const ProgIvDev iv = b.iv[i0 + blockIdx.x];
+  const ScanDev& sc = b.scan[iv.scan];
+  const ImgDev& im = b.img[sc.img];
+  const uint8_t* d = b.bytes + iv.byte_base;
+  int16_t* coef = b.coef + im.coef_block * 64;
+  const long long nb = (long long)iv.n_mcus * sc.bpm;
+  if (threadIdx.x == 0 && nb > (long long)iv.nbits) prog_error(b, sc, 2);
+  const int p1 = 1 << sc.al;
+  for (long long t = threadIdx.x; t < nb && t < (long long)iv.nbits; t += blockDim.x) {
+    if (!((d[t >> 3] >> (7 - (t & 7))) & 1)) continue;
+    const int m = iv.first_mcu + (int)(t / sc.bpm), k = (int)(t % sc.bpm);
+    int16_t& c = coef[frame_block(im, sc, m, k) * 64];
+    c = (int16_t)(c | p1);
+  }
+}
+
+// AC first (decode_mcu_AC_first): one thread per interval, single component, EOBRUN carried across blocks and reset
+// at the interval's start.
+__device__ int ac_first(const ProgBatch& b, const ProgIvDev& iv) {
+  const ScanDev& sc = b.scan[iv.scan];
+  const ImgDev& im = b.img[sc.img];
+  const HuffTab& tab = b.tabs[3 * iv.scan];
+  const uint8_t* d = b.bytes + iv.byte_base;
+  int16_t* coef = b.coef + im.coef_block * 64;
+  uint32_t pos = 0;
+  int eobrun = 0;
+  for (int m = iv.first_mcu; m < iv.first_mcu + iv.n_mcus; ++m) {
+    if (eobrun > 0) {
+      --eobrun;
+      continue;
+    }
+    int16_t* blk = coef + frame_block(im, sc, m, 0) * 64;
+    for (int k = sc.ss; k <= sc.se; ++k) {
+      if (pos >= iv.nbits) return 2;
+      const uint32_t bits = peek32(d, pos);
+      int len;
+      const int rs = huff_decode(tab, bits, &len);
+      if (rs < 0) return 1;
+      const int r = rs >> 4, s = rs & 15;
+      if (s) {
+        k += r;
+        blk[c_natural[k < 63 ? k : 63]] = (int16_t)((uint32_t)extend((bits << len) >> (32 - s), s) << sc.al);
+        pos += len + s;
+      } else if (r == 15) {
+        k += 15;
+        pos += len;
+      } else {
+        eobrun = (1 << r) + (r ? (int)((bits << len) >> (32 - r)) : 0) - 1;
+        pos += len + r;
+        break;
+      }
+    }
+  }
+  return eobrun > 0 ? 4 : 0;
+}
+
+__global__ void jpeg_prog_ac_first_kernel(ProgBatch b, int i0, int i1) {
+  const int i = i0 + (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+  if (i >= i1 || (threadIdx.x & 31)) return;
+  const ProgIvDev iv = b.iv[i];
+  if (const int e = ac_first(b, iv)) prog_error(b, b.scan[iv.scan], e);
+}
+
+// AC refinement (decode_mcu_AC_refine): how many bits a block takes depends on which of its coefficients are already
+// nonzero, so each interval is decoded sequentially by one thread.  A 64-bit zig-zag mask of the block's nonzero
+// coefficients replaces libjpeg's coefficient-by-coefficient walk: the r zeros a symbol skips and the correction bits
+// of the nonzero coefficients passed on the way are found with bit operations, and only those coefficients are read.
+__device__ int ac_refine(const ProgBatch& b, const ProgIvDev& iv) {
+  const ScanDev& sc = b.scan[iv.scan];
+  const ImgDev& im = b.img[sc.img];
+  const HuffTab& tab = b.tabs[3 * iv.scan];
+  const uint8_t* d = b.bytes + iv.byte_base;
+  int16_t* coef = b.coef + im.coef_block * 64;
+  const int p1 = 1 << sc.al, m1 = -p1;
+  const uint64_t band = (sc.se == 63 ? ~0ull : (1ull << (sc.se + 1)) - 1) & (~0ull << sc.ss);
+  uint32_t pos = 0;
+  int eobrun = 0;
+  alignas(16) int16_t blk[64];
+  // one correction bit, in stream order, for every (nonzero) coefficient of `sel`; false when the interval runs out
+  auto correct = [&](uint64_t sel) {
+    if ((uint64_t)pos + __popcll(sel) > iv.nbits) return false;
+    uint32_t word = 0;
+    int avail = 0;
+    for (; sel; sel &= sel - 1) {
+      if (avail == 0) {
+        word = peek32(d, pos);
+        avail = 32;
+      }
+      if (word >> 31) {
+        int16_t& c = blk[c_natural[__ffsll(sel) - 1]];
+        if ((c & p1) == 0) c = (int16_t)(c + (c >= 0 ? p1 : m1));
+      }
+      word <<= 1;
+      --avail;
+      ++pos;
+    }
+    return true;
+  };
+  for (int m = iv.first_mcu; m < iv.first_mcu + iv.n_mcus; ++m) {
+    int4* g = reinterpret_cast<int4*>(coef + frame_block(im, sc, m, 0) * 64);
+    uint64_t nat = 0;                                // nonzero coefficients, natural order
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+      const int4 v = g[q];
+      reinterpret_cast<int4*>(blk)[q] = v;
+      const uint32_t w[4] = {(uint32_t)v.x, (uint32_t)v.y, (uint32_t)v.z, (uint32_t)v.w};
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+        nat |= (uint64_t)((w[j] & 0xFFFFu) != 0) << (8 * q + 2 * j) | (uint64_t)((w[j] >> 16) != 0) << (8 * q + 2 * j + 1);
+    }
+    uint64_t nz = 0;                                 // the same in zig-zag order
+#pragma unroll
+    for (int k = 0; k < 64; ++k) nz |= ((nat >> c_natural[k]) & 1ull) << k;
+    int k = sc.ss;
+    if (eobrun == 0) {
+      for (; k <= sc.se; ++k) {
+        if (pos >= iv.nbits) return 2;
+        const uint32_t bits = peek32(d, pos);
+        int len;
+        const int rs = huff_decode(tab, bits, &len);
+        if (rs < 0 || (rs & 15) > 1) return 1;     // a new coefficient always has size 1
+        const int r = rs >> 4;
+        int s = 0;
+        pos += len;
+        if (rs & 15) {
+          if (pos >= iv.nbits) return 2;
+          s = (bits << len) >> 31 ? p1 : m1;
+          ++pos;
+        } else if (r != 15) {
+          eobrun = (1 << r) + (r ? (int)((bits << len) >> (32 - r)) : 0);
+          pos += r;
+          break;
+        }
+        // skip r still-zero coefficients of the band, stop on the next one (or run off the band's end), and
+        // append a correction bit to every nonzero coefficient passed
+        const uint64_t from = band & (~0ull << k);
+        uint64_t zeros = ~nz & from;
+        for (int i = 0; i < r && zeros; ++i) zeros &= zeros - 1;
+        const int t = zeros ? __ffsll(zeros) - 1 : sc.se + 1;
+        if (!correct(nz & from & (t < 64 ? (1ull << t) - 1 : ~0ull))) return 2;
+        k = t;
+        if (s) {
+          blk[c_natural[k < 63 ? k : 63]] = (int16_t)s;
+          if (k < 64) nz |= 1ull << k;
+        }
+      }
+    }
+    if (eobrun > 0) {                                // the rest of the band of a block inside an EOB run
+      if (k <= sc.se && !correct(nz & band & (~0ull << k))) return 2;
+      --eobrun;
+    }
+#pragma unroll
+    for (int q = 0; q < 8; ++q) g[q] = reinterpret_cast<int4*>(blk)[q];
+  }
+  return eobrun > 0 ? 4 : 0;
+}
+
+__global__ void jpeg_prog_ac_refine_kernel(ProgBatch b, int i0, int i1) {
+  const int i = i0 + (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+  if (i >= i1 || (threadIdx.x & 31)) return;
+  const ProgIvDev iv = b.iv[i];
+  if (const int e = ac_refine(b, iv)) prog_error(b, b.scan[iv.scan], e);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // host parser
+
+// one scan of a progressive file, as the decoder needs it after the whole file has been read
+struct ScanInfo {
+  int ncomp = 0;
+  int comp[3] = {0, 0, 0};           // frame component indices, in frame order
+  int ss = 0, se = 0, ah = 0, al = 0;
+  int restart = 0;                   // DRI in force for this scan
+  int mcus = 0;                      // MCUs of the scan (blocks of the component for a single-component scan)
+  int first_iv = 0, n_iv = 0;        // its intervals in iv_start
+  HuffTab tab[3];                    // per scan component: DC table (DC first) or AC table (AC scans)
+};
 
 struct Parsed {
   ibl_jpeg_info info;
@@ -488,8 +755,14 @@ struct Parsed {
   bool dc_def[4] = {false, false, false, false}, ac_def[4] = {false, false, false, false};
   int restart = 0;
   int mcus_x = 0, mcus_y = 0;
-  std::vector<uint8_t> entropy;      // destuffed, intervals back to back
+  std::vector<uint8_t> entropy;      // destuffed, intervals back to back (all scans, in file order)
   std::vector<uint64_t> iv_start;    // first byte of every interval; entropy.size() closes the last
+  // progressive only
+  std::vector<ScanInfo> scans;
+  uint16_t comp_q[3][64];            // quantisation table latched at the component's first scan (jdinput.c)
+  bool comp_q_set[3] = {false, false, false};
+  int coef_bits[3][64];              // libjpeg's coef_bits: -1 never coded, else the Al of the last scan coding it
+  int width_blocks[3] = {0, 0, 0}, height_blocks[3] = {0, 0, 0};   // compptr->width_in_blocks / height_in_blocks
 };
 
 int reject(Parsed& p, const char* why) {
@@ -546,12 +819,90 @@ bool build_huff(const uint8_t* counts, const uint8_t* vals, int nvals, bool is_d
   return true;
 }
 
-int parse_jpeg(const uint8_t* d, size_t n, Parsed& p) {
+// Entropy-coded data of one scan starting at d[j]: destuff, split at RSTn (numbered from 0 in every scan), stop at
+// the next other marker.  Appends the scan's intervals to p.entropy / p.iv_start and leaves j on that marker.
+int read_entropy(const uint8_t* d, size_t n, size_t& j, Parsed& p) {
+  const size_t first_iv = p.iv_start.size();
+  p.iv_start.push_back(p.entropy.size());
+  for (;;) {
+    if (j >= n) return reject(p, "truncated or missing EOI marker: file ends inside the entropy-coded data");
+    const uint8_t c = d[j];
+    if (c != 0xFF) {
+      p.entropy.push_back(c);
+      ++j;
+      continue;
+    }
+    if (j + 1 >= n) return reject(p, "truncated or missing EOI marker: file ends inside the entropy-coded data");
+    const uint8_t c2 = d[j + 1];
+    if (c2 == 0x00) {
+      p.entropy.push_back(0xFF);
+      j += 2;
+    } else if (c2 == 0xFF) {
+      ++j;                                        // fill byte before a marker
+    } else if (c2 >= 0xD0 && c2 <= 0xD7) {
+      if (c2 - 0xD0 != (int)((p.iv_start.size() - 1 - first_iv) & 7))
+        return reject(p, "restart marker out of sequence");
+      p.iv_start.push_back(p.entropy.size());
+      j += 2;
+    } else {
+      return IBL_OK;
+    }
+  }
+}
+
+// Progressive scan header after the component list (jdphuff.c start_pass_phuff_decoder): its range checks, which
+// libjpeg errors on, and the coef_bits bookkeeping whose JWRN_BOGUS_PROGRESSION warnings are rejected here too.
+int progressive_scan(Parsed& p, ScanInfo& sc, const uint8_t* ssz) {
+  sc.ss = ssz[0];
+  sc.se = ssz[1];
+  sc.ah = ssz[2] >> 4;
+  sc.al = ssz[2] & 15;
+  if (sc.ss == 0) {
+    if (sc.se != 0) return reject(p, "bad progression: DC scan with Se != 0");
+  } else {
+    if (sc.ss > sc.se || sc.se > 63) return reject(p, "bad progression: spectral band out of range");
+    if (sc.ncomp != 1) return reject(p, "bad progression: AC scan with more than one component");
+  }
+  if (sc.ah != 0 && sc.al != sc.ah - 1) return reject(p, "bad progression: refinement with Al != Ah - 1");
+  if (sc.al > 13) return reject(p, "bad progression: Al > 13");
+  for (int i = 0; i < sc.ncomp; ++i) {
+    int* cb = p.coef_bits[sc.comp[i]];
+    if (sc.ss > 0 && cb[0] < 0) return reject(p, "bogus progression: AC scan before the component's DC scan");
+    for (int k = sc.ss; k <= sc.se; ++k) {
+      if (sc.ah != (cb[k] < 0 ? 0 : cb[k])) return reject(p, "bogus progression: Ah differs from the previous Al");
+      cb[k] = sc.al;
+    }
+  }
+  for (int i = 0; i < sc.ncomp; ++i) {
+    const int c = sc.comp[i];
+    if (sc.ss == 0 && sc.ah == 0) {
+      if (!p.dc_def[p.td[c]]) return reject(p, "missing Huffman table");
+      sc.tab[i] = p.dc[p.td[c]];                     // snapshot: DHT may redefine it before a later scan
+    } else if (sc.ss > 0) {
+      if (!p.ac_def[p.ta[c]]) return reject(p, "missing Huffman table");
+      sc.tab[i] = p.ac[p.ta[c]];
+    }
+    if (!p.comp_q_set[c]) {                          // jdinput.c latch_quant_tables
+      if (!p.qt_def[p.tq[c]]) return reject(p, "missing quantisation table");
+      memcpy(p.comp_q[c], p.qt[p.tq[c]], sizeof(p.comp_q[c]));
+      p.comp_q_set[c] = true;
+    }
+  }
+  return IBL_OK;
+}
+
+// Baseline (SOF0/SOF1, one interleaved scan) or, with `progressive`, progressive Huffman (SOF2, any valid scan
+// script).  Both share the marker reader, the Huffman table derivation, the component and sampling rules and the
+// destuffing; each rejects the other kind.
+int parse_jpeg(const uint8_t* d, size_t n, Parsed& p, bool progressive = false) {
   memset(&p.info, 0, sizeof(p.info));
   if (!d || n < 4 || d[0] != 0xFF || d[1] != 0xD8) return reject(p, "not a JPEG file (no SOI marker)");
   size_t i = 2;
   bool sof = false, sos = false, jfif = false, adobe = false;
   int adobe_transform = -1, width = 0, height = 0;
+  if (progressive)
+    for (int c = 0; c < 3; ++c)
+      for (int k = 0; k < 64; ++k) p.coef_bits[c][k] = -1;
   for (;;) {
     if (i >= n) return reject(p, sos ? "missing EOI marker" : "truncated: file ends before the scan");
     if (d[i] != 0xFF) return reject(p, "extraneous bytes between segments");
@@ -574,7 +925,10 @@ int parse_jpeg(const uint8_t* d, size_t n, Parsed& p) {
       return reject(p, "unsupported marker after the scan");
     switch (m) {
       case 0xC0:
-      case 0xC1: {
+      case 0xC1:
+      case 0xC2: {
+        if (m == 0xC2 && !progressive) return reject(p, "progressive");
+        if (m != 0xC2 && progressive) return reject(p, "sequential (not progressive)");
         if (sof) return reject(p, "more than one frame");
         if (sl < 6) return reject(p, "bad segment length");
         if (seg[0] != 8) return reject(p, "12-bit (not 8-bit) samples");
@@ -598,7 +952,7 @@ int parse_jpeg(const uint8_t* d, size_t n, Parsed& p) {
         sof = true;
         break;
       }
-      case 0xC2: case 0xC6: return reject(p, "progressive");
+      case 0xC6: return reject(p, "progressive");
       case 0xC3: case 0xC7: return reject(p, "lossless");
       case 0xC5: case 0xDE: case 0xDF: return reject(p, "hierarchical");
       case 0xC9: case 0xCA: case 0xCB: case 0xCD: case 0xCE: case 0xCF: case 0xCC:
@@ -638,25 +992,39 @@ int parse_jpeg(const uint8_t* d, size_t n, Parsed& p) {
         break;
       case 0xDA: {
         if (!sof) return reject(p, "scan before the frame header");
-        if (sos) return reject(p, "multi-scan");
+        if (sos && !progressive) return reject(p, "multi-scan");
         if (sl < 1) return reject(p, "bad segment length");
         const int ns = seg[0];
         if (sl != 4 + 2 * (size_t)ns) return reject(p, "bad segment length");
-        if (ns != p.ncomp) return reject(p, "multi-scan (components in separate scans)");
-        for (int c = 0; c < ns; ++c) {
-          if (seg[1 + 2 * c] != p.comp_id[c]) return reject(p, "scan component order differs from the frame");
-          p.td[c] = seg[2 + 2 * c] >> 4;
-          p.ta[c] = seg[2 + 2 * c] & 15;
-          if (p.td[c] > 3 || p.ta[c] > 3) return reject(p, "bad scan header");
-        }
-        const uint8_t* ssz = seg + 1 + 2 * ns;
-        if (ssz[0] != 0 || ssz[1] != 63 || ssz[2] != 0) return reject(p, "not a sequential scan");
-        for (int c = 0; c < ns; ++c) {
-          if (!p.qt_def[p.tq[c]]) return reject(p, "missing quantisation table");
-          if (!p.dc_def[p.td[c]] || !p.ac_def[p.ta[c]]) return reject(p, "missing Huffman table");
+        ScanInfo sc;
+        if (!progressive) {
+          if (ns != p.ncomp) return reject(p, "multi-scan (components in separate scans)");
+          for (int c = 0; c < ns; ++c) {
+            if (seg[1 + 2 * c] != p.comp_id[c]) return reject(p, "scan component order differs from the frame");
+            p.td[c] = seg[2 + 2 * c] >> 4;
+            p.ta[c] = seg[2 + 2 * c] & 15;
+            if (p.td[c] > 3 || p.ta[c] > 3) return reject(p, "bad scan header");
+          }
+          const uint8_t* ssz = seg + 1 + 2 * ns;
+          if (ssz[0] != 0 || ssz[1] != 63 || ssz[2] != 0) return reject(p, "not a sequential scan");
+          for (int c = 0; c < ns; ++c) {
+            if (!p.qt_def[p.tq[c]]) return reject(p, "missing quantisation table");
+            if (!p.dc_def[p.td[c]] || !p.ac_def[p.ta[c]]) return reject(p, "missing Huffman table");
+          }
+        } else {
+          if (ns < 1 || ns > p.ncomp) return reject(p, "bad scan header");
+          sc.ncomp = ns;
+          for (int s = 0, c = 0; s < ns; ++s, ++c) {
+            while (c < p.ncomp && p.comp_id[c] != seg[1 + 2 * s]) ++c;
+            if (c == p.ncomp) return reject(p, "scan component order differs from the frame");
+            sc.comp[s] = c;
+            p.td[c] = seg[2 + 2 * s] >> 4;
+            p.ta[c] = seg[2 + 2 * s] & 15;
+            if (p.td[c] > 3 || p.ta[c] > 3) return reject(p, "bad scan header");
+          }
         }
         // colour space as libjpeg decides it (jdapimin.c default_decompress_parms)
-        if (p.ncomp == 3) {
+        if (!sos && p.ncomp == 3) {
           bool rgb = false;
           if (jfif) rgb = false;
           else if (adobe) rgb = adobe_transform == 0;
@@ -668,43 +1036,38 @@ int parse_jpeg(const uint8_t* d, size_t n, Parsed& p) {
           if (!chroma11 || !luma_ok) return reject(p, "sampling other than 4:4:4, 4:2:2 or 4:2:0");
           p.mcus_x = (width + 8 * p.hs[0] - 1) / (8 * p.hs[0]);
           p.mcus_y = (height + 8 * p.vs[0] - 1) / (8 * p.vs[0]);
-        } else {
+        } else if (!sos) {
           p.hs[0] = p.vs[0] = 1;                       // one component: one block per MCU whatever its factors
           p.mcus_x = (width + 7) / 8;
           p.mcus_y = (height + 7) / 8;
         }
-        // entropy-coded data: destuff, split at RSTn, stop at the next other marker
-        p.entropy.clear();
-        p.entropy.reserve(n - i);
-        p.iv_start.assign(1, 0);
-        size_t j = i;
-        for (;;) {
-          if (j >= n) return reject(p, "truncated or missing EOI marker: file ends inside the entropy-coded data");
-          const uint8_t c = d[j];
-          if (c != 0xFF) {
-            p.entropy.push_back(c);
-            ++j;
-            continue;
-          }
-          if (j + 1 >= n) return reject(p, "truncated or missing EOI marker: file ends inside the entropy-coded data");
-          const uint8_t c2 = d[j + 1];
-          if (c2 == 0x00) {
-            p.entropy.push_back(0xFF);
-            j += 2;
-          } else if (c2 == 0xFF) {
-            ++j;                                        // fill byte before a marker
-          } else if (c2 >= 0xD0 && c2 <= 0xD7) {
-            if (c2 - 0xD0 != (int)((p.iv_start.size() - 1) & 7)) return reject(p, "restart marker out of sequence");
-            p.iv_start.push_back(p.entropy.size());
-            j += 2;
-          } else {
-            break;
-          }
+        long long mcus = (long long)p.mcus_x * p.mcus_y;
+        if (progressive) {
+          if (!sos)
+            for (int c = 0; c < p.ncomp; ++c) {        // jdinput.c initial_setup: ceil(size * samp / (max_samp * 8))
+              p.width_blocks[c] = (int)(((long long)width * p.hs[c] + 8 * p.hs[0] - 1) / (8 * p.hs[0]));
+              p.height_blocks[c] = (int)(((long long)height * p.vs[c] + 8 * p.vs[0] - 1) / (8 * p.vs[0]));
+            }
+          IBL_RET(progressive_scan(p, sc, seg + 1 + 2 * ns));
+          if (ns == 1) mcus = (long long)p.width_blocks[sc.comp[0]] * p.height_blocks[sc.comp[0]];
+          sc.restart = p.restart;
+          sc.mcus = (int)mcus;
+          sc.first_iv = (int)p.iv_start.size();
+        } else {
+          p.entropy.clear();
+          p.iv_start.clear();
         }
+        if (!sos) p.entropy.reserve(n - i);
+        size_t j = i;
+        IBL_RET(read_entropy(d, n, j, p));
         i = j;
-        const long long mcus = (long long)p.mcus_x * p.mcus_y;
+        const long long n_iv = (long long)p.iv_start.size() - sc.first_iv;
         const long long want = p.restart ? (mcus + p.restart - 1) / p.restart : 1;
-        if ((long long)p.iv_start.size() != want) return reject(p, "restart markers do not match the restart interval");
+        if (n_iv != want) return reject(p, "restart markers do not match the restart interval");
+        if (progressive) {
+          sc.n_iv = (int)n_iv;
+          p.scans.push_back(sc);
+        }
         sos = true;
         break;
       }
@@ -733,6 +1096,12 @@ int parse_jpeg(const uint8_t* d, size_t n, Parsed& p) {
   p.info.intervals = (int)p.iv_start.size();
   p.info.mcus = p.mcus_x * p.mcus_y;
   p.info.entropy_bytes = p.entropy.size();
+  // jdcoefct.c smoothing_ok: libjpeg smooths the blocks of a progressive file when the DC or one of the first nine
+  // AC coefficients (SAVED_COEFS) of a component is not fully refined after the last scan; such files stay on the host
+  if (progressive)
+    for (int c = 0; c < p.ncomp; ++c)
+      for (int k = 0; k < 10; ++k)
+        if (p.coef_bits[c][k] != 0) return reject(p, "block smoothing (a low-frequency coefficient not fully refined)");
   return IBL_OK;
 }
 
@@ -776,13 +1145,72 @@ static int grow_device(void** p, size_t* cap, size_t need) {
   return IBL_OK;
 }
 
-int jpeg_decode_u8(JpegWs** pws, const uint8_t* const* files, const size_t* lens, int N, uint8_t* out_u8,
-                   const uint64_t* out_offsets, int* status, int* err_dev, cudaStream_t s, uint64_t* launches) {
+static int ws_open(JpegWs** pws) {
   if (!*pws) {
     *pws = new (std::nothrow) JpegWs();
     if (!*pws) return IBL_ERR_OOM;
     IBL_CUDA_OK(cudaEventCreateWithFlags(&(*pws)->copied, cudaEventDisableTiming));
   }
+  return IBL_OK;
+}
+
+// pinned staging of at least `bytes`, once the previous call's H2D copy no longer reads it
+static int stage_host(JpegWs* ws, size_t bytes) {
+  if (ws->pending) {
+    IBL_CUDA_OK(cudaEventSynchronize(ws->copied));
+    ws->pending = false;
+  }
+  if (ws->host_cap < bytes) {
+    if (ws->host) cudaFreeHost(ws->host);
+    ws->host = nullptr;
+    ws->host_cap = 0;
+    if (cudaMallocHost(&ws->host, bytes) != cudaSuccess) {
+      cudaGetLastError();
+      set_last_error("jpeg staging cudaMallocHost failed");
+      return IBL_ERR_OOM;
+    }
+    ws->host_cap = bytes;
+  }
+  return IBL_OK;
+}
+
+// frame layout of one parsed image: MCU grid, blocks per MCU, component planes at libjpeg's sizes, quantisation
+// tables q[c]; reserves its coefficient blocks and plane bytes
+static void fill_img(const Parsed& p, const uint16_t (*q)[64], ImgDev& im, uint64_t& coef_blocks,
+                     uint64_t& plane_bytes) {
+  memset(&im, 0, sizeof(im));
+  im.width = p.info.width;
+  im.height = p.info.height;
+  im.ncomp = p.ncomp;
+  im.mcus_x = p.mcus_x;
+  im.mcus_y = p.mcus_y;
+  const int hmax = p.hs[0], vmax = p.vs[0];
+  int k = 0;
+  for (int c = 0; c < p.ncomp; ++c) {
+    im.comp_hs[c] = p.hs[c];
+    im.comp_vs[c] = p.vs[c];
+    for (int v = 0; v < p.vs[c]; ++v)
+      for (int h = 0; h < p.hs[c]; ++h, ++k) {
+        im.blk_comp[k] = (int8_t)c;
+        im.blk_dx[k] = (int8_t)h;
+        im.blk_dy[k] = (int8_t)v;
+      }
+    im.comp_w[c] = (int)(((long long)im.width * p.hs[c] + hmax - 1) / hmax);
+    im.comp_h[c] = (int)(((long long)im.height * p.vs[c] + vmax - 1) / vmax);
+    im.plane_w[c] = im.mcus_x * p.hs[c] * 8;
+    im.plane_off[c] = plane_bytes;
+    plane_bytes += align16((uint64_t)im.plane_w[c] * im.mcus_y * p.vs[c] * 8);
+    memcpy(im.q[c], q[c], sizeof(im.q[c]));
+  }
+  im.bpm = k;
+  im.nblocks = im.mcus_x * im.mcus_y * im.bpm;
+  im.coef_block = coef_blocks;
+  coef_blocks += im.nblocks;
+}
+
+int jpeg_decode_u8(JpegWs** pws, const uint8_t* const* files, const size_t* lens, int N, uint8_t* out_u8,
+                   const uint64_t* out_offsets, int* status, int* err_dev, cudaStream_t s, uint64_t* launches) {
+  IBL_RET(ws_open(pws));
   JpegWs* ws = *pws;
   IBL_CUDA_OK(cudaMemsetAsync(err_dev, 0, (size_t)N * sizeof(int), s));
   std::vector<Parsed> ps;
@@ -804,34 +1232,9 @@ int jpeg_decode_u8(JpegWs** pws, const uint8_t* const* files, const size_t* lens
   for (int m = 0; m < M; ++m) {
     const Parsed& p = ps[m];
     ImgDev& im = imgs[m];
-    memset(&im, 0, sizeof(im));
-    im.width = p.info.width;
-    im.height = p.info.height;
-    im.ncomp = p.ncomp;
-    im.mcus_x = p.mcus_x;
-    im.mcus_y = p.mcus_y;
-    const int hmax = p.hs[0], vmax = p.vs[0];
-    int k = 0;
-    for (int c = 0; c < p.ncomp; ++c) {
-      im.comp_hs[c] = p.hs[c];
-      im.comp_vs[c] = p.vs[c];
-      for (int v = 0; v < p.vs[c]; ++v)
-        for (int h = 0; h < p.hs[c]; ++h, ++k) {
-          im.blk_comp[k] = (int8_t)c;
-          im.blk_dx[k] = (int8_t)h;
-          im.blk_dy[k] = (int8_t)v;
-        }
-      im.comp_w[c] = (int)(((long long)im.width * p.hs[c] + hmax - 1) / hmax);
-      im.comp_h[c] = (int)(((long long)im.height * p.vs[c] + vmax - 1) / vmax);
-      im.plane_w[c] = im.mcus_x * p.hs[c] * 8;
-      im.plane_off[c] = plane_bytes;
-      plane_bytes += align16((uint64_t)im.plane_w[c] * im.mcus_y * p.vs[c] * 8);
-      memcpy(im.q[c], p.qt[p.tq[c]], sizeof(im.q[c]));
-    }
-    im.bpm = k;
-    im.nblocks = im.mcus_x * im.mcus_y * im.bpm;
-    im.coef_block = coef_blocks;
-    coef_blocks += im.nblocks;
+    uint16_t q[3][64];
+    for (int c = 0; c < p.ncomp; ++c) memcpy(q[c], p.qt[p.tq[c]], sizeof(q[c]));
+    fill_img(p, q, im, coef_blocks, plane_bytes);
     im.out_off = out_offsets[slot[m]];
     im.first_seq = (int)seq_iv.size();
     const int n_iv = (int)p.iv_start.size();
@@ -863,21 +1266,7 @@ int jpeg_decode_u8(JpegWs** pws, const uint8_t* const* files, const size_t* lens
   const size_t o_img = 0, o_iv = align16(o_img + sizeof(ImgDev) * M), o_tab = align16(o_iv + sizeof(IntervalDev) * NI),
                o_seq = align16(o_tab + sizeof(HuffTab) * 6 * M), o_slot = align16(o_seq + sizeof(int) * NS),
                o_bytes = align16(o_slot + sizeof(int) * M), blob_bytes = align16(o_bytes + ebytes);
-  if (ws->pending) {                                 // the previous call's H2D copy still reads the pinned buffer
-    IBL_CUDA_OK(cudaEventSynchronize(ws->copied));
-    ws->pending = false;
-  }
-  if (ws->host_cap < blob_bytes) {
-    if (ws->host) cudaFreeHost(ws->host);
-    ws->host = nullptr;
-    ws->host_cap = 0;
-    if (cudaMallocHost(&ws->host, blob_bytes) != cudaSuccess) {
-      cudaGetLastError();
-      set_last_error("jpeg staging cudaMallocHost failed");
-      return IBL_ERR_OOM;
-    }
-    ws->host_cap = blob_bytes;
-  }
+  IBL_RET(stage_host(ws, blob_bytes));
   uint8_t* h = ws->host;
   memcpy(h + o_img, imgs.data(), sizeof(ImgDev) * M);
   memcpy(h + o_iv, ivs.data(), sizeof(IntervalDev) * NI);
@@ -956,6 +1345,188 @@ int jpeg_decode_u8(JpegWs** pws, const uint8_t* const* files, const size_t* lens
   return IBL_OK;
 }
 
+// Progressive files: the parser records the scan script; the scans of one image run in file order, one launch per
+// (scan round, scan kind) covering that scan of every image of the batch, then the baseline IDCT and colour kernels.
+int jpeg_decode_progressive_u8(JpegWs** pws, const uint8_t* const* files, const size_t* lens, int N, uint8_t* out_u8,
+                               const uint64_t* out_offsets, int* status, int* err_dev, cudaStream_t s,
+                               uint64_t* launches) {
+  IBL_RET(ws_open(pws));
+  JpegWs* ws = *pws;
+  IBL_CUDA_OK(cudaMemsetAsync(err_dev, 0, (size_t)N * sizeof(int), s));
+  std::vector<Parsed> ps;
+  std::vector<int> slot;
+  for (int n = 0; n < N; ++n) {
+    Parsed p;
+    status[n] = files[n] ? parse_jpeg(files[n], lens[n], p, true) : IBL_ERR_BAD_ARG;
+    if (status[n] != IBL_OK) continue;
+    ps.push_back(std::move(p));
+    slot.push_back(n);
+  }
+  const int M = (int)ps.size();
+  if (M == 0) return IBL_OK;
+  // layout: frames, scans (in image order), entropy bytes per image in file order
+  std::vector<ImgDev> imgs(M);
+  std::vector<ScanDev> scans;
+  std::vector<int> scan0(M);                         // first ScanDev of every image
+  std::vector<std::vector<uint64_t>> iv_base(M);     // arena byte of every interval of every image
+  uint64_t ebytes = 0, coef_blocks = 0, plane_bytes = 0;
+  int rounds = 0;
+  for (int m = 0; m < M; ++m) {
+    const Parsed& p = ps[m];
+    fill_img(p, p.comp_q, imgs[m], coef_blocks, plane_bytes);
+    imgs[m].out_off = out_offsets[slot[m]];
+    int comp_first[3] = {0, 0, 0};
+    for (int c = 1; c < p.ncomp; ++c) comp_first[c] = comp_first[c - 1] + p.hs[c - 1] * p.vs[c - 1];
+    scan0[m] = (int)scans.size();
+    rounds = std::max(rounds, (int)p.scans.size());
+    for (const ScanInfo& si : p.scans) {
+      ScanDev sd;
+      memset(&sd, 0, sizeof(sd));
+      sd.img = m;
+      sd.ncomp = si.ncomp;
+      sd.ss = si.ss;
+      sd.se = si.se;
+      sd.al = si.al;
+      if (si.ncomp > 1) {
+        sd.mcus_x = p.mcus_x;
+        for (int i = 0; i < si.ncomp; ++i) {
+          const int c = si.comp[i];
+          for (int v = 0; v < p.vs[c]; ++v)
+            for (int h = 0; h < p.hs[c]; ++h, ++sd.bpm) {
+              sd.blk_slot[sd.bpm] = (int8_t)i;
+              sd.blk_off[sd.bpm] = (int8_t)(comp_first[c] + v * p.hs[c] + h);
+            }
+        }
+      } else {
+        const int c = si.comp[0];
+        sd.bpm = 1;
+        sd.mcus_x = p.width_blocks[c];
+        sd.hs = p.hs[c];
+        sd.vs = p.vs[c];
+        sd.comp_first = comp_first[c];
+      }
+      scans.push_back(sd);
+    }
+    const size_t n_iv = p.iv_start.size();
+    for (size_t t = 0; t < n_iv; ++t) {
+      const uint64_t b0 = p.iv_start[t], b1 = t + 1 < n_iv ? p.iv_start[t + 1] : p.entropy.size();
+      if ((b1 - b0) * 8 > 0xFFFFFFFFull - 64) {
+        status[slot[m]] = IBL_ERR_UNSUPPORTED;       // cannot happen below 512 MB per interval
+        return IBL_ERR_UNSUPPORTED;
+      }
+      iv_base[m].push_back(ebytes);
+      ebytes += (b1 - b0) + kPad;
+    }
+  }
+  // intervals grouped by (round, kind): round r holds the r-th scan of every image
+  std::vector<ProgIvDev> ivs;
+  std::vector<int> group(4 * rounds + 1, 0);
+  for (int r = 0; r < rounds; ++r)
+    for (int kind = 0; kind < 4; ++kind) {
+      group[4 * r + kind] = (int)ivs.size();
+      for (int m = 0; m < M; ++m) {
+        const Parsed& p = ps[m];
+        if (r >= (int)p.scans.size()) continue;
+        const ScanInfo& si = p.scans[r];
+        if ((si.ss == 0 ? 0 : 2) + (si.ah == 0 ? 0 : 1) != kind) continue;
+        for (int t = 0; t < si.n_iv; ++t) {
+          const int g = si.first_iv + t;
+          const uint64_t b0 = p.iv_start[g], b1 = g + 1 < (int)p.iv_start.size() ? p.iv_start[g + 1] : p.entropy.size();
+          ProgIvDev iv;
+          iv.byte_base = iv_base[m][g];
+          iv.nbits = (uint32_t)((b1 - b0) * 8);
+          iv.scan = scan0[m] + r;
+          iv.first_mcu = si.restart ? t * si.restart : 0;
+          iv.n_mcus = si.restart ? std::min(si.mcus - iv.first_mcu, si.restart) : si.mcus;
+          ivs.push_back(iv);
+        }
+      }
+    }
+  group[4 * rounds] = (int)ivs.size();
+  const int NSC = (int)scans.size(), NI = (int)ivs.size();
+  // staging blob: images | scans | intervals | Huffman tables | slots | entropy bytes
+  const size_t o_img = 0, o_scan = align16(o_img + sizeof(ImgDev) * M),
+               o_iv = align16(o_scan + sizeof(ScanDev) * NSC), o_tab = align16(o_iv + sizeof(ProgIvDev) * NI),
+               o_slot = align16(o_tab + sizeof(HuffTab) * 3 * NSC), o_bytes = align16(o_slot + sizeof(int) * M),
+               blob_bytes = align16(o_bytes + ebytes);
+  IBL_RET(stage_host(ws, blob_bytes));
+  uint8_t* h = ws->host;
+  memcpy(h + o_img, imgs.data(), sizeof(ImgDev) * M);
+  memcpy(h + o_scan, scans.data(), sizeof(ScanDev) * NSC);
+  memcpy(h + o_iv, ivs.data(), sizeof(ProgIvDev) * NI);
+  HuffTab* tabs = reinterpret_cast<HuffTab*>(h + o_tab);
+  for (int m = 0; m < M; ++m)
+    for (size_t r = 0; r < ps[m].scans.size(); ++r)
+      for (int i = 0; i < 3; ++i) tabs[3 * (scan0[m] + r) + i] = ps[m].scans[r].tab[i];
+  memcpy(h + o_slot, slot.data(), sizeof(int) * M);
+  for (int m = 0; m < M; ++m) {
+    const Parsed& p = ps[m];
+    const size_t n_iv = p.iv_start.size();
+    for (size_t t = 0; t < n_iv; ++t) {
+      const uint64_t b0 = p.iv_start[t], b1 = t + 1 < n_iv ? p.iv_start[t + 1] : p.entropy.size();
+      uint8_t* e = h + o_bytes + iv_base[m][t];
+      memcpy(e, p.entropy.data() + b0, b1 - b0);
+      memset(e + (b1 - b0), 0, kPad);
+    }
+  }
+  // device arena: coefficients | planes
+  const size_t a_coef = 0, a_planes = align16(a_coef + coef_blocks * 64 * sizeof(int16_t)),
+               arena_bytes = align16(a_planes + plane_bytes);
+  IBL_RET(grow_device(&ws->blob, &ws->blob_cap, blob_bytes));
+  IBL_RET(grow_device(&ws->arena, &ws->arena_cap, arena_bytes));
+  IBL_CUDA_OK(cudaMemcpyAsync(ws->blob, ws->host, blob_bytes, cudaMemcpyHostToDevice, s));
+  IBL_CUDA_OK(cudaEventRecord(ws->copied, s));
+  ws->pending = true;
+  uint8_t* db = static_cast<uint8_t*>(ws->blob);
+  uint8_t* da = static_cast<uint8_t*>(ws->arena);
+  ProgBatch pb;
+  pb.img = reinterpret_cast<const ImgDev*>(db + o_img);
+  pb.scan = reinterpret_cast<const ScanDev*>(db + o_scan);
+  pb.iv = reinterpret_cast<const ProgIvDev*>(db + o_iv);
+  pb.tabs = reinterpret_cast<const HuffTab*>(db + o_tab);
+  pb.err_slot = reinterpret_cast<const int*>(db + o_slot);
+  pb.bytes = db + o_bytes;
+  pb.coef = reinterpret_cast<int16_t*>(da + a_coef);
+  pb.err = err_dev;
+  Batch b;
+  memset(&b, 0, sizeof(b));
+  b.img = pb.img;
+  b.coef = pb.coef;
+  b.planes = da + a_planes;
+  b.out = out_u8;
+  IBL_CUDA_OK(cudaMemsetAsync(pb.coef, 0, coef_blocks * 64 * sizeof(int16_t), s));
+  uint64_t n_launch = 2;
+  for (int r = 0; r < rounds; ++r)
+    for (int kind = 0; kind < 4; ++kind) {
+      const int i0 = group[4 * r + kind], i1 = group[4 * r + kind + 1];
+      if (i0 == i1) continue;
+      const unsigned warps = (unsigned)((i1 - i0 + kProgWarps - 1) / kProgWarps);
+      switch (kind) {
+        case kDcFirst: jpeg_prog_dc_first_kernel<<<warps, 32 * kProgWarps, 0, s>>>(pb, i0, i1); break;
+        case kDcRefine: jpeg_prog_dc_refine_kernel<<<(unsigned)(i1 - i0), 256, 0, s>>>(pb, i0); break;
+        case kAcFirst: jpeg_prog_ac_first_kernel<<<warps, 32 * kProgWarps, 0, s>>>(pb, i0, i1); break;
+        default: jpeg_prog_ac_refine_kernel<<<warps, 32 * kProgWarps, 0, s>>>(pb, i0, i1); break;
+      }
+      ++n_launch;
+    }
+  const int sms = device_sm_count();
+  auto grid1 = [&](long long work, int threads) {
+    const long long g = (work + threads - 1) / threads;
+    return (unsigned)std::max(1ll, std::min(g, (long long)sms * 16));
+  };
+  int max_blocks = 0;
+  long long max_px = 0;
+  for (const ImgDev& im : imgs) {
+    max_blocks = std::max(max_blocks, im.nblocks);
+    max_px = std::max(max_px, (long long)im.width * im.height);
+  }
+  jpeg_idct_kernel<<<dim3(std::min(grid1(max_blocks, 128), 1024u), M), 128, 0, s>>>(b);
+  jpeg_color_kernel<<<dim3(std::min(grid1(max_px, 256), 1024u), M), 256, 0, s>>>(b);
+  IBL_CUDA_OK(cudaGetLastError());
+  if (launches) *launches += n_launch;
+  return IBL_OK;
+}
+
 }  // namespace ibl
 
 extern "C" int ibl_jpeg_parse(const uint8_t* data, size_t len, ibl_jpeg_info* out) {
@@ -964,5 +1535,28 @@ extern "C" int ibl_jpeg_parse(const uint8_t* data, size_t len, ibl_jpeg_info* ou
   const int st = ibl::parse_jpeg(data, len, p);
   *out = p.info;
   if (st != IBL_OK) ibl::set_last_error(std::string("ibl_jpeg_parse: ") + p.info.reason);
+  return st;
+}
+
+extern "C" int ibl_jpeg_parse_progressive(const uint8_t* data, size_t len, ibl_jpeg_info* out, int* n_scans,
+                                          ibl_jpeg_scan* scans, int max_scans) {
+  IBL_REQUIRE(out, "null argument");
+  ibl::Parsed p;
+  const int st = ibl::parse_jpeg(data, len, p, true);
+  *out = p.info;
+  if (n_scans) *n_scans = (int)p.scans.size();
+  for (int t = 0; scans && t < max_scans && t < (int)p.scans.size(); ++t) {
+    const ibl::ScanInfo& si = p.scans[t];
+    ibl_jpeg_scan& o = scans[t];
+    o.components = si.ncomp;
+    for (int i = 0; i < 3; ++i) o.comp[i] = i < si.ncomp ? si.comp[i] : -1;
+    o.ss = si.ss;
+    o.se = si.se;
+    o.ah = si.ah;
+    o.al = si.al;
+    o.restart_interval = si.restart;
+    o.intervals = si.n_iv;
+  }
+  if (st != IBL_OK) ibl::set_last_error(std::string("ibl_jpeg_parse_progressive: ") + p.info.reason);
   return st;
 }

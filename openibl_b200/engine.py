@@ -343,9 +343,10 @@ class Engine:
         return _cabi.jpeg_parse(data)
 
     def decode_jpeg_async(self, files: Sequence[bytes], fallback=None):
-        """In-memory JPEG files -> ([device uint8 [H,W,3] or None], device int32 error words [N]).  None marks a file
-        the parser rejected (progressive, CMYK, ...); nothing is synchronised, so a corrupt entropy stream shows
-        only in its error word (nonzero) once the stream has run.
+        """In-memory JPEG files -> ([device uint8 [H,W,3] or None], device int32 error words [N]).  Baseline files
+        go to ibl_jpeg_decode_u8 and progressive ones to ibl_jpeg_decode_progressive_u8; None marks a file both
+        parsers rejected (CMYK, arithmetic, a progressive file libjpeg would block-smooth, ...).  Nothing is
+        synchronised, so a corrupt entropy stream shows only in its error word (nonzero) once the stream has run.
 
         With `fallback` (bytes -> host uint8 [H,W,3] array), rejected files are decoded by it instead and copied into
         the same device buffer, so every returned image is a view into one allocation (what color_jitter_u8 takes)."""
@@ -353,11 +354,19 @@ class Engine:
         if n == 0:
             return [], torch.zeros(0, dtype=torch.int32, device=torch.device("cuda", self.device))
         infos = [_cabi.jpeg_parse(f) for f in files]
-        host = {i: fallback(f) for i, (f, inf) in enumerate(zip(files, infos)) if fallback and not inf["ok"]}
+        prog = {}
+        for i, (f, inf) in enumerate(zip(files, infos)):
+            if not inf["ok"] and inf["reason"] == "progressive":
+                p = _cabi.jpeg_parse_progressive(f)
+                if p["ok"]:
+                    prog[i] = p
+        host = {i: fallback(f) for i, (f, inf) in enumerate(zip(files, infos))
+                if fallback and not inf["ok"] and i not in prog}
         offsets = (c_uint64 * n)()
         total = 0
         for i, inf in enumerate(infos):
             offsets[i] = total
+            inf = prog.get(i, inf)
             if inf["ok"]:
                 total += inf["height"] * inf["width"] * 3
             elif i in host:
@@ -370,8 +379,22 @@ class Engine:
         status = (c_int * n)()
         check(self.lib.ibl_jpeg_decode_u8(self.h, ptrs, lens, n, _ptr(out), offsets, status, _ptr(err),
                                           _stream(self.device)), "ibl_jpeg_decode_u8")
+        if prog:
+            idx = sorted(prog)
+            m = len(idx)
+            p_status = (c_int * m)()
+            p_err = torch.empty(m, dtype=torch.int32, device=dev)
+            check(self.lib.ibl_jpeg_decode_progressive_u8(
+                self.h, (ctypes.c_char_p * m)(*[bytes(files[i]) for i in idx]),
+                (ctypes.c_size_t * m)(*[len(files[i]) for i in idx]),
+                m, _ptr(out), (c_uint64 * m)(*[offsets[i] for i in idx]), p_status, _ptr(p_err), _stream(self.device)),
+                "ibl_jpeg_decode_progressive_u8")
+            err[idx] = p_err
+            for j, i in enumerate(idx):
+                status[i] = p_status[j]
         imgs = []
         for i, inf in enumerate(infos):
+            inf = prog.get(i, inf)
             if i in host:
                 im = out[offsets[i]: offsets[i] + host[i].size].view(host[i].shape)
                 im.copy_(torch.from_numpy(host[i]))
@@ -385,8 +408,8 @@ class Engine:
 
     def decode_jpeg(self, files: Sequence[bytes]):
         """In-memory JPEG files -> list of device uint8 [H,W,3], bit-identical to
-        np.asarray(Image.open(f).convert('RGB')); None for a file the device decoder does not take.  Waits for the
-        stream and raises RuntimeError if an entropy stream is corrupt."""
+        np.asarray(Image.open(f).convert('RGB')) for baseline and progressive files; None for a file the device
+        decoders do not take.  Waits for the stream and raises RuntimeError if an entropy stream is corrupt."""
         imgs, err = self.decode_jpeg_async(files)
         bad = torch.nonzero(err).flatten().tolist()
         if bad:

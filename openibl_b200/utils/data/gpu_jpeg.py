@@ -4,9 +4,10 @@ ibl/utils/data/preprocessor.py:31-42: `Image.open(f).convert('RGB')`, `T.Resize`
 A loader opts in with `get_transformer_test(h, w, tokyo, device_decode=True)`: `Preprocessor` then yields each file's
 bytes as an `EncodedImage` (about 0.1 MB for a 480x640 JPEG instead of 3.7 MB of fp32), and `extract_cnn_feature`
 turns a batch of them into the normalised fp32 tensor with `decode_to_tensor`:
-  * `Engine.decode_jpeg_async` (csrc/jpeg.cu) decodes baseline JPEGs on the device, bit-identical to Pillow;
-  * files the device decoder does not take (progressive, CMYK, PNG, ...) are decoded by Pillow on the host and join
-    the same uint8 pipeline;
+  * `Engine.decode_jpeg_async` (csrc/jpeg.cu) decodes baseline and progressive JPEGs on the device, bit-identical to
+    Pillow;
+  * files the device decoders do not take (CMYK, arithmetic-coded, progressive files libjpeg would block-smooth, PNG,
+    ...) are decoded by Pillow on the host and join the same uint8 pipeline;
   * the existing Pillow-exact resize (`Engine.resize_u8`, skipped when the size already matches) and
     ToTensor + Normalize (`Engine.preprocess_u8`) finish the transform.
 The result equals `get_transformer_test(h, w, tokyo)(Image.open(f).convert('RGB'))` bit for bit.

@@ -242,6 +242,32 @@ int ibl_jpeg_decode_progressive_u8(ibl_engine* e, const uint8_t* const* files, c
                                    uint8_t* out_u8, const uint64_t* out_offsets, int* status, int* err_dev,
                                    void* stream);
 
+/* ---- input side: PNG decode on the GPU ---------------------------------------- */
+/* `Image.open(f).convert('RGB')` for PNGs, bit-identical to Pillow: non-interlaced, bit depth 8, colour types 0 (grey,
+ * replicated), 2 (RGB), 3 (palette; an index past a short PLTE gives black, tRNS is ignored), 4 (grey + alpha, alpha
+ * dropped) and 6 (RGBA, alpha dropped).  The chunk walk follows Pillow's: CRCs are verified for every chunk before the
+ * first IDAT and for none after; the image data is the first run of IDAT chunks (cut at the end of the file); IEND is
+ * optional.  Everything else is IBL_ERR_UNSUPPORTED with `reason` set: other bit depths, interlace, APNG, a zlib preset
+ * dictionary or bad zlib header, a palette image without PLTE, a zero size, and chunks Pillow would raise on or
+ * interpret. */
+typedef struct ibl_png_info {
+  int width, height;
+  int color_type;            /* 0, 2, 3, 4 or 6 */
+  int bit_depth;             /* 8 when accepted */
+  int palette_size;          /* PLTE entries (0 without PLTE) */
+  uint64_t zlib_bytes;       /* bytes of the zlib stream (the IDAT payloads, concatenated) */
+  char reason[120];          /* why the file was rejected ("" when accepted) */
+} ibl_png_info;
+/* Host-only parse of one in-memory file (no device, no engine). */
+int ibl_png_parse(const uint8_t* data, size_t len, ibl_png_info* out);
+/* ibl_jpeg_decode_u8's contract for PNGs (status[i] is the ibl_png_parse result; image i needs height*width*3 bytes at
+ * out_u8 + out_offsets[i]).  The whole zlib stream is inflated on the device, one block per image; err_dev[i] becomes
+ * nonzero for a deflate error (bad block type, invalid or incomplete code, stored length mismatch, distance past the
+ * output), a stream that ends before the last row, a wrong Adler-32 (when the stream carries one) or a filter type
+ * above 4.  Every read is bounded by the staged stream and its zero padding, so corrupt data never faults. */
+int ibl_png_decode_u8(ibl_engine* e, const uint8_t* const* files, const size_t* lens, int N, uint8_t* out_u8,
+                      const uint64_t* out_offsets, int* status, int* err_dev, void* stream);
+
 /* ---- input side: the training transform's colour jitter on the GPU ------------ */
 /* T.ColorJitter(0.7, 0.7, 0.7, 0.5), the first step of the reference's training transform
  * (ibl/utils/data/__init__.py:29-35), bit-identical to torchvision's PIL path: ColorJitter.forward applies, in the

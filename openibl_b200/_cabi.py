@@ -16,6 +16,7 @@ STATUS_NAMES = {0: "IBL_OK", 1: "IBL_ERR_BAD_ARG", 2: "IBL_ERR_NOT_READY", 3: "I
                 4: "IBL_ERR_NO_DEVICE", 5: "IBL_ERR_OOM", 6: "IBL_ERR_UNSUPPORTED"}
 OUT_VLAD, OUT_PCA, OUT_POOL = 0x1, 0x2, 0x4
 CONV_SIMT_FP32, CONV_TC_BF16X3 = 0, 1
+PNG_SIGNATURE = b"\x89PNG\r\n\x1a\n"
 
 _P = c_void_p
 
@@ -31,6 +32,12 @@ class JpegScan(Structure):
     """ibl_jpeg_scan (include/iblb200.h)."""
     _fields_ = [("components", c_int), ("comp", c_int * 3), ("ss", c_int), ("se", c_int), ("ah", c_int), ("al", c_int),
                 ("restart_interval", c_int), ("intervals", c_int)]
+
+
+class PngInfo(Structure):
+    """ibl_png_info (include/iblb200.h)."""
+    _fields_ = [("width", c_int), ("height", c_int), ("color_type", c_int), ("bit_depth", c_int),
+                ("palette_size", c_int), ("zlib_bytes", c_uint64), ("reason", c_char * 120)]
 
 
 class ColorJitterParams(Structure):
@@ -76,6 +83,8 @@ SIGNATURES = {
     "ibl_jpeg_parse_progressive": (c_int, [c_char_p, c_size_t, POINTER(JpegInfo), POINTER(c_int), POINTER(JpegScan),
                                            c_int]),
     "ibl_jpeg_decode_progressive_u8": (c_int, [_P, _P, _P, c_int, _P, _P, _P, _P, _P]),
+    "ibl_png_parse": (c_int, [c_char_p, c_size_t, POINTER(PngInfo)]),
+    "ibl_png_decode_u8": (c_int, [_P, _P, _P, c_int, _P, _P, _P, _P, _P]),
     "ibl_color_jitter_u8": (c_int, [_P, _P, _P, _P, _P, POINTER(ColorJitterParams), c_int, _P]),
     "ibl_l2dist_dense": (c_int, [_P, _P, c_int, _P, c_int, c_int, _P, _P]),
     "ibl_l2dist_self": (c_int, [_P, _P, c_int, c_int, _P, _P]),
@@ -161,6 +170,17 @@ def jpeg_parse_progressive(data: bytes) -> dict:
             "scans": [{"components": tuple(s.comp[:s.components]), "ss": s.ss, "se": s.se, "ah": s.ah, "al": s.al,
                        "restart_interval": s.restart_interval, "intervals": s.intervals}
                       for s in scans[:n.value]]}
+
+
+def png_parse(data: bytes) -> dict:
+    """ibl_png_parse on one in-memory file; runs on the host, no device needed."""
+    lib = load()
+    info = PngInfo()
+    data = bytes(data)
+    st = lib.ibl_png_parse(data, len(data), ctypes.byref(info))
+    return {"ok": st == IBL_OK, "status": st, "width": info.width, "height": info.height,
+            "color_type": info.color_type, "bit_depth": info.bit_depth, "palette_size": info.palette_size,
+            "zlib_bytes": info.zlib_bytes, "reason": info.reason.decode()}
 
 
 def check(status: int, where: str) -> None:

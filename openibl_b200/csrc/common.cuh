@@ -126,13 +126,30 @@ int launch_resize_bilinear_u8(const uint8_t* x, int N, int Hin, int Win, int Hou
                               const int* kk_h, int ksize_h, const int* bounds_v, const int* kk_v, int ksize_v,
                               uint8_t* tmp, uint8_t* out, cudaStream_t s, uint64_t* launches);
 // jpeg.cu  (baseline and progressive JPEG decode, bit-exact with libjpeg's defaults; the parser is host code)
-struct JpegWs;   // opaque per-engine workspace: pinned staging blob, device tables, coefficients, planes
+// Per-engine decode workspace (the JPEG and PNG paths each own one): pinned staging blob, its device copy, and an
+// arena for tables, coefficients, planes or inflated rows.  `copied` marks the end of the last H2D copy from `host`.
+struct JpegWs {
+  uint8_t* host = nullptr;
+  size_t host_cap = 0;
+  void* blob = nullptr;
+  size_t blob_cap = 0;
+  void* arena = nullptr;
+  size_t arena_cap = 0;
+  cudaEvent_t copied = nullptr;
+  bool pending = false;
+};
 void jpeg_ws_destroy(JpegWs* ws);
+int ws_open(JpegWs** pws);
+int grow_device(void** p, size_t* cap, size_t need);   // device buffer of at least `need` bytes (contents dropped)
+int stage_host(JpegWs* ws, size_t bytes);             // pinned staging once the previous H2D copy no longer reads it
 int jpeg_decode_u8(JpegWs** ws, const uint8_t* const* files, const size_t* lens, int N, uint8_t* out_u8,
                    const uint64_t* out_offsets, int* status, int* err_dev, cudaStream_t s, uint64_t* launches);
 int jpeg_decode_progressive_u8(JpegWs** ws, const uint8_t* const* files, const size_t* lens, int N, uint8_t* out_u8,
                                const uint64_t* out_offsets, int* status, int* err_dev, cudaStream_t s,
                                uint64_t* launches);
+// png.cu  (8-bit non-interlaced PNG decode, bit-exact with Pillow; the chunk parse is host code)
+int png_decode_u8(JpegWs** ws, const uint8_t* const* files, const size_t* lens, int N, uint8_t* out_u8,
+                  const uint64_t* out_offsets, int* status, int* err_dev, cudaStream_t s, uint64_t* launches);
 // color_jitter.cu  (T.ColorJitter, bit-exact with torchvision's PIL path)
 struct JitterWs;   // opaque per-engine workspace: pinned staging of descriptors, device copy, L sums
 void jitter_ws_destroy(JitterWs* ws);

@@ -86,6 +86,7 @@ struct ibl_engine {
   const int* knn_flag_counter = nullptr; // its count of rows sent to the exact scan (null: no call yet)
   JpegWs* jpeg_ws = nullptr;             // JPEG decode: pinned staging blob, tables, coefficients, planes (jpeg.cu)
   JpegWs* jpeg_prog_ws = nullptr;        // the same for progressive JPEGs
+  JpegWs* png_ws = nullptr;              // PNG decode: pinned staging of the zlib streams, inflated rows (png.cu)
   JitterWs* jitter_ws = nullptr;         // colour jitter: pinned staging of per-image descriptors, L sums (color_jitter.cu)
   RerankWs* rr_ws = nullptr;             // sparse stage of the re-ranking: CSR matrices, inverted index, pair buffers
   const int* flag_counter = nullptr;     // guard counter of the last ibl_l2dist_topk call (null: no guard on its path)
@@ -282,6 +283,7 @@ int ibl_engine_destroy(ibl_engine* e) {
   rerank_ws_destroy(e->rr_ws);
   jpeg_ws_destroy(e->jpeg_ws);
   jpeg_ws_destroy(e->jpeg_prog_ws);
+  jpeg_ws_destroy(e->png_ws);
   jitter_ws_destroy(e->jitter_ws);
   delete e;
   return IBL_OK;
@@ -832,6 +834,15 @@ int ibl_jpeg_decode_progressive_u8(ibl_engine* e, const uint8_t* const* files, c
   DeviceGuard g(e->device);
   return jpeg_decode_progressive_u8(&e->jpeg_prog_ws, files, lens, N, out_u8, out_offsets, status, err_dev, S(stream),
                                     &e->launches);
+}
+
+// The same for 8-bit non-interlaced PNGs: one block per image inflates, one block per image unfilters (png.cu).
+int ibl_png_decode_u8(ibl_engine* e, const uint8_t* const* files, const size_t* lens, int N, uint8_t* out_u8,
+                      const uint64_t* out_offsets, int* status, int* err_dev, void* stream) {
+  IBL_REQUIRE(e && files && lens && out_offsets && status && err_dev, "null argument");
+  IBL_REQUIRE(N >= 1, "empty batch");
+  DeviceGuard g(e->device);
+  return png_decode_u8(&e->png_ws, files, lens, N, out_u8, out_offsets, status, err_dev, S(stream), &e->launches);
 }
 
 // T.ColorJitter of the reference's training transform (ibl/utils/data/__init__.py:29-35) on decoded uint8 HWC images,

@@ -1109,17 +1109,6 @@ size_t align16(size_t x) { return (x + 15) & ~(size_t)15; }
 
 }  // namespace
 
-struct JpegWs {
-  uint8_t* host = nullptr;
-  size_t host_cap = 0;
-  void* blob = nullptr;
-  size_t blob_cap = 0;
-  void* arena = nullptr;
-  size_t arena_cap = 0;
-  cudaEvent_t copied = nullptr;
-  bool pending = false;
-};
-
 void jpeg_ws_destroy(JpegWs* ws) {
   if (!ws) return;
   if (ws->pending) cudaEventSynchronize(ws->copied);
@@ -1130,7 +1119,7 @@ void jpeg_ws_destroy(JpegWs* ws) {
   delete ws;
 }
 
-static int grow_device(void** p, size_t* cap, size_t need) {
+int grow_device(void** p, size_t* cap, size_t need) {
   if (need <= *cap) return IBL_OK;
   if (*p) cudaFree(*p);
   *p = nullptr;
@@ -1145,7 +1134,7 @@ static int grow_device(void** p, size_t* cap, size_t need) {
   return IBL_OK;
 }
 
-static int ws_open(JpegWs** pws) {
+int ws_open(JpegWs** pws) {
   if (!*pws) {
     *pws = new (std::nothrow) JpegWs();
     if (!*pws) return IBL_ERR_OOM;
@@ -1155,7 +1144,7 @@ static int ws_open(JpegWs** pws) {
 }
 
 // pinned staging of at least `bytes`, once the previous call's H2D copy no longer reads it
-static int stage_host(JpegWs* ws, size_t bytes) {
+int stage_host(JpegWs* ws, size_t bytes) {
   if (ws->pending) {
     IBL_CUDA_OK(cudaEventSynchronize(ws->copied));
     ws->pending = false;

@@ -342,11 +342,18 @@ class Engine:
         layout; `ok` is False with `reason` set for files the device decoder does not take."""
         return _cabi.jpeg_parse(data)
 
+    @staticmethod
+    def png_parse(data: bytes) -> dict:
+        """Host-only chunk walk of one in-memory PNG (no device needed): size, colour type, bit depth, palette size,
+        zlib byte count; `ok` is False with `reason` set for files the device decoder does not take."""
+        return _cabi.png_parse(data)
+
     def decode_jpeg_async(self, files: Sequence[bytes], fallback=None):
-        """In-memory JPEG files -> ([device uint8 [H,W,3] or None], device int32 error words [N]).  Baseline files
-        go to ibl_jpeg_decode_u8 and progressive ones to ibl_jpeg_decode_progressive_u8; None marks a file both
-        parsers rejected (CMYK, arithmetic, a progressive file libjpeg would block-smooth, ...).  Nothing is
-        synchronised, so a corrupt entropy stream shows only in its error word (nonzero) once the stream has run.
+        """In-memory JPEG or PNG files -> ([device uint8 [H,W,3] or None], device int32 error words [N]).  Baseline
+        JPEGs go to ibl_jpeg_decode_u8, progressive ones to ibl_jpeg_decode_progressive_u8 and 8-bit non-interlaced
+        PNGs to ibl_png_decode_u8; None marks a file all parsers rejected (CMYK, arithmetic, a progressive file libjpeg
+        would block-smooth, a 16-bit or interlaced PNG, ...).  Nothing is synchronised, so a corrupt entropy or zlib
+        stream shows only in its error word (nonzero) once the stream has run.
 
         With `fallback` (bytes -> host uint8 [H,W,3] array), rejected files are decoded by it instead and copied into
         the same device buffer, so every returned image is a view into one allocation (what color_jitter_u8 takes)."""
@@ -354,19 +361,26 @@ class Engine:
         if n == 0:
             return [], torch.zeros(0, dtype=torch.int32, device=torch.device("cuda", self.device))
         infos = [_cabi.jpeg_parse(f) for f in files]
-        prog = {}
+        prog, png = {}, {}
         for i, (f, inf) in enumerate(zip(files, infos)):
-            if not inf["ok"] and inf["reason"] == "progressive":
+            if inf["ok"]:
+                continue
+            if inf["reason"] == "progressive":
                 p = _cabi.jpeg_parse_progressive(f)
                 if p["ok"]:
                     prog[i] = p
+            elif bytes(f[:8]) == _cabi.PNG_SIGNATURE:
+                p = _cabi.png_parse(f)
+                if p["ok"]:
+                    png[i] = p
+        device = {**prog, **png}
         host = {i: fallback(f) for i, (f, inf) in enumerate(zip(files, infos))
-                if fallback and not inf["ok"] and i not in prog}
+                if fallback and not inf["ok"] and i not in device}
         offsets = (c_uint64 * n)()
         total = 0
         for i, inf in enumerate(infos):
             offsets[i] = total
-            inf = prog.get(i, inf)
+            inf = device.get(i, inf)
             if inf["ok"]:
                 total += inf["height"] * inf["width"] * 3
             elif i in host:
@@ -379,22 +393,24 @@ class Engine:
         status = (c_int * n)()
         check(self.lib.ibl_jpeg_decode_u8(self.h, ptrs, lens, n, _ptr(out), offsets, status, _ptr(err),
                                           _stream(self.device)), "ibl_jpeg_decode_u8")
-        if prog:
-            idx = sorted(prog)
+        for name, sub in (("ibl_jpeg_decode_progressive_u8", prog), ("ibl_png_decode_u8", png)):
+            if not sub:
+                continue
+            idx = sorted(sub)
             m = len(idx)
-            p_status = (c_int * m)()
-            p_err = torch.empty(m, dtype=torch.int32, device=dev)
-            check(self.lib.ibl_jpeg_decode_progressive_u8(
+            s_status = (c_int * m)()
+            s_err = torch.empty(m, dtype=torch.int32, device=dev)
+            check(getattr(self.lib, name)(
                 self.h, (ctypes.c_char_p * m)(*[bytes(files[i]) for i in idx]),
                 (ctypes.c_size_t * m)(*[len(files[i]) for i in idx]),
-                m, _ptr(out), (c_uint64 * m)(*[offsets[i] for i in idx]), p_status, _ptr(p_err), _stream(self.device)),
-                "ibl_jpeg_decode_progressive_u8")
-            err[idx] = p_err
+                m, _ptr(out), (c_uint64 * m)(*[offsets[i] for i in idx]), s_status, _ptr(s_err), _stream(self.device)),
+                name)
+            err[idx] = s_err
             for j, i in enumerate(idx):
-                status[i] = p_status[j]
+                status[i] = s_status[j]
         imgs = []
         for i, inf in enumerate(infos):
-            inf = prog.get(i, inf)
+            inf = device.get(i, inf)
             if i in host:
                 im = out[offsets[i]: offsets[i] + host[i].size].view(host[i].shape)
                 im.copy_(torch.from_numpy(host[i]))
@@ -407,13 +423,18 @@ class Engine:
         return imgs, err
 
     def decode_jpeg(self, files: Sequence[bytes]):
-        """In-memory JPEG files -> list of device uint8 [H,W,3], bit-identical to
-        np.asarray(Image.open(f).convert('RGB')) for baseline and progressive files; None for a file the device
-        decoders do not take.  Waits for the stream and raises RuntimeError if an entropy stream is corrupt."""
+        """In-memory JPEG or PNG files -> list of device uint8 [H,W,3], bit-identical to
+        np.asarray(Image.open(f).convert('RGB')) for baseline and progressive JPEGs and 8-bit non-interlaced PNGs;
+        None for a file the device decoders do not take.  Waits for the stream and raises RuntimeError if an entropy
+        or zlib stream is corrupt."""
         imgs, err = self.decode_jpeg_async(files)
         bad = torch.nonzero(err).flatten().tolist()
         if bad:
-            raise RuntimeError(f"corrupt JPEG entropy data in file(s) {bad} of the batch")
+            png = [i for i in bad if bytes(files[i][:8]) == _cabi.PNG_SIGNATURE]
+            jpeg = [i for i in bad if i not in png]
+            what = ([f"corrupt JPEG entropy data in file(s) {jpeg}"] if jpeg else []) + \
+                   ([f"corrupt PNG image data in file(s) {png}"] if png else [])
+            raise RuntimeError(" and ".join(what) + " of the batch")
         return imgs
 
     def color_jitter_u8(self, images: Sequence[torch.Tensor], params: Sequence) -> None:

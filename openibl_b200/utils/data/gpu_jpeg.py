@@ -4,10 +4,10 @@ ibl/utils/data/preprocessor.py:31-42: `Image.open(f).convert('RGB')`, `T.Resize`
 A loader opts in with `get_transformer_test(h, w, tokyo, device_decode=True)`: `Preprocessor` then yields each file's
 bytes as an `EncodedImage` (about 0.1 MB for a 480x640 JPEG instead of 3.7 MB of fp32), and `extract_cnn_feature`
 turns a batch of them into the normalised fp32 tensor with `decode_to_tensor`:
-  * `Engine.decode_jpeg_async` (csrc/jpeg.cu) decodes baseline and progressive JPEGs on the device, bit-identical to
-    Pillow;
-  * files the device decoders do not take (CMYK, arithmetic-coded, progressive files libjpeg would block-smooth, PNG,
-    ...) are decoded by Pillow on the host and join the same uint8 pipeline;
+  * `Engine.decode_jpeg_async` decodes baseline and progressive JPEGs (csrc/jpeg.cu) and 8-bit non-interlaced PNGs
+    of every colour type (csrc/png.cu) on the device, bit-identical to Pillow;
+  * files the device decoders do not take (CMYK, arithmetic-coded, progressive files libjpeg would block-smooth,
+    16-bit or interlaced PNGs, ...) are decoded by Pillow on the host and join the same uint8 pipeline;
   * the existing Pillow-exact resize (`Engine.resize_u8`, skipped when the size already matches) and
     ToTensor + Normalize (`Engine.preprocess_u8`) finish the transform.
 The result equals `get_transformer_test(h, w, tokyo)(Image.open(f).convert('RGB'))` bit for bit.
@@ -105,12 +105,13 @@ def _host_decode(data: bytes) -> np.ndarray:
 def decode_to_tensor(files: Sequence[bytes], height: int, width: int, tokyo: bool = False, device=None,
                      names: Optional[Sequence[str]] = None, pending: Optional[list] = None,
                      jitter: Optional[Sequence] = None) -> torch.Tensor:
-    """JPEG file bytes -> fp32 [N,3,H,W] on the device, equal to the reference's test transform of the decoded image,
+    """JPEG or PNG file bytes -> fp32 [N,3,H,W] on the device, equal to the reference's test transform of the decoded image,
     or with `jitter` (one `ColorJitter.get_params` result per file) to its training transform.
 
-    Corrupt entropy data is reported by the device after the fact: with `pending` None this call waits for the
-    stream and raises RuntimeError naming the file; otherwise it appends (error words, names) to `pending` for
-    `check_decode_errors` and does not synchronise."""
+    Corrupt entropy or zlib data is reported by the device after the fact: with `pending` None this call waits for
+    the stream and raises RuntimeError naming the file; otherwise it appends (error words, names, PNG flags) to
+    `pending` for `check_decode_errors` and does not synchronise."""
+    from ... import _cabi
     from ...engine import Engine
     from . import _MEAN, _STD
     if len(files) == 0:
@@ -134,19 +135,21 @@ def decode_to_tensor(files: Sequence[bytes], height: int, width: int, tokyo: boo
         src = torch.stack([imgs[i] for i in idx])
         u8[idx] = src if (h, w) == (oh, ow) else eng.resize_u8(src, oh, ow)
     out = eng.preprocess_u8(u8, _MEAN, _STD)
+    png = [bytes(f[:8]) == _cabi.PNG_SIGNATURE for f in files]
     if pending is None:
-        check_decode_errors([(err, names)])
+        check_decode_errors([(err, names, png)])
     else:
-        pending.append((err, names))
+        pending.append((err, names, png))
     return out
 
 
 def check_decode_errors(pending: List) -> None:
-    """Raise RuntimeError naming the first file whose device decode reported corrupt entropy data."""
-    for err, names in pending:
+    """Raise RuntimeError naming the first file whose device decode reported corrupt entropy or zlib data."""
+    for err, names, png in pending:
         bad = torch.nonzero(err).flatten().tolist()
         if bad:
-            raise RuntimeError(f"corrupt JPEG entropy data in {names[bad[0]]!r}"
+            what = "corrupt PNG image data" if png[bad[0]] else "corrupt JPEG entropy data"
+            raise RuntimeError(f"{what} in {names[bad[0]]!r}"
                                + (f" (and {len(bad) - 1} more in the batch)" if len(bad) > 1 else ""))
     pending.clear()
 

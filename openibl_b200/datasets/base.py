@@ -7,6 +7,9 @@ from __future__ import annotations
 import os.path as osp
 
 import numpy as np
+# imported with the package, as the reference's dataset module does: importing scikit-learn draws from the global
+# `random`, and a script that seeds `random` before creating a dataset must see the reference's stream afterwards
+from sklearn.neighbors import NearestNeighbors
 
 from ..utils.serialization import read_json
 
@@ -21,7 +24,6 @@ def radius_groundtruth(query, gallery, pos_radius, neg_radius=None):
     """dataset.py:23-42: for every query the gallery indices within `pos_radius` metres (UTM) that belong to a
     different place id; queries without any are dropped (their indices are returned as `kept`).  With
     `neg_radius`, also the indices within that radius (the "not a negative" set)."""
-    from sklearn.neighbors import NearestNeighbors
     nn = NearestNeighbors(n_jobs=-1).fit(np.asarray([[g[2], g[3]] for g in gallery], dtype=np.float64))
     q_xy = np.asarray([[q[2], q[3]] for q in query], dtype=np.float64)
     _, near = nn.radius_neighbors(q_xy, radius=pos_radius)

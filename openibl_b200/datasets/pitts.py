@@ -9,11 +9,14 @@ from ..utils.serialization import read_mat, write_json
 from .base import PlaceDataset, _rank
 
 
-def read_dbstruct(path):
-    """dbStruct fields used: [1] dbImage, [2] utmDb (2 x n), [3] qImage, [4] utmQ (2 x n) (pitts.py:11-23)."""
+def read_dbstruct(path, time_stamp=False):
+    """dbStruct fields used: [1] dbImage, [2] utmDb (2 x n), [3] qImage, [4] utmQ (2 x n) (pitts.py:11-23).  With
+    `time_stamp` (Tokyo Time Machine), a time-stamp vector follows each UTM matrix, so qImage / utmQ sit at [4] / [5]
+    (tokyo.py:12-23)."""
     s = read_mat(path)
     names = lambda cell: [c[0].item() for c in cell]
-    return {"db": names(s[1]), "db_utm": s[2].T, "q": names(s[3]), "q_utm": s[4].T}
+    ts = int(time_stamp)
+    return {"db": names(s[1]), "db_utm": s[2].T, "q": names(s[3 + ts]), "q_utm": s[4 + ts].T}
 
 
 class Pittsburgh(PlaceDataset):

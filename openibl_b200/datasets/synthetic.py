@@ -6,7 +6,10 @@ items = (fname, pid, x, y); ibl/utils/data/dataset.py) -- images are generated f
 write_synthetic_pitts_tree: a Pittsburgh-shaped tree ON DISK -- NetVLAD-style dbStruct .mat files for the
 train / val / test splits and small JPEG images laid out as `raw/Pittsburgh/{images,queries}/...` -- so that
 code written for the real dataset (the reference's examples/test.py) runs end to end through
-`datasets.create('pitts', root, scale='30k')`, PIL decoding and the torchvision transforms."""
+`datasets.create('pitts', root, scale='30k')`, PIL decoding and the torchvision transforms.
+
+write_synthetic_tokyo_tree: the same for Tokyo -- Time Machine and Tokyo 24/7 dbStruct .mat files, JPEGs and the PNG
+database -- shaped to exercise every rule of the Tokyo arrangement, for `datasets.create('tokyo', root)`."""
 import os
 import os.path as osp
 
@@ -81,6 +84,83 @@ def write_synthetic_pitts_tree(root, scale="30k", n_places=(24, 10, 40), views=2
               "numImages": float(len(db_names)), "numQueries": float(len(q_names))}
         os.makedirs(raw, exist_ok=True)
         savemat(osp.join(raw, "pitts%s_%s.mat" % (scale, split)), {"dbStruct": st})
+    return root
+
+
+def write_synthetic_tokyo_tree(root, n_places=(12, 9, 8), views=2, size=(120, 160), seed=0):
+    """Writes <root>/raw/tokyoTM_{train,val}.mat, <root>/raw/tokyo247.mat and the images they name, laid out as the
+    Tokyo loader reads them: `raw/tokyoTM/images/<group>/<place>/<time stamp>/<file>.jpg`,
+    `raw/tokyo247/query/<file>.jpg` and `raw/tokyo247/images/<place>/<file>.png` (named .jpg in the struct).
+
+    Time Machine: place p of a split has 1 + p % 3 time stamps of `views` images each; the first view of every time
+    stamp is listed as a query image, the others as database images, and one path is listed twice.  Places come in
+    pairs 4 m apart on a 100 m grid, both views of one scene, so every identity has a positive within 10 m.
+    Tokyo 24/7: n places of `views` database images; every place gets a query 4 m away, two for every third place
+    (at the same UTM position, so they form one query place), landscape and portrait at four sizes.  Returns the root."""
+    from PIL import Image
+    from scipy.io import savemat
+    rng = np.random.RandomState(seed)
+    raw = osp.join(root, "raw")
+    h, w = size
+    cell = lambda names: np.array([[n] for n in names], dtype=object)
+    utm_of = lambda pts: np.asarray(pts, dtype=np.float64).reshape(-1, 2).T
+    n_place = 0
+    for split, n in zip(("train", "val"), n_places[:2]):
+        q_names, q_utm, db_names, db_utm = [], [], [], []
+        for p in range(n):
+            if p % 2 == 0:
+                scene = _scene(rng, h, w, _street(rng, h, w))
+            x = 360000.5 + 1000.0 * ("train", "val").index(split) + 100.0 * (p // 2 % 6) + 4.0 * (p % 2)
+            y = 3940000.25 + 100.0 * (p // 12)
+            place = "%05d" % n_place
+            n_place += 1
+            stamps = ["%d%02d" % (2009 + t, 1 + 5 * t) for t in range(1 + p % 3)]
+            for t, ts in enumerate(stamps if p % 2 == 0 else stamps[::-1]):      # first-seen order != name order
+                light = 18 * t - 12
+                for v in range(views):
+                    name = "%02d/%s/%s/%s_%s_v%d.jpg" % (n_place // 50, place, ts, place, ts, v)
+                    view = np.clip(np.roll(scene, 3 * v + 5 * (p % 2), axis=1) + light
+                                   + rng.randint(-6, 7, size=scene.shape), 0, 255)
+                    _save(Image, osp.join(raw, "tokyoTM", "images", name), view)
+                    (q_names if v == 0 else db_names).append(name)
+                    (q_utm if v == 0 else db_utm).append((x, y))
+        db_names.append(q_names[0])                      # listed twice: registered once
+        db_utm.append(q_utm[0])
+        st = {"whichSet": split, "dbImageFns": cell(db_names), "utmDb": utm_of(db_utm),
+              "dbTimeStamp": np.arange(len(db_names), dtype=np.float64)[None],
+              "qImageFns": cell(q_names), "utmQ": utm_of(q_utm),
+              "qTimeStamp": np.arange(len(q_names), dtype=np.float64)[None],
+              "numImages": float(len(db_names)), "numQueries": float(len(q_names))}
+        os.makedirs(raw, exist_ok=True)
+        savemat(osp.join(raw, "tokyoTM_%s.mat" % split), {"dbStruct": st})
+
+    q_sizes = ((h, w), (w, h), (h * 4 // 5, w * 9 // 10), (w * 9 // 10, h * 4 // 5))   # landscape / portrait
+    q_names, q_utm, db_names, db_utm = [], [], [], []
+    n_q = 0
+    for p in range(n_places[2]):
+        if p % 8 == 0:
+            street = _street(rng, h, w)
+        scene = _scene(rng, h, w, street)
+        x, y = 381234.567 + 100.0 * (p % 6), 3946789.125 + 100.0 * (p // 6)
+        for v in range(views):
+            name = "%05d/%05d%03d.jpg" % (p, p, v)
+            view = np.clip(np.roll(scene, 3 * v, axis=1) + rng.randint(-6, 7, size=scene.shape), 0, 255)
+            _save(Image, osp.join(raw, "tokyo247", "images", name[:-3] + "png"), view)
+            db_names.append(name)
+            db_utm.append((x, y))
+        for _ in range(2 if p % 3 == 0 else 1):
+            qh, qw = q_sizes[n_q % len(q_sizes)]
+            view = np.clip(np.roll(scene, -6 - 2 * n_q, axis=1) + rng.randint(-40, 41, size=scene.shape), 0, 255)
+            view = np.asarray(Image.fromarray(view.astype(np.uint8)).resize((qw, qh), Image.BILINEAR))
+            name = "%06d.jpg" % (100 * p + n_q)
+            _save(Image, osp.join(raw, "tokyo247", "query", name), view)
+            q_names.append(name)
+            q_utm.append((x + 4.0, y))
+            n_q += 1
+    st = {"whichSet": "test", "dbImageFns": cell(db_names), "utmDb": utm_of(db_utm),
+          "qImageFns": cell(q_names), "utmQ": utm_of(q_utm),
+          "numImages": float(len(db_names)), "numQueries": float(len(q_names))}
+    savemat(osp.join(raw, "tokyo247.mat"), {"dbStruct": st})
     return root
 
 

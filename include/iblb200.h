@@ -377,7 +377,8 @@ int ibl_selftest_tc(ibl_engine* e, float* max_rel_err);
 /* One 3x3/s1/p1 conv layer in isolation (test hook): x NHWC [N,H,W,Cin] fp32, w OIHW, optional
  * ReLU and fused 2x2 max-pool, y NHWC fp32.  mode: IBL_CONV_SIMT_FP32, IBL_CONV_TC_BF16X3 (fp32
  * epilogue) or 2 (tensor cores with the bf16 hi/lo plane epilogue, converted back to fp32).
- * bn_override forces the N tile (64/128) when it divides Cout, 0 = default. Synchronises. */
+ * bn_override forces the N tile (64/128) of the 128-pixel kernels when it divides Cout, 0 = default.
+ * Synchronises. */
 int ibl_debug_conv3x3(ibl_engine* e, const float* x_nhwc, int N, int H, int W, int cin,
                       const float* w_oihw, const float* bias, int cout, int relu, int pool, int mode,
                       int bn_override, float* y_nhwc, void* stream);
@@ -395,6 +396,14 @@ int ibl_debug_umma_strided(ibl_engine* e, const void* A, int rows, const void* B
  * patch: view row m is row s0 + ((m%64)/8)*group_rows + (m/64)*half_rows + (m%8)), base_offset 0. */
 int ibl_debug_umma_halo_view(ibl_engine* e, const void* A, int rows, const void* B, int s0, int group_rows,
                              int half_rows, float* D, void* stream);
+/* Register-A probe of the 256-pixel conv kernel: D[64,n] = W . view(X)^T on the tensor cores (wgmma, W's fragments
+ * loaded by ldmatrix from a TMA-staged, 128B-swizzled [64][64] bf16 tile) where view row j (n = 64 or 128) is row
+ * s0 + (j/8)*pitch + (j%8) of the TMA-staged halo tile X = [hrows][pitch][64] bf16. */
+int ibl_debug_wgmma_rs_halo_view(ibl_engine* e, const void* W, const void* X, int pitch, int hrows, int n, int s0,
+                                 float* D, void* stream);
+/* Test and timing hook, process-wide: which 3x3 conv kernel later tensor-core conv launches use.  0 = chosen from the
+ * layer's shape, 1 = the 128-pixel kernels, 2 = the 256-pixel kernel (64 output channels x 256 pixels per tile). */
+int ibl_debug_set_conv3x3_variant(ibl_engine* e, int variant);
 /* The fused conv1_1 + ReLU + conv1_2 + ReLU + 2x2 max-pool kernel of the forward alone, weights from the engine
  * (ibl_engine_set_vgg16): x NCHW [N,3,H,W] fp32, y_hi / y_lo the bf16 hi/lo planes [N,H/2,W/2,64] (device). */
 int ibl_debug_conv1_fused(ibl_engine* e, const float* x, int N, int H, int W, void* y_hi, void* y_lo, void* stream);

@@ -106,6 +106,8 @@ SIGNATURES = {
     "ibl_debug_gemm_tn": (c_int, [_P, _P, _P, _P, _P]),
     "ibl_debug_umma_strided": (c_int, [_P, _P, c_int, _P, c_int, c_int, c_int, _P, _P]),
     "ibl_debug_umma_halo_view": (c_int, [_P, _P, c_int, _P, c_int, c_int, c_int, _P, _P]),
+    "ibl_debug_wgmma_rs_halo_view": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, _P, _P]),
+    "ibl_debug_set_conv3x3_variant": (c_int, [_P, c_int]),
     "ibl_debug_conv1_fused": (c_int, [_P, _P, c_int, c_int, c_int, _P, _P, _P]),
     "ibl_debug_time_layer": (c_int, [_P, c_int, _P, c_int, c_int, c_int, c_int, c_int, POINTER(c_float)]),
     "ibl_debug_conv3x3": (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P, _P, c_int, c_int, c_int, c_int,

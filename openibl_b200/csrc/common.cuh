@@ -173,6 +173,7 @@ int launch_conv1_1_tc(const float* x_nchw, const float* w_oihw, const float* bia
 // tc_probe.cu
 int debug_gmma_strided(const void* A, int rows, const void* B, int s0, int group_rows, int half_rows, int base_mode,
                        float* D, cudaStream_t s);
+int debug_wgmma_rs_halo(const void* W, const void* X, int pitch, int hrows, int n, int s0, float* D, cudaStream_t s);
 // tc_netvlad.cu
 int debug_gemm_tn(const float* A, const float* B, float* C, cudaStream_t s);
 int netvlad_tc_units(int B, int S);

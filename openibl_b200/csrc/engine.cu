@@ -15,6 +15,7 @@ namespace ibl {
 static thread_local std::string g_last_error;
 void set_last_error(const std::string& s) { g_last_error = s; }
 void tc_set_bn_override(int bn);
+void tc_set_variant_override(int v);
 
 static const ConvLayer kVgg16[13] = {
     {3, 64, true, false},    {64, 64, true, true},     // block 1
@@ -193,7 +194,7 @@ int vgg_forward_impl(ibl_engine* e, const float* x, int N, int H, int W, float* 
     const size_t out_elems = (size_t)N * oh * ow * L.cout;
     if (last && planes_out) {
       // fused-NetVLAD path: conv5_3 leaves hi/lo planes + per-pixel |x|^2 partials instead of fp32
-      IBL_RET(e->ssq.ensure((size_t)8 * N * oh * ow * sizeof(float)));
+      IBL_RET(e->ssq.ensure((size_t)(L.cout / 16) * N * oh * ow * sizeof(float)));   // at most one partial per 16 channels
       IBL_RET(launch_conv3x3_tc(hi_of(cur, in_elems), lo_of(cur, in_elems), e->conv[l], N, h, w, L.cin,
                                 L.cout, L.relu, L.pool, hi_of(cur ^ 1, out_elems), lo_of(cur ^ 1, out_elems),
                                 nullptr, s, e->ssq.as<float>(), &planes_out->ssq_parts));
@@ -1340,6 +1341,20 @@ int ibl_debug_umma_halo_view(ibl_engine* e, const void* A, int rows, const void*
   DeviceGuard g(e->device);
   e->launches += 1;
   return debug_gmma_strided(A, rows, B, s0, group_rows, half_rows, 0, D, S(stream));
+}
+
+int ibl_debug_wgmma_rs_halo_view(ibl_engine* e, const void* W, const void* X, int pitch, int hrows, int n, int s0,
+                                 float* D, void* stream) {
+  IBL_REQUIRE(e && W && X && D, "null argument");
+  DeviceGuard g(e->device);
+  e->launches += 1;
+  return debug_wgmma_rs_halo(W, X, pitch, hrows, n, s0, D, S(stream));
+}
+
+int ibl_debug_set_conv3x3_variant(ibl_engine* e, int variant) {
+  IBL_REQUIRE(e && variant >= 0 && variant <= 2, "bad argument");
+  tc_set_variant_override(variant);
+  return IBL_OK;
 }
 
 // The fused conv1_1 + ReLU + conv1_2 + ReLU + 2x2 pool kernel alone (test hook), weights from the engine: x NCHW

@@ -231,6 +231,18 @@ __device__ __forceinline__ uint64_t gmma_desc_mnmajor_sw128(uint32_t smem_addr, 
   return d;
 }
 
+// Register A operand of one k16 step (WgmmaRS) out of a K-major SW128 tile (128-byte rows, 1024-byte aligned base):
+// ldmatrix.x4, lane l addressing tile row `row` at k (16 k16 + 8 (l >> 4)): matrices 0-3 are the fragment's rows 0-7
+// and 8-15 at k + 0 and k + 8, so lanes 0-7 / 8-15 / 16-23 / 24-31 name the rows of matrix 0 / 1 / 2 / 3.
+__device__ __forceinline__ void ldsm_a_sw128(uint32_t (&r)[4], uint32_t tile, int row, int k16) {
+  const uint32_t chunk = (uint32_t)(2 * k16 + ((threadIdx.x >> 4) & 1)) ^ (uint32_t)(row & 7);
+  const uint32_t addr = tile + (uint32_t)row * 128u + (chunk << 4);
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr)
+               : "memory");
+}
+
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>

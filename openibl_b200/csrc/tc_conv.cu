@@ -22,6 +22,16 @@
 //                   other issues the next tile's MMAs
 // Epilogue: accumulator -> row-per-thread views (Acc128::rows32), + bias, ReLU, optional fused 2x2 max-pool
 // (warp shuffles), split into hi/lo planes (or fp32 for conv5_3), 16-byte stores.
+//
+// Wide tiles (WTW = 16: 16x16 patches of 256 pixels, the same 384-thread halo staging and ping-pong consumers) swap
+// the operand roles:
+//   M = 64 output channels per tile, A = the weights, loaded into registers by ldmatrix once per k16 step
+//   N = the 256 pixels, B = two n128 views of the halo tile (patch columns 0-7 and 8-15 of all 16 rows), 8-pixel
+//       groups one 18-pixel halo row (2304 B) apart, the second view 8 rows in
+// so each weight fragment serves 256 pixels and the pixels are the only operand the tensor core reads from shared
+// memory.  A thread then holds both pixels of every horizontal and vertical pool pair, so the epilogue is register-local
+// up to one 4-lane transpose per 4 pixels for the NHWC 16-byte stores (conv_wide_epilogue).  (An 8x32 patch, read as
+// four n64 views, tiles 120x160 exactly but measured no faster there than the 128-pixel kernel: DESIGN 5, K1b.)
 #include "common.cuh"
 #include "tc_common.cuh"
 
@@ -79,7 +89,7 @@ int tc_driver_init() { return get_encode_tiled() ? IBL_OK : IBL_ERR_NO_DEVICE; }
 // ---- kernel ---------------------------------------------------------------------------------
 struct ConvTcArgs {
   int N, H, W, cin, cout;
-  int tw_log2;            // TW = 1 << tw_log2 (8 or 16), TH = 128 / TW
+  int tw_log2;            // TW = 1 << tw_log2 (8 or 16), TH = pixels per tile / TW
   int tiles_w, tiles_h;   // patches per image
   int n_tiles;            // cout / BN
   int total_tiles;        // N * tiles_h * tiles_w * n_tiles
@@ -237,26 +247,164 @@ constexpr int TC_HALO_ROWS = TC_HALO_W * TC_HALO_H;
 constexpr int TC_HALO_PLANE = 23 * 1024;        // 180 rows x 128 B = 23040 B, padded to the swizzle period
 constexpr int TC_HALO_STAGE = 2 * TC_HALO_PLANE;
 
-template <int BN, int STAGES, bool HALO = false, int NA = 0>
+// The wide tiles' halo: (16+2) x (16+2) = 324 rows of 128 B per plane, padded to the swizzle period.  Two stages of both
+// planes and three 16 KiB weight taps leave no room for epilogue staging.
+constexpr int TC_WIDE_PX = 256;
+constexpr int TC_WIDE_HALO_PLANE = 41 * 1024;
+
+template <int BN, int STAGES, bool HALO = false, int NA = 0, int WTW = 0>
 struct ConvTcSmem {
   static constexpr int THREADS = HALO ? 384 : 160;
   static constexpr int CONSUMERS = HALO ? 2 : 1;   // consumer warpgroups, each with its own epilogue staging buffer
   static constexpr int B_BYTES = BN * TC_BK * 2;
   static constexpr int STAGE_BYTES = HALO ? 2 * B_BYTES : 2 * TC_A_BYTES + 2 * B_BYTES;
-  static constexpr int A_RING = HALO ? NA * TC_HALO_STAGE : 0;
-  static constexpr int STG = CONSUMERS * ACC_STG_BYTES;
+  static constexpr int HALO_PLANE = WTW ? TC_WIDE_HALO_PLANE : TC_HALO_PLANE;
+  static constexpr int A_RING = HALO ? NA * 2 * HALO_PLANE : 0;
+  static constexpr int STG = WTW ? 0 : CONSUMERS * ACC_STG_BYTES;
   static constexpr int BYTES = A_RING + STAGES * STAGE_BYTES + STG + 1024 /*align slack*/ + 256 /*barriers*/;
 };
 
-template <int BN, int STAGES, bool HALO, int NA>
-__global__ void __launch_bounds__(ConvTcSmem<BN, STAGES, HALO, NA>::THREADS, 1)
+// One wide tile's accumulator: 64 output channels x 256 pixels as two n128 fragments, one per view.  Thread t (warp w,
+// lane l) holds in view v, for patch row i: [4i + e] = pixel (i, 8v + 2(l%4) + (e & 1)) of the channel that accumulator
+// row 16w + l/4 + 8(e >> 1) stands for (see the weight row map in the kernel).
+struct AccWide {
+  float d[2][64];
+};
+
+__device__ __forceinline__ float wide_pick(bool swap, float a, float b) { return swap ? b : a; }
+
+// In-place transpose of x[4][2] across the four lanes l, l ^ 4, l ^ 8, l ^ 12 (index j = (l >> 2) & 3): afterwards lane j
+// holds in x[p] what lane p held in x[j].
+__device__ __forceinline__ void wide_transpose4(uint32_t (&x)[4][2], int j) {
+#pragma unroll
+  for (int bit = 0; bit < 2; ++bit) {
+    const bool mine = ((j >> bit) & 1) != 0;
+#pragma unroll
+    for (int p0 = 0; p0 < 4; ++p0) {
+      if (p0 & (1 << bit)) continue;
+      const int p1 = p0 | (1 << bit);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const uint32_t got = __shfl_xor_sync(0xffffffffu, mine ? x[p0][h] : x[p1][h], 4 << bit);
+        if (mine) x[p0][h] = got; else x[p1][h] = got;
+      }
+    }
+  }
+}
+
+// Wide tile -> global memory: bias + ReLU + fused 2x2 max-pool + bf16 hi/lo split (or fp32), optional per-pixel sum of
+// squares (one partial per warp: 16 channels).  The thread's two accumulator rows are the adjacent channels
+// c = n0 + 16w + 2(l/4) and c + 1; four pixels at a time go through wide_transpose4, after which lane l stores the 8
+// channels n0 + 16w + 8((l >> 4) & 1) .. + 7 of pixel ((l >> 2) & 3) of the four as one 16-byte word per plane.
+__device__ __forceinline__ void conv_wide_epilogue(const ConvTcArgs& a, const AccWide& acc, int img, int h0, int w0,
+                                                   int nt) {
+  constexpr int NV = 2, TH = 16;
+  const int t = threadIdx.x & 127, w = t >> 5, lane = t & 31, g = lane >> 2, q = lane & 3, j = g & 3;
+  const bool sw = (g >> 2) != 0;                 // rows 16w + g / + 8 are channels c + 1 / c (not c / c + 1)
+  const int c = nt * 64 + 16 * w + 2 * g;
+  const int cst = nt * 64 + 16 * w + 8 * (g >> 2);   // first of the 8 channels this lane stores
+  const float b0 = __ldg(a.bias + c), b1 = __ldg(a.bias + c + 1);
+  auto activate = [&](float& v0, float& v1) {
+    v0 += b0; v1 += b1;
+    if (a.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+  };
+  auto pack = [&](float v0, float v1, uint32_t (&x)[2]) {
+    if (a.y_f32) {
+      x[0] = __float_as_uint(v0); x[1] = __float_as_uint(v1);
+    } else {
+      const __nv_bfloat16 h0b = __float2bfloat16_rn(v0), h1b = __float2bfloat16_rn(v1);
+      __nv_bfloat162 hh(h0b, h1b);
+      x[0] = *reinterpret_cast<uint32_t*>(&hh);
+      x[1] = pack_bf16x2(v0 - __bfloat162float(h0b), v1 - __bfloat162float(h1b));
+    }
+  };
+  auto store = [&](const uint32_t (&x)[4][2], bool valid, long long pix) {
+    if (!valid) return;
+    const long long off = pix * a.cout + cst;
+    if (a.y_f32) {
+      float4* o = reinterpret_cast<float4*>(a.y_f32 + off);
+      o[0] = make_float4(__uint_as_float(x[0][0]), __uint_as_float(x[0][1]), __uint_as_float(x[1][0]), __uint_as_float(x[1][1]));
+      o[1] = make_float4(__uint_as_float(x[2][0]), __uint_as_float(x[2][1]), __uint_as_float(x[3][0]), __uint_as_float(x[3][1]));
+    } else {
+      *reinterpret_cast<uint4*>(a.y_hi + off) = make_uint4(x[0][0], x[1][0], x[2][0], x[3][0]);
+      *reinterpret_cast<uint4*>(a.y_lo + off) = make_uint4(x[0][1], x[1][1], x[2][1], x[3][1]);
+    }
+  };
+  if (a.pool) {
+    // 2x2 max-pool BEFORE bias / ReLU / split, as conv_epilogue_tile: window (b, v) = patch rows 2b, 2b + 1 and columns
+    // 8v + 2q, + 1, all four pixels in this thread; four windows b = 4m .. 4m + 3 per transpose
+    const int OH = a.H >> 1, OW = a.W >> 1;
+    const int ow = (w0 >> 1) + q;   // window column of view 0
+#pragma unroll
+    for (int v = 0; v < NV; ++v)
+#pragma unroll
+      for (int m = 0; m < TH / 8; ++m) {
+        uint32_t x[4][2];
+#pragma unroll
+        for (int p = 0; p < 4; ++p) {
+          const float* r0 = &acc.d[v][4 * (2 * (4 * m + p))];
+          const float* r1 = r0 + 4;
+          const float e0 = fmaxf(fmaxf(r0[0], r0[1]), fmaxf(r1[0], r1[1]));   // accumulator row 16w + g
+          const float e1 = fmaxf(fmaxf(r0[2], r0[3]), fmaxf(r1[2], r1[3]));   // row 16w + g + 8
+          float v0 = wide_pick(sw, e0, e1), v1 = wide_pick(sw, e1, e0);
+          activate(v0, v1);
+          pack(v0, v1, x[p]);
+        }
+        wide_transpose4(x, j);
+        const int oh = (h0 >> 1) + 4 * m + j, owv = ow + 4 * v;
+        store(x, oh < OH && owv < OW && img < a.N, ((long long)img * OH + oh) * OW + owv);
+      }
+    return;
+  }
+#pragma unroll
+  for (int v = 0; v < NV; ++v)
+#pragma unroll
+    for (int b = 0; b < TH / 2; ++b) {
+      // pixels p = (patch row 2b + (p >> 1), column 8v + 2q + (p & 1))
+      uint32_t x[4][2];
+      float sq[4];
+#pragma unroll
+      for (int p = 0; p < 4; ++p) {
+        const float* r = &acc.d[v][4 * (2 * b + (p >> 1)) + (p & 1)];
+        const float e0 = r[0], e1 = r[2];
+        float v0 = wide_pick(sw, e0, e1), v1 = wide_pick(sw, e1, e0);
+        activate(v0, v1);
+        sq[p] = fmaf(v1, v1, v0 * v0);
+        pack(v0, v1, x[p]);
+      }
+      wide_transpose4(x, j);
+      const int h = h0 + 2 * b + (j >> 1), wc = w0 + 8 * v + 2 * q + (j & 1);
+      const bool valid = h < a.H && wc < a.W && img < a.N;
+      const long long pix = ((long long)img * a.H + h) * a.W + wc;
+      store(x, valid, pix);
+      if (a.ssq) {
+        // |x|^2 over the warp's 16 channels: the eight lanes of a pixel column (l ^ 4, l ^ 8, l ^ 16), in a fixed order
+        float mine = 0.f;
+#pragma unroll
+        for (int p = 0; p < 4; ++p) {
+          float s2 = sq[p];
+          s2 += __shfl_xor_sync(0xffffffffu, s2, 4);
+          s2 += __shfl_xor_sync(0xffffffffu, s2, 8);
+          s2 += __shfl_xor_sync(0xffffffffu, s2, 16);
+          if (p == j) mine = s2;
+        }
+        if (valid && g < 4) a.ssq[(long long)(nt * 4 + w) * a.ssq_stride + pix] = mine;
+      }
+    }
+}
+
+template <int BN, int STAGES, bool HALO, int NA, int WTW = 0>
+__global__ void __launch_bounds__(ConvTcSmem<BN, STAGES, HALO, NA, WTW>::THREADS, 1)
 conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tm_xhi, const __grid_constant__ CUtensorMap tm_xlo,
                   const __grid_constant__ CUtensorMap tm_whi, const __grid_constant__ CUtensorMap tm_wlo,
                   const ConvTcArgs a) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // 1024-byte alignment is required by the 128B swizzle; dynamic smem base is only 16B-aligned
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  using L = ConvTcSmem<BN, STAGES, HALO, NA>;
+  using L = ConvTcSmem<BN, STAGES, HALO, NA, WTW>;
+  constexpr int HALO_PLANE = L::HALO_PLANE;
+  constexpr int HALO_STAGE = 2 * HALO_PLANE;
+  constexpr int PX = WTW ? TC_WIDE_PX : TC_BM;   // pixels per tile
   constexpr int B_BYTES = L::B_BYTES;
   constexpr int STAGE_BYTES = L::STAGE_BYTES;
   constexpr int A_RING = L::A_RING;           // HALO: the halo ring sits in front of the weight ring
@@ -304,7 +452,7 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tm_xhi, const __grid_const
     const int pt = tile / a.n_tiles;
     img = pt / tiles_per_img;
     const int rem = pt - img * tiles_per_img;
-    h0 = (rem / a.tiles_w) * (TC_BM >> a.tw_log2);
+    h0 = (rem / a.tiles_w) * (PX >> a.tw_log2);
     w0 = (rem % a.tiles_w) * TW;
   };
 
@@ -354,12 +502,12 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tm_xhi, const __grid_const
           img = (int)warp_uniform((uint32_t)img); h0 = (int)warp_uniform((uint32_t)h0);
           w0 = (int)warp_uniform((uint32_t)w0);
           const int c0 = (int)warp_uniform((uint32_t)(kcA * TC_BK));
-          const uint32_t sa = smem_a + as_u * TC_HALO_STAGE;
-          constexpr uint32_t kHaloBytes = 2u * TC_HALO_ROWS * 128u;
+          const uint32_t sa = smem_a + as_u * HALO_STAGE;
+          constexpr uint32_t kHaloBytes = WTW ? 2u * (WTW + 2) * (TC_WIDE_PX / WTW + 2) * 128u : 2u * TC_HALO_ROWS * 128u;
           if (elect_one()) {
             mbar_arrive_expect_tx_a(afull_a + 8 * as_u, kHaloBytes);
             tma_load_4d_a(sa, &tm_xhi, afull_a + 8 * as_u, c0, w0 - 1, h0 - 1, img);
-            tma_load_4d_a(sa + TC_HALO_PLANE, &tm_xlo, afull_a + 8 * as_u, c0, w0 - 1, h0 - 1, img);
+            tma_load_4d_a(sa + HALO_PLANE, &tm_xlo, afull_a + 8 * as_u, c0, w0 - 1, h0 - 1, img);
           }
           __syncwarp();
           if (++astage == NA) { astage = 0; aphase ^= 1; }
@@ -414,7 +562,89 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tm_xhi, const __grid_const
     auto release_w = [&](int st) {          // this warp is done reading weight slot st
       if (lane == 0) mbar_arrive(&empty_bar[st]);
     };
-    if constexpr (HALO) {
+    if constexpr (WTW != 0) {
+    // ================= wide tiles: two consumer warpgroups (ping-pong), weights in registers =================
+    setmaxnreg_inc<232>();
+    static_assert(WTW == 16, "the wide tiles are 16x16 patches");
+    constexpr int NV = 2;                         // n128 pixel views per tap
+    const int cw = warp / 4 - 1;
+    // Weight row map: accumulator rows 16w + j and 16w + j + 8 (j < 8) read output channels 16w + 2j + s and
+    // 16w + 2j + (s ^ 1), s = j >> 2: a thread's two rows are adjacent channels, and the eight rows of each ldmatrix
+    // phase fall on eight distinct 128B-swizzle phases (no bank conflicts).  Lane l addresses row 16w + (l & 7) + 8 bit3(l).
+    const int wq = (threadIdx.x >> 5) & 3, jl = lane & 7, hl = (lane >> 3) & 1;
+    const int wrow = 16 * wq + 2 * jl + (hl ^ (jl >> 2));
+    const uint32_t halo_w = (uint32_t)WTW + 2;     // halo row pitch (pixels): the views' 8-pixel group stride
+    const uint64_t halo_desc = ((uint64_t)1 << 16) | ((uint64_t)((halo_w * 128) >> 4) << 32) | ((uint64_t)1 << 62);
+    // Ring arithmetic and order barrier as in the 128-pixel halo kernel below.
+    for (int i = cw; worker + i * n_workers < a.total_tiles; i += 2) {
+      int img, h0, w0, nt;
+      coords(worker + i * n_workers, img, h0, w0, nt);
+      int astage = (i * kchunks) % NA, stage = (i * kiters) % STAGES;
+      uint32_t aphase = (uint32_t)((i * kchunks) / NA) & 1u, phase = (uint32_t)((i * kiters) / STAGES) & 1u;
+      if (i > 0) mbar_wait(&order_bar[cw], (uint32_t)((i - 1) >> 1) & 1u);
+      AccWide acc;
+      int prev = -1, prev_a = -1, kc = 0, tap = 0;
+      // The weight fragments of one k16 step go into f[k & 1] while the previous step's MMAs run: 16 registers next to
+      // the 128 of the accumulator (the kernel is compiled for 168).
+      uint32_t f[2][2][4];
+      for (int kit = 0; kit < kiters; ++kit) {
+        if (tap == 0) mbar_wait(&afull_bar[astage], aphase);
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sb = ring_a + stage * STAGE_BYTES;
+        ldsm_a_sw128(f[0][0], sb, wrow, 0);
+        ldsm_a_sw128(f[0][1], sb + B_BYTES, wrow, 0);
+        const uint32_t ha = smem_a + astage * HALO_STAGE;
+        const uint32_t toff = ((uint32_t)(tap / 3) * halo_w + (uint32_t)(tap % 3)) * 128u;
+        const uint64_t x_hi = halo_desc | (uint64_t)(((ha + toff) >> 4) & 0x3fffu);
+        const uint64_t x_lo = halo_desc | (uint64_t)(((ha + HALO_PLANE + toff) >> 4) & 0x3fffu);
+        const uint32_t acc0 = (kc > 0 || tap > 0) ? 1u : 0u;
+#pragma unroll
+        for (int k = 0; k < TC_BK / 16; ++k) {
+          const uint32_t(&fh)[4] = f[k & 1][0];
+          const uint32_t(&fl)[4] = f[k & 1][1];
+          const uint64_t ko = (uint64_t)(k * 2);
+          wgmma_fence();
+          // view v starts 8v pixels into patch row 0: +1 KiB
+#pragma unroll
+          for (int v = 0; v < NV; ++v) WgmmaRS<256 / NV>::mma(acc.d[v], fh, x_lo + 64 * v + ko, (acc0 | k) ? 1u : 0u);
+#pragma unroll
+          for (int v = 0; v < NV; ++v) WgmmaRS<256 / NV>::mma(acc.d[v], fl, x_hi + 64 * v + ko, 1u);
+#pragma unroll
+          for (int v = 0; v < NV; ++v) WgmmaRS<256 / NV>::mma(acc.d[v], fh, x_hi + 64 * v + ko, 1u);
+          wgmma_commit();
+          if (k == 3 && kc == kchunks - 1 && tap == 8 && lane == 0) mbar_arrive(&order_bar[cw ^ 1]);
+          wgmma_wait<1>();                    // the previous k16 step's MMAs have retired: its fragments are free
+          if (k == 0) {                       // ... and the previous tap's weight slot, and after the first tap of a
+            if (prev >= 0) release_w(prev);   // chunk the previous chunk's halo slot
+            if (prev_a >= 0) {
+              if (lane == 0) mbar_arrive(&aempty_bar[prev_a]);
+              prev_a = -1;
+            }
+          }
+          if (k + 1 < TC_BK / 16) {
+            ldsm_a_sw128(f[(k + 1) & 1][0], sb, wrow, k + 1);
+            ldsm_a_sw128(f[(k + 1) & 1][1], sb + B_BYTES, wrow, k + 1);
+          }
+        }
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        if (++tap == 9) {
+          tap = 0;
+          ++kc;
+          prev_a = astage;
+          if (++astage == NA) { astage = 0; aphase ^= 1; }
+        }
+      }
+      wgmma_wait<0>();
+#pragma unroll
+      for (int v = 0; v < NV; ++v)
+#pragma unroll
+        for (int e = 0; e < 128 / NV; ++e) asm volatile("" : "+f"(acc.d[v][e])::"memory");
+      release_w(prev);
+      if (lane == 0) mbar_arrive(&aempty_bar[prev_a]);
+      conv_wide_epilogue(a, acc, img, h0, w0, nt);
+    }
+    } else if constexpr (HALO) {
     // ================= two consumer warpgroups (ping-pong): main loop + epilogue =================
     setmaxnreg_inc<232>();
     const int cw = warp / 4 - 1;            // consumer 0 / 1
@@ -443,7 +673,7 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tm_xhi, const __grid_const
       int prev = -1, prev_a = -1;
       for (int kc = 0; kc < kchunks; ++kc) {
         mbar_wait(&afull_bar[astage], aphase);
-        const uint32_t ha = smem_a + astage * TC_HALO_STAGE;
+        const uint32_t ha = smem_a + astage * HALO_STAGE;
         for (int tap = 0; tap < 9; ++tap) {
           mbar_wait(&full_bar[stage], phase);
           const uint32_t toff = ((uint32_t)(tap / 3) * halo_w + (uint32_t)(tap % 3)) * 128u;
@@ -523,25 +753,29 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tm_xhi, const __grid_const
 }
 
 // ---- host launcher --------------------------------------------------------------------------
-template <int BN, int STAGES, bool HALO = false, int NA = 0>
+template <int BN, int STAGES, bool HALO = false, int NA = 0, int WTW = 0>
 static int launch_tc_variant(const CUtensorMap& xhi, const CUtensorMap& xlo, const CUtensorMap& whi,
                              const CUtensorMap& wlo, const ConvTcArgs& a, cudaStream_t s) {
-  constexpr int smem = ConvTcSmem<BN, STAGES, HALO, NA>::BYTES;
+  constexpr int smem = ConvTcSmem<BN, STAGES, HALO, NA, WTW>::BYTES;
   static_assert(smem <= 232448, "shared-memory budget");
   static DeviceOnce attr_done;   // the attribute is per device
   if (!attr_done.done()) {
-    IBL_CUDA_OK(cudaFuncSetAttribute(conv3x3_tc_kernel<BN, STAGES, HALO, NA>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    IBL_CUDA_OK(cudaFuncSetAttribute(conv3x3_tc_kernel<BN, STAGES, HALO, NA, WTW>,
+                                     cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     attr_done.mark();
   }
   const int sms = device_sm_count();
   const int grid = a.total_tiles < sms ? a.total_tiles : sms;
-  conv3x3_tc_kernel<BN, STAGES, HALO, NA><<<grid, ConvTcSmem<BN, STAGES, HALO, NA>::THREADS, smem, s>>>(xhi, xlo, whi, wlo, a);
+  conv3x3_tc_kernel<BN, STAGES, HALO, NA, WTW>
+      <<<grid, ConvTcSmem<BN, STAGES, HALO, NA, WTW>::THREADS, smem, s>>>(xhi, xlo, whi, wlo, a);
   IBL_CUDA_OK(cudaGetLastError());
   return IBL_OK;
 }
 
-static int g_tc_bn_override = 0;   // test hook: force BN (64/128) where it divides Cout
+static int g_tc_bn_override = 0;   // test hook: force BN (64/128) of the 128-pixel kernels where it divides Cout
 void tc_set_bn_override(int bn) { g_tc_bn_override = bn; }
+static int g_tc_variant_override = 0;   // test hook: 1 forces the 128-pixel kernels, 2 the 256-pixel one
+void tc_set_variant_override(int v) { g_tc_variant_override = v; }
 
 int launch_conv3x3_tc(const __nv_bfloat16* x_hi, const __nv_bfloat16* x_lo, const ConvParams& p,
                       int N, int H, int W, int cin, int cout, bool relu, bool pool,
@@ -552,31 +786,43 @@ int launch_conv3x3_tc(const __nv_bfloat16* x_hi, const __nv_bfloat16* x_lo, cons
   IBL_REQUIRE(H >= 1 && W >= 1 && N >= 1, "empty conv input");
   ConvTcArgs a{};
   a.N = N; a.H = H; a.W = W; a.cin = cin; a.cout = cout;
-  // patch shape: 8x16 or 16x8, whichever wastes fewer accumulator rows
-  auto waste = [&](int tw) {
-    int th = 128 / tw;
+  // patch shape of the 128-pixel kernels: 8x16 or 16x8, whichever wastes fewer accumulator rows (pixels computed for
+  // the map)
+  auto waste = [&](int tw, int px) {
+    int th = px / tw;
     return (long long)cdiv(W, tw) * tw * cdiv(H, th) * th;
   };
-  a.tw_log2 = (waste(16) <= waste(8)) ? 4 : 3;
-  const int TW = 1 << a.tw_log2, TH = 128 / TW;
+  const int tw128 = (waste(16, 128) <= waste(8, 128)) ? 16 : 8;
+  // The 256-pixel kernel (64 output channels x 256 pixels per tile, weights in registers) on 16x16 patches wherever
+  // they waste no more rows than the 128-pixel kernels: conv2_x and conv4_x at 480x640, not conv3_x at 120x160 (8x16
+  // tiles it exactly, 16x16 wastes 6.7 %) or conv5_x at 30x40 (28 %).  The kernel's 8x32 patch tiles 120x160 exactly
+  // but measured no faster there than the 128-pixel kernel (DESIGN 5, K1b), so it is not built.  Like the N tile below,
+  // the choice depends on the layer's shape only, never on the batch, so an image's descriptor does not depend on the
+  // batch it travels in (tests: bit-identical across batch compositions).
+  constexpr int tw256 = 16;
+  bool wide = waste(tw256, 256) <= waste(tw128, 128);
+  if (g_tc_bn_override) wide = false;
+  if (g_tc_variant_override) wide = g_tc_variant_override == 2;
+  const int TW = wide ? tw256 : tw128, TH = (wide ? TC_WIDE_PX : TC_BM) / TW;
+  a.tw_log2 = TW == 16 ? 4 : 3;
   a.tiles_w = cdiv(W, TW);
   a.tiles_h = cdiv(H, TH);
-  // N tile: 128 where Cout allows (the accumulator is 128 registers per consumer thread), 64 for Cout = 64.  The
-  // choice depends on Cout only, never on the batch, so an image's descriptor does not depend on the batch it
-  // travels in (tests: bit-identical across batch compositions).
-  int bn = cout % 128 == 0 ? 128 : 64;
-  if (g_tc_bn_override && cout % g_tc_bn_override == 0 && (g_tc_bn_override == 64 || g_tc_bn_override == 128))
+  // N tile of the 128-pixel kernels: 128 where Cout allows (the accumulator is 128 registers per consumer thread), 64
+  // for Cout = 64; the 256-pixel kernel's tile is 64 channels.
+  int bn = wide ? 64 : cout % 128 == 0 ? 128 : 64;
+  if (!wide && g_tc_bn_override && cout % g_tc_bn_override == 0 && (g_tc_bn_override == 64 || g_tc_bn_override == 128))
     bn = g_tc_bn_override;
-  // Halo staging on the 128-wide tiles.  The choice depends on Cout only, never on the batch (the two kernels walk K in
-  // different orders); the patch shape only moves pixels between accumulator rows, not the order of any pixel's sums.
-  const bool halo = bn == 128;
+  // Halo staging on the 128-wide and the 256-pixel tiles.  The 128-pixel kernels walk K in different orders, so the
+  // choice depends on Cout only; the patch shape only moves pixels between accumulator rows, not the order of any
+  // pixel's sums.
+  const bool halo = wide || bn == 128;
   a.n_tiles = cout / bn;
   a.total_tiles = (int)((long long)N * a.tiles_h * a.tiles_w * a.n_tiles);
   a.relu = relu; a.pool = pool;
   a.bias = p.bias; a.y_hi = y_hi; a.y_lo = y_lo; a.y_f32 = y_f32;
   a.ssq = pool ? nullptr : ssq;
   a.ssq_stride = (long long)N * H * W;
-  if (ssq_parts) *ssq_parts = a.n_tiles;
+  if (ssq_parts) *ssq_parts = wide ? cout / 16 : a.n_tiles;   // the 256-pixel kernel writes one partial per warp
 
   CUtensorMap m_xhi, m_xlo, m_whi, m_wlo;
   {
@@ -593,6 +839,7 @@ int launch_conv3x3_tc(const __nv_bfloat16* x_hi, const __nv_bfloat16* x_lo, cons
     IBL_RET(make_tmap(&m_whi, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, p.w_hi, dims, str, box));
     IBL_RET(make_tmap(&m_wlo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, p.w_lo, dims, str, box));
   }
+  if (wide) return launch_tc_variant<64, 3, true, 2, 16>(m_xhi, m_xlo, m_whi, m_wlo, a, s);
   if (halo) return launch_tc_variant<128, 3, true, 2>(m_xhi, m_xlo, m_whi, m_wlo, a, s);
   return launch_tc_variant<64, 4>(m_xhi, m_xlo, m_whi, m_wlo, a, s);
 }

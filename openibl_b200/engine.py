@@ -721,7 +721,8 @@ class Engine:
         return gx
 
     # ---- test hooks ----------------------------------------------------------------------
-    def debug_conv3x3(self, x_nhwc, w_oihw, bias, relu=True, pool=False, mode=CONV_TC_BF16X3, bn=0):
+    def debug_conv3x3(self, x_nhwc, w_oihw, bias, relu=True, pool=False, mode=CONV_TC_BF16X3, bn=0, variant=0):
+        """One conv layer alone; `variant` 1 / 2 forces the 128-pixel / 256-pixel tensor-core kernel (0: by shape)."""
         x = _require_cuda(x_nhwc, "x")
         w = _require_cuda(w_oihw, "w")
         b = _require_cuda(bias, "bias")
@@ -729,9 +730,13 @@ class Engine:
         cout = w.shape[0]
         oh, ow = (H // 2, W // 2) if pool else (H, W)
         y = torch.empty(N, oh, ow, cout, device=x.device)
-        check(self.lib.ibl_debug_conv3x3(self.h, _ptr(x), N, H, W, cin, _ptr(w), _ptr(b), cout, int(relu),
-                                         int(pool), int(mode), int(bn), _ptr(y), _stream(self.device)),
-              "ibl_debug_conv3x3")
+        check(self.lib.ibl_debug_set_conv3x3_variant(self.h, int(variant)), "ibl_debug_set_conv3x3_variant")
+        try:
+            check(self.lib.ibl_debug_conv3x3(self.h, _ptr(x), N, H, W, cin, _ptr(w), _ptr(b), cout, int(relu),
+                                             int(pool), int(mode), int(bn), _ptr(y), _stream(self.device)),
+                  "ibl_debug_conv3x3")
+        finally:
+            self.lib.ibl_debug_set_conv3x3_variant(self.h, 0)
         return y
 
     def debug_conv1_fused(self, x_nchw):

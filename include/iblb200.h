@@ -141,6 +141,18 @@ int ibl_vlad_normalize(ibl_engine* e, const float* vlad_raw, int N, int K, int C
  * v [N,D], W [P,D], b [P] -> out [N,P]. */
 int ibl_pca_l2(ibl_engine* e, const float* v, int N, int D, const float* W, const float* b,
                int P, float* out, void* stream);
+/* Training surface of the PCA layer (EmbedNetPCA trained end to end: autograd through netvlad.py:105-107 in the
+ * reference; the L2 of :108 stays with the caller).
+ * Forward: y = v W^T + b, v [N,D], W [P,D], b [P] -> y [N,P] before the L2, any N >= 1, P <= 12288.
+ * Backward, given gy = dL/dy [N,P]: gv = gy W [N,D], gW = gy^T v [P,D], gb = sum over rows of gy [P].  Each of gv, gW,
+ * gb may be NULL (a frozen layer skips the [P,D] write, a frozen trunk + NetVLAD skips gv); W is read only for gv, v
+ * only for gW.  In the tensor-core math mode with D % 64 == 0 both GEMMs run as bf16x3 wgmma kernels and need the
+ * planes of this W: call ibl_engine_set_pca(e, W, b, P, D) first (IBL_ERR_NOT_READY otherwise); with D % 64 != 0 or
+ * IBL_CONV_SIMT_FP32 (ibl_engine_set_gemm_mode) they run on fp32 CUDA cores. */
+int ibl_pca_forward_train(ibl_engine* e, const float* v, int N, int D, const float* W, const float* b, int P,
+                          float* y, void* stream);
+int ibl_pca_backward(ibl_engine* e, const float* v, int N, int D, const float* W, int P, const float* gy,
+                     float* gv, float* gW, float* gb, void* stream);
 /* F.normalize(x, p=2, dim=-1) (evaluators.py:29-33): rows [N,D] in place or to out. */
 int ibl_l2_normalize_rows(ibl_engine* e, const float* x, int N, int D, float* out, void* stream);
 

@@ -70,6 +70,8 @@ SIGNATURES = {
     "ibl_netvlad_backward": (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P, _P, c_int, c_int, _P, _P, _P, _P, _P]),
     "ibl_vlad_normalize": (c_int, [_P, _P, c_int, c_int, c_int, _P, _P]),
     "ibl_pca_l2": (c_int, [_P, _P, c_int, c_int, _P, _P, c_int, _P, _P]),
+    "ibl_pca_forward_train": (c_int, [_P, _P, c_int, c_int, _P, _P, c_int, _P, _P]),
+    "ibl_pca_backward": (c_int, [_P, _P, c_int, c_int, _P, c_int, _P, _P, _P, _P, _P]),
     "ibl_l2_normalize_rows": (c_int, [_P, _P, c_int, c_int, _P, _P]),
     "ibl_extract": (c_int, [_P, _P, c_int, c_int, c_int, c_uint, _P, _P, _P]),
     "ibl_extract_host": (c_int, [_P, _P, c_int, c_int, c_int, c_uint, _P, _P, _P]),

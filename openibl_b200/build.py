@@ -10,7 +10,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libiblb200.so")
-SOURCES = ["engine.cu", "simt_conv.cu", "netvlad.cu", "gemm_simt.cu", "topk.cu", "tc_conv.cu", "tc_gemm.cu", "tc_netvlad.cu", "tc_conv1.cu", "tc_probe.cu", "netvlad_bwd.cu", "tc_dist1.cu", "tc_conv_bwd.cu", "resize.cu", "sort_rows.cu", "rerank.cu", "jpeg.cu", "png.cu", "color_jitter.cu"]
+SOURCES = ["engine.cu", "simt_conv.cu", "netvlad.cu", "gemm_simt.cu", "topk.cu", "tc_conv.cu", "tc_gemm.cu", "tc_netvlad.cu", "tc_conv1.cu", "tc_probe.cu", "netvlad_bwd.cu", "tc_dist1.cu", "tc_conv_bwd.cu", "resize.cu", "sort_rows.cu", "rerank.cu", "jpeg.cu", "png.cu", "color_jitter.cu", "tc_pca_bwd.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",

@@ -213,8 +213,18 @@ int launch_pca_partial_tc(const __nv_bfloat16* w_hi, const __nv_bfloat16* w_lo, 
 int launch_rescore_sort(const float* q, const float* qn, int m, const float* db, const float* dbn, int d,
                         const long long* cand_i, int kc, int k_out, long long idx_base, float* out_dist,
                         long long* out_idx, cudaStream_t s);
+// out = bias + sum of the partials, then L2 per row when `normalize` (false: the pre-normalisation y of training)
 int launch_pca_finalize(const float* partial, int splits, int N, int P, const float* bias, float* out,
-                        cudaStream_t s);
+                        cudaStream_t s, bool normalize = true);
+// tc_pca_bwd.cu: backward of the PCA layer (gy planes [N][Pp], Pp = P rounded up to 8)
+int launch_pca_gy_planes(const float* gy, int N, int P, int Pp, __nv_bfloat16* hi, __nv_bfloat16* lo, cudaStream_t s);
+int launch_pca_dgrad_tc(const __nv_bfloat16* w_hi, const __nv_bfloat16* w_lo, int P, int D, const __nv_bfloat16* g_hi,
+                        const __nv_bfloat16* g_lo, int Pp, int N, float* gv, cudaStream_t s);
+int launch_pca_wgrad_tc(const __nv_bfloat16* v_hi, const __nv_bfloat16* v_lo, int N, int D, const __nv_bfloat16* g_hi,
+                        const __nv_bfloat16* g_lo, int P, int Pp, float* gW, cudaStream_t s);
+int launch_pca_bias_grad(const float* gy, int N, int P, float* gb, cudaStream_t s);
+int launch_pca_tn_simt(const float* A, long long sr, long long sk, int R, int K, const float* B, int D, float* C,
+                       cudaStream_t s);
 
 // netvlad.cu
 struct NetvladWorkspace {
@@ -240,7 +250,7 @@ int launch_netvlad_backward(const float* x, bool nhwc, int N, int C, int S, cons
 
 // gemm_simt.cu  (C = A[m,K] . B[n,K]^T family)
 int launch_pca_l2(const float* v, int N, int D, const float* W, const float* b, int P,
-                  float* partial, int splits, float* out, cudaStream_t s, uint64_t* launches);
+                  float* partial, int splits, float* out, cudaStream_t s, uint64_t* launches, bool normalize = true);
 int launch_l2_normalize_rows(const float* x, int N, int D, float* out, cudaStream_t s);
 int launch_row_sqnorm(const float* x, int N, int D, float* out, cudaStream_t s);
 int launch_scale(const float* x, float s, int n, float* y, cudaStream_t st);

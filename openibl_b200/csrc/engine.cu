@@ -79,6 +79,7 @@ struct ibl_engine {
   DevBuf stage_in, stage_out, stage_out2, stage_u8;
   DevBuf q_pl, db_pl, v_pl, pca_pl;     // bf16 hi|lo planes of queries, database shard, descriptors, PCA W
   const float* pca_pl_src = nullptr;    // W pointer the cached planes were made from
+  DevBuf pca_gy_pl;                     // PCA backward: bf16 hi|lo planes of dL/dy, rows padded to 8 columns
   DevBuf mrg_d, mrg_i;
   DevBuf bw_g, bw_x, bw_part, bw_w;      // conv backward: dY planes, X planes, wgrad/bias partials, dgrad filter planes
   DevBuf d1_ws;                          // workspace of the single-pass distance/top-k path (tc_dist1.cu)
@@ -278,7 +279,7 @@ int ibl_engine_destroy(ibl_engine* e) {
   DevBuf* bufs[] = {&e->act[0], &e->act[1], &e->feat, &e->nv_assign, &e->nv_inv, &e->nv_raw, &e->vlad,
                     &e->pca_partial, &e->qn, &e->dbn, &e->dist_chunk, &e->cand_d, &e->cand_i,
                     &e->stage_in, &e->stage_out, &e->stage_out2, &e->stage_u8, &e->q_pl, &e->db_pl, &e->v_pl, &e->pca_pl,
-                    &e->mrg_d, &e->mrg_i, &e->d1_ws, &e->bw_g, &e->bw_x, &e->bw_part, &e->bw_w, &e->ssq, &e->nv_part, &e->nv_asum, &e->nvw_pl, &e->nv_ticket};
+                    &e->mrg_d, &e->mrg_i, &e->d1_ws, &e->bw_g, &e->bw_x, &e->bw_part, &e->bw_w, &e->ssq, &e->nv_part, &e->nv_asum, &e->nvw_pl, &e->nv_ticket, &e->pca_gy_pl};
   for (DevBuf* b : bufs) b->release();
   e->knn_ws.release();
   rerank_ws_destroy(e->rr_ws);
@@ -586,11 +587,10 @@ int ibl_vlad_normalize(ibl_engine* e, const float* vlad_raw, int N, int K, int C
   return launch_vlad_normalize(vlad_raw, N, K, C, out, S(stream));
 }
 
-int ibl_pca_l2(ibl_engine* e, const float* v, int N, int D, const float* W, const float* b, int P,
-               float* out, void* stream) {
-  IBL_REQUIRE(e && v && W && b && out, "null argument");
-  IBL_REQUIRE(N >= 1 && P >= 1 && D >= 4, "bad shape");
-  IBL_REQUIRE((size_t)P * sizeof(float) <= 48 * 1024, "PCA output dim above 12288 is not supported");
+// y = v W^T + b, then L2 per row when `normalize`.  Tensor cores when the engine holds planes of this W (set_pca with
+// D % 64 == 0) in the tensor-core math mode, 32 descriptor rows per launch; fp32 CUDA cores otherwise.
+static int pca_project(ibl_engine* e, const float* v, int N, int D, const float* W, const float* b, int P, float* out,
+                       bool normalize, void* stream) {
   DeviceGuard g(e->device);
   if (e->gemm_mode == IBL_CONV_TC_BF16X3 && W == e->pca_pl_src && P == e->pca_P && D == e->pca_D) {
     const size_t nw = (size_t)P * D;
@@ -605,7 +605,7 @@ int ibl_pca_l2(ibl_engine* e, const float* v, int N, int D, const float* W, cons
       int sp = 0;
       IBL_RET(launch_pca_partial_tc(e->pca_pl.as<__nv_bfloat16>(), e->pca_pl.as<__nv_bfloat16>() + nw, P, vh,
                                     vh + nv, nb, D, e->pca_partial.as<float>(), &sp, S(stream)));
-      IBL_RET(launch_pca_finalize(e->pca_partial.as<float>(), sp, nb, P, b, out + (size_t)n0 * P, S(stream)));
+      IBL_RET(launch_pca_finalize(e->pca_partial.as<float>(), sp, nb, P, b, out + (size_t)n0 * P, S(stream), normalize));
       e->launches += 3;
     }
     return IBL_OK;
@@ -617,7 +617,81 @@ int ibl_pca_l2(ibl_engine* e, const float* v, int N, int D, const float* W, cons
   if (splits > 32) splits = 32;
   while (splits > 1 && D / splits < 256) --splits;
   IBL_RET(e->pca_partial.ensure((size_t)splits * N * P * sizeof(float)));
-  return launch_pca_l2(v, N, D, W, b, P, e->pca_partial.as<float>(), splits, out, S(stream), &e->launches);
+  return launch_pca_l2(v, N, D, W, b, P, e->pca_partial.as<float>(), splits, out, S(stream), &e->launches, normalize);
+}
+
+int ibl_pca_l2(ibl_engine* e, const float* v, int N, int D, const float* W, const float* b, int P,
+               float* out, void* stream) {
+  IBL_REQUIRE(e && v && W && b && out, "null argument");
+  IBL_REQUIRE(N >= 1 && P >= 1 && D >= 4, "bad shape");
+  IBL_REQUIRE((size_t)P * sizeof(float) <= 48 * 1024, "PCA output dim above 12288 is not supported");
+  return pca_project(e, v, N, D, W, b, P, out, true, stream);
+}
+
+// The tensor-core training entry points need the engine's planes of this very W: a stale or missing re-layout is an
+// error, not a silent switch to the CUDA-core path.
+static int pca_train_path(ibl_engine* e, const float* W, int P, int D, bool* tc) {
+  *tc = e->gemm_mode == IBL_CONV_TC_BF16X3 && D % 64 == 0;
+  if (*tc && !(W == e->pca_pl_src && P == e->pca_P && D == e->pca_D)) {
+    set_last_error("tensor-core PCA training needs ibl_engine_set_pca with this W (and P, D) first");
+    return IBL_ERR_NOT_READY;
+  }
+  return IBL_OK;
+}
+
+int ibl_pca_forward_train(ibl_engine* e, const float* v, int N, int D, const float* W, const float* b, int P,
+                          float* y, void* stream) {
+  IBL_REQUIRE(e && v && W && b && y, "null argument");
+  IBL_REQUIRE(N >= 1 && P >= 1 && D >= 4 && D % 4 == 0, "bad shape");
+  IBL_REQUIRE((size_t)P * sizeof(float) <= 48 * 1024, "PCA output dim above 12288 is not supported");
+  bool tc = false;
+  IBL_RET(pca_train_path(e, W, P, D, &tc));
+  return pca_project(e, v, N, D, W, b, P, y, false, stream);
+}
+
+int ibl_pca_backward(ibl_engine* e, const float* v, int N, int D, const float* W, int P, const float* gy, float* gv,
+                     float* gW, float* gb, void* stream) {
+  IBL_REQUIRE(e && gy, "null argument");
+  IBL_REQUIRE(!gv || W, "gv needs W");
+  IBL_REQUIRE(!gW || v, "gW needs v");
+  IBL_REQUIRE(N >= 1 && P >= 1 && D >= 4 && D % 4 == 0, "bad shape");
+  DeviceGuard g(e->device);
+  cudaStream_t s = S(stream);
+  bool tc = false;
+  if (gv) IBL_RET(pca_train_path(e, W, P, D, &tc));
+  else tc = e->gemm_mode == IBL_CONV_TC_BF16X3 && D % 64 == 0;
+  if (gb) {
+    IBL_RET(launch_pca_bias_grad(gy, N, P, gb, s));
+    e->launches++;
+  }
+  if (!gv && !gW) return IBL_OK;
+  if (!tc) {
+    if (gv) IBL_RET(launch_pca_tn_simt(gy, P, 1, N, P, W, D, gv, s));
+    if (gW) IBL_RET(launch_pca_tn_simt(gy, 1, P, P, N, v, D, gW, s));
+    e->launches += (gv ? 1 : 0) + (gW ? 1 : 0);
+    return IBL_OK;
+  }
+  const int Pp = (P + 7) / 8 * 8;
+  const size_t ng = (size_t)N * Pp;
+  IBL_RET(e->pca_gy_pl.ensure(ng * 4));
+  __nv_bfloat16* gh = e->pca_gy_pl.as<__nv_bfloat16>();
+  IBL_RET(launch_pca_gy_planes(gy, N, P, Pp, gh, gh + ng, s));
+  e->launches++;
+  if (gv) {
+    const size_t nw = (size_t)P * D;
+    IBL_RET(launch_pca_dgrad_tc(e->pca_pl.as<__nv_bfloat16>(), e->pca_pl.as<__nv_bfloat16>() + nw, P, D, gh, gh + ng, Pp,
+                                N, gv, s));
+    e->launches++;
+  }
+  if (gW) {
+    const size_t nv = (size_t)N * D;
+    IBL_RET(e->v_pl.ensure(nv * 4));
+    __nv_bfloat16* vh = e->v_pl.as<__nv_bfloat16>();
+    IBL_RET(launch_f32_to_planes(v, nv, vh, vh + nv, s));
+    IBL_RET(launch_pca_wgrad_tc(vh, vh + nv, N, D, gh, gh + ng, P, Pp, gW, s));
+    e->launches += 2;
+  }
+  return IBL_OK;
 }
 
 int ibl_l2_normalize_rows(ibl_engine* e, const float* x, int N, int D, float* out, void* stream) {

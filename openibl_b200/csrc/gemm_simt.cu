@@ -114,10 +114,10 @@ __global__ void __launch_bounds__(256) gemm_nt_kernel(GemmArgs g) {
   }
 }
 
-// out[n][p] = normalize( bias[p] + sum_z partial[z][n][p] )
+// out[n][p] = normalize( bias[p] + sum_z partial[z][n][p] ); without `normalize` the sum itself
 __global__ void __launch_bounds__(256)
 pca_finalize_kernel(const float* __restrict__ partial, int splits, int N, int P,
-                    const float* __restrict__ bias, float* __restrict__ out) {
+                    const float* __restrict__ bias, float* __restrict__ out, int normalize) {
   extern __shared__ float row[];  // [P]
   __shared__ float red[8];
   __shared__ float inv_s;
@@ -141,18 +141,22 @@ pca_finalize_kernel(const float* __restrict__ partial, int splits, int N, int P,
   }
   __syncthreads();
   const float inv = inv_s;
-  for (int p = threadIdx.x; p < P; p += blockDim.x) out[n * P + p] = row[p] * inv;
+  if (normalize) {
+    for (int p = threadIdx.x; p < P; p += blockDim.x) out[n * P + p] = row[p] * inv;
+  } else {
+    for (int p = threadIdx.x; p < P; p += blockDim.x) out[n * P + p] = row[p];
+  }
 }
 
 int launch_pca_finalize(const float* partial, int splits, int N, int P, const float* bias, float* out,
-                        cudaStream_t s) {
-  pca_finalize_kernel<<<N, 256, P * sizeof(float), s>>>(partial, splits, N, P, bias, out);
+                        cudaStream_t s, bool normalize) {
+  pca_finalize_kernel<<<N, 256, P * sizeof(float), s>>>(partial, splits, N, P, bias, out, normalize ? 1 : 0);
   IBL_CUDA_OK(cudaGetLastError());
   return IBL_OK;
 }
 
 int launch_pca_l2(const float* v, int N, int D, const float* W, const float* b, int P,
-                  float* partial, int splits, float* out, cudaStream_t s, uint64_t* launches) {
+                  float* partial, int splits, float* out, cudaStream_t s, uint64_t* launches, bool normalize) {
   IBL_REQUIRE(D % 4 == 0, "PCA input dim must be a multiple of 4");
   GemmArgs g{};
   g.A = W; g.lda = D; g.M = P;
@@ -165,7 +169,7 @@ int launch_pca_l2(const float* v, int N, int D, const float* W, const float* b, 
   dim3 grid((unsigned)cdiv(P, G_BM), (unsigned)cdiv(N, G_BN), (unsigned)cdiv(D, kps));
   gemm_nt_kernel<EPI_PCA_PARTIAL><<<grid, 256, 0, s>>>(g);
   IBL_CUDA_OK(cudaGetLastError());
-  pca_finalize_kernel<<<N, 256, P * sizeof(float), s>>>(partial, (int)grid.z, N, P, b, out);
+  pca_finalize_kernel<<<N, 256, P * sizeof(float), s>>>(partial, (int)grid.z, N, P, b, out, normalize ? 1 : 0);
   IBL_CUDA_OK(cudaGetLastError());
   *launches += 2;
   return IBL_OK;

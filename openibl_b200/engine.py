@@ -229,6 +229,43 @@ class Engine:
               "ibl_pca_l2")
         return out
 
+    def pca_forward_train(self, v: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor) -> torch.Tensor:
+        """y = v W^T + b before the L2 (ibl_pca_forward_train).  In the tensor-core math mode the engine must hold the
+        planes of `weight` (set_pca)."""
+        v = _require_cuda(v, "descriptors")
+        P = weight.shape[0]
+        w = _require_cuda(weight.detach().reshape(P, -1), "pca weight")
+        b = _require_cuda(bias.detach().reshape(-1), "pca bias")
+        N, D = v.shape
+        if w.shape[1] != D:
+            raise ValueError(f"PCA expects dim {w.shape[1]}, got {D}")
+        y = torch.empty(N, P, device=v.device)
+        check(self.lib.ibl_pca_forward_train(self.h, _ptr(v), N, D, _ptr(w), _ptr(b), P, _ptr(y), _stream(self.device)),
+              "ibl_pca_forward_train")
+        return y
+
+    def pca_backward(self, v: Optional[torch.Tensor], weight: torch.Tensor, gy: torch.Tensor, need_gv=True,
+                     need_gw=True, need_gb=True):
+        """Backward of y = v W^T + b given gy = dL/dy [N,P] -> (gv [N,D], gW [P,D], gb [P]); what is not needed is None
+        and is not computed.  `v` is read only for gW."""
+        gy = _require_cuda(gy, "grad of the PCA output")
+        P = weight.shape[0]
+        w = _require_cuda(weight.detach().reshape(P, -1), "pca weight")
+        N, D = gy.shape[0], w.shape[1]
+        if gy.shape[1] != P:
+            raise ValueError(f"grad has {gy.shape[1]} columns, the PCA layer {P}")
+        if need_gw:
+            v = _require_cuda(v, "descriptors")
+            if tuple(v.shape) != (N, D):
+                raise ValueError(f"descriptors are {tuple(v.shape)}, expected {(N, D)}")
+        dev = gy.device
+        gv = torch.empty(N, D, device=dev) if need_gv else None
+        gw = torch.empty(P, D, device=dev) if need_gw else None
+        gb = torch.empty(P, device=dev) if need_gb else None
+        check(self.lib.ibl_pca_backward(self.h, _ptr(v if need_gw else None), N, D, _ptr(w), P, _ptr(gy), _ptr(gv),
+                                        _ptr(gw), _ptr(gb), _stream(self.device)), "ibl_pca_backward")
+        return gv, gw, gb
+
     def l2_normalize_rows(self, x: torch.Tensor) -> torch.Tensor:
         x = _require_cuda(x, "rows")
         N, D = x.shape

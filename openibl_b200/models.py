@@ -10,6 +10,7 @@ No CPU path: calling a model on CPU tensors raises.  Training (config 5, SURVEY 
 suffix of the VGG trunk (conv5_x when `train_layers='conv5'`, vgg.py:50-53) are `torch.autograd.Function`s whose
 forward AND backward run in libiblb200 (Hopper wgmma dgrad / wgrad, NetVLAD backward kernels); the region algebra of
 EmbedRegionNet's train branch (sums of quarter VLADs, two normalisations, a 9x9 matmul per pair) stays in torch.
+EmbedNetPCA trains end to end: its PCA layer is a third such Function (tensor-core dgrad / wgrad in libiblb200).
 """
 from __future__ import annotations
 
@@ -77,13 +78,6 @@ class _VGGTrunkFunction(torch.autograd.Function):
             grads[2 * i], grads[2 * i + 1] = gw, gb
             g = gx
         return (None, None, *grads)
-
-
-def _no_train(module: nn.Module, what: str) -> None:
-    if module.training and torch.is_grad_enabled():
-        raise NotImplementedError(
-            f"{what}: only the inference path (model.eval() / torch.no_grad()) is implemented in the "
-            "H100 engine; the training/backward kernels are scheduled next (SURVEY 8f)")
 
 
 class VGG(nn.Module):
@@ -258,6 +252,30 @@ class _NetVLADFunction(torch.autograd.Function):
         return dx, dw.view_as(conv_w), dc, None
 
 
+class _PCALayerFunction(torch.autograd.Function):
+    """autograd bridge for EmbedNetPCA.pca_layer without its L2 (netvlad.py:105-107): y = v W^T + b forward
+    (ibl_pca_forward_train), dgrad / wgrad / bias gradient backward (ibl_pca_backward, tensor-core wgmma kernels).  The
+    gradient of the weight comes back as [P, D, 1, 1], the conv's own layout."""
+
+    @staticmethod
+    def forward(ctx, v, weight, bias):
+        eng = Engine.get(v.device)
+        vc = v.contiguous()
+        y = eng.pca_forward_train(vc, weight, bias)
+        ctx.save_for_backward(vc, weight, bias)
+        return y
+
+    @staticmethod
+    def backward(ctx, gy):
+        v, weight, bias = ctx.saved_tensors
+        eng = Engine.get(gy.device)
+        need_gv, need_gw, need_gb = ctx.needs_input_grad
+        if need_gv:
+            eng.set_pca(weight, bias)     # a no-op unless another PCA layer was bound since the forward
+        gv, gw, gb = eng.pca_backward(v, weight, gy.contiguous(), need_gv=need_gv, need_gw=need_gw, need_gb=need_gb)
+        return gv, (gw.view_as(weight) if need_gw else None), gb
+
+
 class _EmbedBase(nn.Module):
     def __init__(self, base_model, net_vlad):
         super().__init__()
@@ -276,16 +294,16 @@ class _EmbedBase(nn.Module):
         eng.set_netvlad(self.net_vlad.conv.weight, self.net_vlad.centroids)
         return eng
 
-
-class EmbedNet(_EmbedBase):
-    """netvlad.py:63-82: forward -> (pool_x [B,512], vlad_x [B,K*C]) with intra-norm + L2."""
-
     def _train_forward(self, x):
         # differentiable path (netvlad_img.py training): trunk suffix + NetVLAD in libiblb200 through their
         # autograd Functions, the two normalisations (netvlad.py:78-80) as torch ops on [B,64,512]
         pool_x, feat = self.base_model(x)
         v = torch.nn.functional.normalize(self.net_vlad(feat), p=2, dim=2)
         return pool_x, torch.nn.functional.normalize(v.view(x.size(0), -1), p=2, dim=1)
+
+
+class EmbedNet(_EmbedBase):
+    """netvlad.py:63-82: forward -> (pool_x [B,512], vlad_x [B,K*C]) with intra-norm + L2."""
 
     def forward(self, x):
         if self.training and torch.is_grad_enabled():
@@ -302,8 +320,18 @@ class EmbedNetPCA(_EmbedBase):
         super().__init__(base_model, net_vlad)
         self.pca_layer = nn.Conv2d(net_vlad.num_clusters * net_vlad.dim, dim, 1, stride=1, padding=0)
 
+    def _train_forward(self, x):
+        # differentiable path: trunk suffix + NetVLAD + the two normalisations as EmbedNet._train_forward, then the PCA
+        # layer through its autograd Function and the final L2 (netvlad.py:95-110).  Parameters change every step,
+        # possibly through `.data`, so the weight planes are re-laid out every time (as VGG._bind does for the trunk).
+        _, v = super()._train_forward(x)
+        Engine.get(x.device).set_pca(self.pca_layer.weight, self.pca_layer.bias, force=True)
+        y = _PCALayerFunction.apply(v, self.pca_layer.weight, self.pca_layer.bias)
+        return torch.nn.functional.normalize(y, p=2, dim=-1)
+
     def forward(self, x):
-        _no_train(self, "EmbedNetPCA.forward")     # the reference never trains the PCA wrapper either (inference only)
+        if self.training and torch.is_grad_enabled():
+            return self._train_forward(x)
         eng = self._bind(x)
         eng.set_pca(self.pca_layer.weight, self.pca_layer.bias)
         out, _ = eng.extract(x, pca=True, want_pool=False)

@@ -317,6 +317,19 @@ int ibl_l2dist_dense(ibl_engine* e, const float* q, int m, const float* db, int 
 int ibl_l2dist_topk(ibl_engine* e, const float* q, int m, const float* db, int n, int n_valid,
                     int d, int k, int64_t idx_base, float* out_dist, int64_t* out_idx,
                     void* stream);
+/* A database searched many times (a place index): prepared once, then ranked against small query batches without
+ * converting it again.  ibl_db_prepare: db [n,d] fp32 -> plane_f16 [n,d] (fp16, each row scaled by a power of two),
+ * aux [n,4] fp32 per row {|x|^2, scale, rounding-residual norm, max|x|} and dbmax [4] (the maxima of the residual
+ * norms, of max|x| and of |x|^2 over the rows; the fourth float is scratch).  All buffers are the caller's.
+ * ibl_db_topk: the result of ibl_l2dist_topk(q, db, n, n_valid = n, ...) bit for bit, from the fp32 rows and their
+ * prepared form; db must stay unchanged between the two calls.  Paths (ibl_debug_dist_path), for k <= 12: m > 128,
+ * the single-pass screening (1) on the prepared plane; m <= 128, a streaming scan (4) that reads the plane once per
+ * pass.  k > 12, the fp32 math mode or d % 64 != 0 call ibl_l2dist_topk itself.  1 <= k <= 128. */
+int ibl_db_prepare(ibl_engine* e, const float* db, int n, int d, void* plane_f16, float* aux, float* dbmax,
+                   void* stream);
+int ibl_db_topk(ibl_engine* e, const float* q, int m, const float* db, const void* plane_f16, const float* aux,
+                const float* dbmax, int n, int d, int k, int64_t idx_base, float* out_dist, int64_t* out_idx,
+                void* stream);
 /* Per-row top-k of an existing dense matrix dist [m,n] (row stride n): the ranks evaluate_all reads
  * from np.argsort (evaluators.py:143,151-159).  Same ordering rule as ibl_l2dist_topk.  1 <= k <= 1024. */
 int ibl_topk_rows(ibl_engine* e, const float* dist, int m, int n, int k, float* out_dist,
@@ -371,11 +384,12 @@ int ibl_gemm_nt(ibl_engine* e, const float* A, int m, const float* B, int n, int
                 void* stream);
 
 /* ---- self-tests (GPU) ------------------------------------------------------ */
-/* Queries that the screening guard re-ranked by exact brute force in the last ibl_l2dist_topk call
+/* Queries that the screening guard re-ranked by exact brute force in the last ibl_l2dist_topk or ibl_db_topk call
  * (-1: that call took the exact fp32 path, which has no guard).  Synchronises. */
 int ibl_debug_dist_flagged(ibl_engine* e, int* count, void* stream);
-/* Ranking path of the last ibl_l2dist_topk call: 0 exact fp32 CUDA cores, 1 single-pass fp16 screening,
- * 2 bf16x3 screening with a running top-16, 3 bf16x3 dense tiles + row select (-1: no call yet). */
+/* Ranking path of the last ibl_l2dist_topk or ibl_db_topk call: 0 exact fp32 CUDA cores, 1 single-pass fp16
+ * screening, 2 bf16x3 screening with a running top-16, 3 bf16x3 dense tiles + row select, 4 streaming scan of a
+ * prepared database (-1: no call yet). */
 int ibl_debug_dist_path(ibl_engine* e, int* path);
 /* Rows of the last ibl_knn_rowmax call that its guards sent to the exact scan of all N columns (-1: no call yet).
  * Synchronises. */

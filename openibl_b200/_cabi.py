@@ -91,6 +91,8 @@ SIGNATURES = {
     "ibl_l2dist_dense": (c_int, [_P, _P, c_int, _P, c_int, c_int, _P, _P]),
     "ibl_l2dist_self": (c_int, [_P, _P, c_int, c_int, _P, _P]),
     "ibl_l2dist_topk": (c_int, [_P, _P, c_int, _P, c_int, c_int, c_int, c_int, c_int64, _P, _P, _P]),
+    "ibl_db_prepare": (c_int, [_P, _P, c_int, c_int, _P, _P, _P, _P]),
+    "ibl_db_topk": (c_int, [_P, _P, c_int, _P, _P, _P, _P, c_int, c_int, c_int, c_int64, _P, _P, _P]),
     "ibl_topk_rows": (c_int, [_P, _P, c_int, c_int, c_int, _P, _P, _P]),
     "ibl_argsort_rows": (c_int, [_P, _P, c_int, c_int, _P, _P]),
     "ibl_topk_merge": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, _P, _P, _P]),

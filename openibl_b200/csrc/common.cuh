@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <atomic>
@@ -198,6 +199,17 @@ size_t dist1_workspace_bytes(int m, int n, int d, size_t* off /*[9]*/);
 int launch_dist_topk_1pass(const float* q, int m, const float* db, int n, int n_valid, int d, int k, long long idx_base,
                            void* ws, float* out_dist, long long* out_idx, uint64_t* launches, cudaStream_t s);
 const int* dist1_flag_counter(const void* ws, int m, int n, int d);
+// ... on a database prepared once by ibl_db_prepare (plane, aux, maxima as rows_f16_kernel / dist_colmax_kernel
+// make them): the same screening with the database conversion skipped, and the small-batch streaming search
+int launch_db_prepare(const float* db, int n, int d, __half* plane, float4* aux, float* dbmax, cudaStream_t s);
+int launch_dist_topk_1pass_prepared(const float* q, int m, const float* db, const __half* plane, const float4* aux,
+                                    const float* dbmax, int n, int d, int k, long long idx_base, void* ws,
+                                    float* out_dist, long long* out_idx, uint64_t* launches, cudaStream_t s);
+size_t db_scan_workspace_bytes(int m, int n, int d);
+int launch_db_scan_topk(const float* q, int m, const float* db, const __half* plane, const float4* aux,
+                        const float* dbmax, int n, int d, int k, long long idx_base, void* ws, float* out_dist,
+                        long long* out_idx, uint64_t* launches, cudaStream_t s);
+const int* db_scan_flag_counter(const void* ws, int m, int n, int d);
 // ... and the same guard + exact fallback after the bf16x3 screening of tc_gemm.cu
 size_t dist_guard_workspace_bytes(int m);
 int launch_dist_guard_bf16x3(const float* q, const float* q_sq, const float2* q_err, int m, const float* db,
@@ -212,7 +224,7 @@ int launch_pca_partial_tc(const __nv_bfloat16* w_hi, const __nv_bfloat16* w_lo, 
                           float* partial, int* splits_out, cudaStream_t s);
 int launch_rescore_sort(const float* q, const float* qn, int m, const float* db, const float* dbn, int d,
                         const long long* cand_i, int kc, int k_out, long long idx_base, float* out_dist,
-                        long long* out_idx, cudaStream_t s);
+                        long long* out_idx, cudaStream_t s, int sq_stride = 1);
 // out = bias + sum of the partials, then L2 per row when `normalize` (false: the pre-normalisation y of training)
 int launch_pca_finalize(const float* partial, int splits, int N, int P, const float* bias, float* out,
                         cudaStream_t s, bool normalize = true);
@@ -277,6 +289,8 @@ int launch_rerank_dense(RerankWs* W, const float* qg, const float* qq, const flo
 // topk.cu
 int launch_topk_rows(const float* dist, long long ld, int m, int n_valid, int k, int64_t idx_base,
                      float* out_dist, int64_t* out_idx, bool accumulate, cudaStream_t s);
+int launch_topk_rows_seg(const float* dist, long long ld, int m, int n_valid, int k, int segs, int seg,
+                         int64_t idx_base, float* out_dist, int64_t* out_idx, cudaStream_t s);
 int launch_topk_merge(const float* cand_dist, const int64_t* cand_idx, int parts, int m, int k_in,
                       int k_out, float* out_dist, int64_t* out_idx, cudaStream_t s);
 

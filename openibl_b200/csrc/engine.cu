@@ -83,6 +83,7 @@ struct ibl_engine {
   DevBuf mrg_d, mrg_i;
   DevBuf bw_g, bw_x, bw_part, bw_w;      // conv backward: dY planes, X planes, wgrad/bias partials, dgrad filter planes
   DevBuf d1_ws;                          // workspace of the single-pass distance/top-k path (tc_dist1.cu)
+  DevBuf db_ws;                          // workspace of the searches over a prepared database (ibl_db_topk)
   DevBuf q_err, db_err, guard_ws;        // guard of the bf16x3 screening paths: per-row error norms, workspace
   DevBuf knn_ws;                         // neighbour pass of the re-ranking (rerank.cu)
   const int* knn_flag_counter = nullptr; // its count of rows sent to the exact scan (null: no call yet)
@@ -1183,6 +1184,48 @@ int ibl_l2dist_topk(ibl_engine* e, const float* q, int m, const float* db, int n
     e->launches++;
   }
   return IBL_OK;
+}
+
+int ibl_db_prepare(ibl_engine* e, const float* db, int n, int d, void* plane_f16, float* aux, float* dbmax,
+                   void* stream) {
+  IBL_REQUIRE(e && db && plane_f16 && aux && dbmax, "null argument");
+  IBL_REQUIRE(n >= 1 && d >= 4 && d % 4 == 0, "bad shape");
+  DeviceGuard g(e->device);
+  IBL_RET(launch_db_prepare(db, n, d, reinterpret_cast<__half*>(plane_f16), reinterpret_cast<float4*>(aux), dbmax,
+                            S(stream)));
+  e->launches += 2;
+  return IBL_OK;
+}
+
+int ibl_db_topk(ibl_engine* e, const float* q, int m, const float* db, const void* plane_f16, const float* aux,
+                const float* dbmax, int n, int d, int k, int64_t idx_base, float* out_dist, int64_t* out_idx,
+                void* stream) {
+  IBL_REQUIRE(e && q && db && plane_f16 && aux && dbmax && out_dist && out_idx, "null argument");
+  IBL_REQUIRE(m >= 1 && n >= 1 && d >= 4 && d % 4 == 0, "bad shape");
+  IBL_REQUIRE(k >= 1 && k <= 128, "top-k supports 1 <= k <= 128");
+  IBL_REQUIRE((reinterpret_cast<uintptr_t>(plane_f16) & 15) == 0, "the fp16 plane must be 16-byte aligned");
+  // The fp32 math mode and dimensions the tensor-core paths do not take rank the fp32 rows as ibl_l2dist_topk does.
+  // So does k > 12: fp16 screening with k + 8 survivors rarely separates the k-th exact distance from the last
+  // screened one by the guard's bound, and the exact fallback behind it costs more than bf16x3 screening.
+  if (e->gemm_mode != IBL_CONV_TC_BF16X3 || d % 64 != 0 || k > 12)
+    return ibl_l2dist_topk(e, q, m, db, n, n, d, k, idx_base, out_dist, out_idx, stream);
+  DeviceGuard g(e->device);
+  const __half* plane = reinterpret_cast<const __half*>(plane_f16);
+  const float4* a4 = reinterpret_cast<const float4*>(aux);
+  if (m > 128) {
+    // the single-pass screening of ibl_l2dist_topk on the prepared plane
+    size_t off[9];
+    IBL_RET(e->db_ws.ensure(dist1_workspace_bytes(m, 0, d, off)));
+    e->flag_counter = dist1_flag_counter(e->db_ws.p, m, 0, d);
+    e->dist_path = 1;
+    return launch_dist_topk_1pass_prepared(q, m, db, plane, a4, dbmax, n, d, k, (long long)idx_base, e->db_ws.p,
+                                           out_dist, reinterpret_cast<long long*>(out_idx), &e->launches, S(stream));
+  }
+  IBL_RET(e->db_ws.ensure(db_scan_workspace_bytes(m, n, d)));
+  e->flag_counter = db_scan_flag_counter(e->db_ws.p, m, n, d);
+  e->dist_path = 4;
+  return launch_db_scan_topk(q, m, db, plane, a4, dbmax, n, d, k, (long long)idx_base, e->db_ws.p, out_dist,
+                             reinterpret_cast<long long*>(out_idx), &e->launches, S(stream));
 }
 
 int ibl_topk_rows(ibl_engine* e, const float* dist, int m, int n, int k, float* out_dist, int64_t* out_idx,

@@ -611,18 +611,31 @@ size_t dist1_workspace_bytes(int m, int n, int d, size_t* off /*[8]*/) {
   return o;
 }
 
-// q [m,d], db [n,d] fp32 (device); n_valid <= n; k <= 12.  ws: dist1_workspace_bytes(m, n, d).
-int launch_dist_topk_1pass(const float* q, int m, const float* db, int n, int n_valid, int d, int k, long long idx_base,
-                           void* ws, float* out_dist, long long* out_idx, uint64_t* launches, cudaStream_t s) {
+// Database preparation of ibl_db_prepare: the fp16 plane and aux rows of rows_f16_kernel, and in dbmax[0..2] the
+// maxima of dist_colmax_kernel, exactly as the single-pass screening makes them on every call.
+int launch_db_prepare(const float* db, int n, int d, __half* plane, float4* aux, float* dbmax, cudaStream_t s) {
+  IBL_CUDA_OK(cudaMemsetAsync(dbmax, 0, 16, s));
+  rows_f16_kernel<<<n, 256, 0, s>>>(db, d, plane, aux);
+  dist_colmax_kernel<<<cdiv(n, 256) < 64 ? cdiv(n, 256) : 64, 256, 0, s>>>(aux, n, dbmax);
+  IBL_CUDA_OK(cudaGetLastError());
+  return IBL_OK;
+}
+
+// q [m,d], db [n,d] fp32 (device); n_valid <= n; k <= 12.  plane / aux / dbmax: the prepared database
+// (launch_db_prepare over the n_valid rows), or null to prepare it here in the workspace.
+// ws: dist1_workspace_bytes(m, plane ? 0 : n, d).
+static int dist_topk_1pass(const float* q, int m, const float* db, int n, int n_valid, int d, int k, long long idx_base,
+                           const __half* plane, const float4* aux, const float* dbmax, void* ws, float* out_dist,
+                           long long* out_idx, uint64_t* launches, cudaStream_t s) {
   IBL_REQUIRE(d % 64 == 0 && k >= 1 && k <= 12 && n_valid >= 1, "1-pass distance: d % 64 == 0, 1 <= k <= 12");
   size_t off[9];
-  dist1_workspace_bytes(m, n, d, off);
+  dist1_workspace_bytes(m, plane ? 0 : n, d, off);
   uint8_t* w = reinterpret_cast<uint8_t*>(ws);
   __half* qp = reinterpret_cast<__half*>(w + off[0]);
-  __half* dp = reinterpret_cast<__half*>(w + off[1]);
+  const __half* dp = plane ? plane : reinterpret_cast<__half*>(w + off[1]);
   float4* qa = reinterpret_cast<float4*>(w + off[2]);
-  float4* da = reinterpret_cast<float4*>(w + off[3]);
-  float* dmax2 = reinterpret_cast<float*>(w + off[4]);
+  const float4* da = plane ? aux : reinterpret_cast<float4*>(w + off[3]);
+  const float* dmax2 = plane ? dbmax : reinterpret_cast<float*>(w + off[4]);
   int* fcount = reinterpret_cast<int*>(w + off[4] + 16);
   int* flist = reinterpret_cast<int*>(w + off[5]);
   unsigned* gate = reinterpret_cast<unsigned*>(w + off[5] + (size_t)m * 4);
@@ -634,8 +647,11 @@ int launch_dist_topk_1pass(const float* q, int m, const float* db, int n, int n_
   IBL_CUDA_OK(cudaMemsetAsync(w + off[4], 0, 32, s));
   IBL_CUDA_OK(cudaMemsetAsync(gate, 0xFF, (size_t)m * 4, s));      // orderable +max: no gate yet
   rows_f16_kernel<<<m, 256, 0, s>>>(q, d, qp, qa);
-  rows_f16_kernel<<<n, 256, 0, s>>>(db, d, dp, da);
-  dist_colmax_kernel<<<cdiv(n_valid, 256) < 64 ? cdiv(n_valid, 256) : 64, 256, 0, s>>>(da, n_valid, dmax2);
+  if (!plane) {
+    rows_f16_kernel<<<n, 256, 0, s>>>(db, d, reinterpret_cast<__half*>(w + off[1]), reinterpret_cast<float4*>(w + off[3]));
+    dist_colmax_kernel<<<cdiv(n_valid, 256) < 64 ? cdiv(n_valid, 256) : 64, 256, 0, s>>>(
+        reinterpret_cast<float4*>(w + off[3]), n_valid, reinterpret_cast<float*>(w + off[4]));
+  }
   IBL_CUDA_OK(cudaGetLastError());
 
   CUtensorMap ma, mb;
@@ -683,8 +699,21 @@ int launch_dist_topk_1pass(const float* q, int m, const float* db, int n, int n_
   dist_exact_scan_kernel<<<device_sm_count(), DX_SCAN_WARPS * 32, dx_scan_smem(d), s>>>(x);   // exits at once when nothing is listed
   dist_exact_finish_kernel<<<64, 256, 0, s>>>(x);
   IBL_CUDA_OK(cudaGetLastError());
-  if (launches) *launches += 7;
+  if (launches) *launches += plane ? 5 : 7;
   return IBL_OK;
+}
+
+int launch_dist_topk_1pass(const float* q, int m, const float* db, int n, int n_valid, int d, int k, long long idx_base,
+                           void* ws, float* out_dist, long long* out_idx, uint64_t* launches, cudaStream_t s) {
+  return dist_topk_1pass(q, m, db, n, n_valid, d, k, idx_base, nullptr, nullptr, nullptr, ws, out_dist, out_idx,
+                         launches, s);
+}
+
+// ws: dist1_workspace_bytes(m, 0, d)
+int launch_dist_topk_1pass_prepared(const float* q, int m, const float* db, const __half* plane, const float4* aux,
+                                    const float* dbmax, int n, int d, int k, long long idx_base, void* ws,
+                                    float* out_dist, long long* out_idx, uint64_t* launches, cudaStream_t s) {
+  return dist_topk_1pass(q, m, db, n, n, d, k, idx_base, plane, aux, dbmax, ws, out_dist, out_idx, launches, s);
 }
 
 // the guard's counter of listed queries in this workspace (test hook ibl_debug_dist_flagged)
@@ -726,6 +755,267 @@ int launch_dist_guard_bf16x3(const float* q, const float* q_sq, const float2* q_
   dist_exact_finish_kernel<<<64, 256, 0, s>>>(x);
   IBL_CUDA_OK(cudaGetLastError());
   if (launches) *launches += 4;
+  return IBL_OK;
+}
+
+// ---- 6. small-batch search over a prepared database -------------------------------------------------
+// A single query, or a phone's burst of a few, against a database prepared once (launch_db_prepare).  The fp16 plane
+// is streamed ONCE per pass of up to 128 queries, with the roles of the operands swapped against
+// gemm_f16_top16_kernel: database rows are the M side (two m64 halves of a 128-row TMA box per 64-column K step),
+// the pass's queries the N side (m64nNk16, N = the pass's queries rounded up to a power of two from 8, their boxes
+// reloaded from L2 each K step).  Persistent CTAs, one per SM, each over a contiguous range of 128-row tiles; a TMA
+// producer warp feeds a ring of up to 8 stages and one consumer warpgroup issues the MMAs.  The epilogue writes the
+// screened distances of the pass (|q|^2 + |d|^2 - 2 2^eq 2^ed q16.d16, the screening value of the single-pass path)
+// to a [queries][n] buffer; a segmented row select keeps 16 per segment, topk_merge keeps 16 per query, and the 16
+// survivors go through the exact re-score, the guard (d1_screen_bound on the fp16 error model) and the exact fallback
+// as on the other screening paths.
+constexpr int DS_BM = 128, DS_BK = 64;
+constexpr int DS_A_BYTES = DS_BM * DS_BK * 2;          // 16 KiB: one 128-row database box
+template <int N> struct DsShape {
+  static constexpr int STAGE = DS_A_BYTES + N * DS_BK * 2;
+  static constexpr int STAGES = (196608 / STAGE) < 8 ? (196608 / STAGE) : 8;
+  static constexpr int SMEM = STAGES * STAGE + 256 + N * 8 + 1024;
+  static_assert(SMEM <= 232448, "shared-memory budget of the database scan");
+  static_assert(STAGE % 1024 == 0, "128-byte swizzled boxes need 1024-byte aligned stages");
+};
+
+struct DbScanArgs {
+  int n, K, q0, mq, n_tiles;
+  const float4* q_aux;    // per query {|q|^2, 2^eq, ...}
+  const float4* db_aux;   // per database row {|d|^2, 2^ed, ...}
+  float* dist;            // [mq][ld] screened distances of this pass
+  long long ld;
+};
+
+template <int N>
+__global__ void __launch_bounds__(160, 1)
+db_scan_dist_kernel(const __grid_constant__ CUtensorMap tm_db, const __grid_constant__ CUtensorMap tm_q,
+                    const DbScanArgs g) {
+  constexpr int STAGE = DsShape<N>::STAGE, STAGES = DsShape<N>::STAGES;
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE);
+  uint64_t* empty_bar = full_bar + STAGES;       // one arrival per consumer warp
+  float2* qterm = reinterpret_cast<float2*>(smem + STAGES * STAGE + 256);   // {|q|^2, -2 2^eq} per query column
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int t0 = (int)((long long)blockIdx.x * g.n_tiles / gridDim.x);
+  const int t1 = (int)((long long)(blockIdx.x + 1) * g.n_tiles / gridDim.x);
+
+  if (warp == 4 && lane == 0) {
+    tma_prefetch_desc(&tm_db); tma_prefetch_desc(&tm_q);
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 4); }
+    fence_barrier_init();
+    fence_proxy_async();
+  }
+  for (int c = threadIdx.x; c < N; c += blockDim.x) {
+    float2 t = make_float2(0.f, 0.f);
+    if (c < g.mq) { const float4 a = __ldg(g.q_aux + g.q0 + c); t = make_float2(a.x, -2.f * a.y); }
+    qterm[c] = t;
+  }
+  __syncthreads();
+  const int kiters = g.K / DS_BK;
+
+  if (warp == 4) {
+    // TMA producer: convergent warp, one elected lane issues, warp-uniform operands
+    const uint32_t smem_a = warp_uniform(smem_u32(smem));
+    const uint32_t full_a = smem_a + STAGES * STAGE, empty_a = full_a + 8 * STAGES;
+    const int q0 = (int)warp_uniform((uint32_t)g.q0);
+    int stage = 0; uint32_t phase = 0;
+    for (int t = t0; t < t1; ++t) {
+      const int row0 = (int)warp_uniform((uint32_t)(t * DS_BM));
+      for (int kit = 0; kit < kiters; ++kit) {
+        const uint32_t sg = warp_uniform((uint32_t)stage);
+        mbar_wait_warp_a(empty_a + 8 * sg, phase ^ 1);
+        const uint32_t st = smem_a + sg * STAGE, fb = full_a + 8 * sg;
+        const int k0 = (int)warp_uniform((uint32_t)(kit * DS_BK));
+        if (elect_one()) {
+          mbar_arrive_expect_tx_a(fb, STAGE);
+          tma_load_2d_a(st, &tm_db, fb, k0, row0);              // rows beyond the database are zero-filled
+          tma_load_2d_a(st + DS_A_BYTES, &tm_q, fb, k0, q0);    // so are query rows beyond the pass
+        }
+        __syncwarp();
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+    }
+  } else {
+    const uint32_t smem_a = smem_u32(smem);
+    int stage = 0; uint32_t phase = 0;
+    for (int t = t0; t < t1; ++t) {
+      float acc[2][N / 2];
+      int prev = -1;
+      for (int kit = 0; kit < kiters; ++kit) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = smem_a + stage * STAGE;
+        const uint64_t da = gmma_desc_kmajor_sw128(sa), dq = gmma_desc_kmajor_sw128(sa + DS_A_BYTES);
+        constexpr uint64_t kHalf = 64 * 128 / 16;   // database rows 64-127: +8 KiB
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < DS_BK / 16; ++k) {
+          const uint32_t accumulate = (kit > 0 || k > 0) ? 1u : 0u;
+          Wgmma<N, true, 0, 0>::mma(acc[0], da + (uint64_t)(k * 2), dq + (uint64_t)(k * 2), accumulate);
+          Wgmma<N, true, 0, 0>::mma(acc[1], da + kHalf + (uint64_t)(k * 2), dq + (uint64_t)(k * 2), accumulate);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+#pragma unroll
+      for (int j = 0; j < 2; ++j)
+#pragma unroll
+        for (int i = 0; i < N / 2; ++i) asm volatile("" : "+f"(acc[j][i])::"memory");
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+      // fragment layout (Acc128): element [4i + 2hh + e] of half j is database row 64j + 16 warp + lane/4 + 8hh,
+      // query column 8i + 2 (lane % 4) + e.  For one column the 8 lanes of equal lane % 4 store 8 consecutive rows.
+#pragma unroll
+      for (int j = 0; j < 2; ++j)
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          const int r = t * DS_BM + 64 * j + 16 * warp + (lane >> 2) + 8 * hh;
+          if (r < g.n) {
+            const float4 b = __ldg(g.db_aux + r);
+            float* out = g.dist + r;
+#pragma unroll
+            for (int i = 0; i < N / 8; ++i)
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const int c = 8 * i + 2 * (lane & 3) + e;
+                if (c < g.mq) {
+                  const float2 qt = qterm[c];
+                  out[(long long)c * g.ld] = fmaf(qt.y * b.y, acc[j][4 * i + 2 * hh + e], qt.x + b.x);
+                }
+              }
+          }
+        }
+    }
+  }
+}
+
+// one thread per query: dist_finish_kernel's guard on kc survivors.  screened [m][kc]: the kc smallest screened
+// distances, ascending; a row that is not among them has a screened distance >= the last.
+__global__ void db_guard_kernel(const float* __restrict__ screened, int kc, const float4* __restrict__ q_aux,
+                                const float* __restrict__ dbmax, const float* __restrict__ out_dist, int k, int m,
+                                int d, int n_valid, int* flag_count, int* flag_list, int* list_cnt) {
+  const int row = blockIdx.x * blockDim.x + threadIdx.x;
+  if (row >= m || n_valid <= kc) return;                // every row was re-scored
+  const float sc = screened[(long long)row * kc + kc - 1], e_k = out_dist[(long long)row * k + k - 1];
+  const float4 qa = __ldg(q_aux + row);
+  const float bound = d1_screen_bound(qa.x, 0.f, qa.z, __ldg(dbmax + 2), 0.f, __ldg(dbmax), d, 1);
+  if (!(sc - bound > e_k)) {                            // also catches NaN
+    const int f = atomicAdd(flag_count, 1);
+    flag_list[f] = row;
+    list_cnt[f] = 0;
+  }
+}
+
+// layout: q plane | q aux | distances [min(m,128)][n] | segment lists d, i | merged d, i | flag count (256 B) |
+// guard list [m] | list counters [m] + lists [m][DX_CAP]
+struct DbScanLayout {
+  static constexpr int kc = 16;                        // survivors per query, as in the single-pass screening
+  int segs, seg, mp;
+  size_t off[9], bytes;
+  explicit DbScanLayout(int m, int n, int d) {
+    seg = cdiv(n, 8192 / kc);                           // topk_merge takes up to 8192 candidates per query
+    if (seg < 4096) seg = 4096;
+    segs = cdiv(n, seg);
+    mp = m < 128 ? m : 128;
+    size_t o = 0;
+    auto take = [&](size_t b) { const size_t at = o; o += (b + 255) & ~(size_t)255; return at; };
+    off[0] = take((size_t)m * d * 2);
+    off[1] = take((size_t)m * 16);
+    off[2] = take((size_t)mp * n * 4);
+    off[3] = take((size_t)segs * mp * kc * 4);
+    off[4] = take((size_t)segs * mp * kc * 8);
+    off[5] = take((size_t)m * kc * 4);
+    off[6] = take((size_t)m * kc * 8);
+    off[7] = take(256 + (size_t)m * 4);
+    off[8] = take(dx_lists_at(m) + (size_t)m * DX_CAP * 8);
+    bytes = o;
+  }
+};
+
+size_t db_scan_workspace_bytes(int m, int n, int d) { return DbScanLayout(m, n, d).bytes; }
+const int* db_scan_flag_counter(const void* ws, int m, int n, int d) {
+  return reinterpret_cast<const int*>(reinterpret_cast<const uint8_t*>(ws) + DbScanLayout(m, n, d).off[7]);
+}
+
+template <int N>
+static int db_scan_pass(const CUtensorMap& tm_db, const __half* qp, const DbScanArgs& g, cudaStream_t s) {
+  CUtensorMap tm_q;
+  uint64_t dims[2] = {(uint64_t)g.K, (uint64_t)(g.q0 + g.mq)}, str[1] = {(uint64_t)g.K * 2};
+  uint32_t box[2] = {(uint32_t)DS_BK, (uint32_t)N};
+  IBL_RET(make_tmap(&tm_q, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, qp, dims, str, box));
+  static DeviceOnce attr_done;   // the attribute is per device
+  if (!attr_done.done()) {
+    IBL_CUDA_OK(cudaFuncSetAttribute(db_scan_dist_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     DsShape<N>::SMEM));
+    attr_done.mark();
+  }
+  const int sms = device_sm_count();
+  db_scan_dist_kernel<N><<<g.n_tiles < sms ? g.n_tiles : sms, 160, DsShape<N>::SMEM, s>>>(tm_db, tm_q, g);
+  IBL_CUDA_OK(cudaGetLastError());
+  return IBL_OK;
+}
+
+// q [m,d] fp32; db [n,d] fp32 and its prepared plane / aux / maxima (launch_db_prepare); 1 <= k <= 12, d % 64 == 0.
+// ws: db_scan_workspace_bytes(m, n, d).  Launches: 5 + 3 per pass of 128 queries, whatever n.
+int launch_db_scan_topk(const float* q, int m, const float* db, const __half* plane, const float4* aux,
+                        const float* dbmax, int n, int d, int k, long long idx_base, void* ws, float* out_dist,
+                        long long* out_idx, uint64_t* launches, cudaStream_t s) {
+  IBL_REQUIRE(d % 64 == 0 && k >= 1 && k <= 12 && n >= 1 && m >= 1, "database scan: d % 64 == 0, 1 <= k <= 12");
+  const DbScanLayout L(m, n, d);
+  uint8_t* w = reinterpret_cast<uint8_t*>(ws);
+  __half* qp = reinterpret_cast<__half*>(w + L.off[0]);
+  float4* qa = reinterpret_cast<float4*>(w + L.off[1]);
+  float* dist = reinterpret_cast<float*>(w + L.off[2]);
+  float* sd = reinterpret_cast<float*>(w + L.off[3]);
+  int64_t* si = reinterpret_cast<int64_t*>(w + L.off[4]);
+  float* md = reinterpret_cast<float*>(w + L.off[5]);
+  int64_t* mi = reinterpret_cast<int64_t*>(w + L.off[6]);
+  int* fcount = reinterpret_cast<int*>(w + L.off[7]);
+  int* flist = reinterpret_cast<int*>(w + L.off[7] + 256);
+  int* lcnt = reinterpret_cast<int*>(w + L.off[8]);
+  unsigned long long* lists = reinterpret_cast<unsigned long long*>(w + L.off[8] + dx_lists_at(m));
+
+  IBL_CUDA_OK(cudaMemsetAsync(fcount, 0, 16, s));
+  rows_f16_kernel<<<m, 256, 0, s>>>(q, d, qp, qa);
+  IBL_CUDA_OK(cudaGetLastError());
+  CUtensorMap tm_db;
+  {
+    uint64_t dims[2] = {(uint64_t)d, (uint64_t)n}, str[1] = {(uint64_t)d * 2};
+    uint32_t box[2] = {(uint32_t)DS_BK, (uint32_t)DS_BM};
+    IBL_RET(make_tmap(&tm_db, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, plane, dims, str, box));
+  }
+  int passes = 0;
+  for (int q0 = 0; q0 < m; q0 += 128, ++passes) {
+    DbScanArgs g{};
+    g.n = n; g.K = d; g.q0 = q0; g.mq = m - q0 < 128 ? m - q0 : 128;
+    g.n_tiles = cdiv(n, DS_BM);
+    g.q_aux = qa; g.db_aux = aux; g.dist = dist; g.ld = n;
+    if (g.mq <= 8) IBL_RET(db_scan_pass<8>(tm_db, qp, g, s));
+    else if (g.mq <= 16) IBL_RET(db_scan_pass<16>(tm_db, qp, g, s));
+    else if (g.mq <= 32) IBL_RET(db_scan_pass<32>(tm_db, qp, g, s));
+    else if (g.mq <= 64) IBL_RET(db_scan_pass<64>(tm_db, qp, g, s));
+    else IBL_RET(db_scan_pass<128>(tm_db, qp, g, s));
+    IBL_RET(launch_topk_rows_seg(dist, n, g.mq, n, L.kc, L.segs, L.seg, 0, sd, si, s));
+    IBL_RET(launch_topk_merge(sd, si, L.segs, g.mq, L.kc, L.kc, md + (size_t)q0 * L.kc, mi + (size_t)q0 * L.kc, s));
+  }
+  IBL_RET(launch_rescore_sort(q, reinterpret_cast<const float*>(qa), m, db, reinterpret_cast<const float*>(aux), d,
+                              reinterpret_cast<const long long*>(mi), L.kc, k, idx_base, out_dist, out_idx, s, 4));
+  db_guard_kernel<<<cdiv(m, 128), 128, 0, s>>>(md, L.kc, qa, dbmax, out_dist, k, m, d, n, fcount, flist, lcnt);
+  IBL_CUDA_OK(cudaGetLastError());
+  ExactArgs x{};
+  x.q = q; x.db = db; x.q_sq = reinterpret_cast<const float*>(qa); x.db_sq = reinterpret_cast<const float*>(aux);
+  x.sq_stride = 4; x.m = m; x.d = d; x.n_valid = n; x.k = k;
+  x.idx_base = idx_base; x.flag_count = fcount; x.flag_list = flist; x.list_cnt = lcnt; x.lists = lists;
+  x.out_dist = out_dist; x.out_idx = out_idx;
+  IBL_RET(dx_scan_attr());
+  dist_exact_scan_kernel<<<device_sm_count(), DX_SCAN_WARPS * 32, dx_scan_smem(d), s>>>(x);   // exits at once when nothing is listed
+  dist_exact_finish_kernel<<<64, 256, 0, s>>>(x);
+  IBL_CUDA_OK(cudaGetLastError());
+  if (launches) *launches += 5 + 3 * passes;
   return IBL_OK;
 }
 

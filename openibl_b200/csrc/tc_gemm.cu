@@ -411,12 +411,13 @@ int pca_tc_splits(int P, int D) {
 
 // ---- exact fp32 re-scoring of a candidate list + final ordering ---------------------------------
 // one block (128 threads) per query: dist = |q|^2 + |d|^2 - 2 q.d with an fp32 dot product, then
-// (dist, idx)-ascending sort of the kc <= 128 candidates; writes the first k_out.
+// (dist, idx)-ascending sort of the kc <= 128 candidates; writes the first k_out.  The squared norms are sq_stride
+// floats apart (1: arrays of norms; 4: the {|x|^2, ...} rows of rows_f16_kernel).
 __global__ void __launch_bounds__(128)
 rescore_sort_kernel(const float* __restrict__ q, const float* __restrict__ qn,
                     const float* __restrict__ db, const float* __restrict__ dbn, int d,
                     const long long* __restrict__ cand_i, int kc, int k_out, long long idx_base,
-                    float* __restrict__ out_dist, long long* __restrict__ out_idx) {
+                    float* __restrict__ out_dist, long long* __restrict__ out_idx, int sq_stride) {
   extern __shared__ __align__(16) float qs[];   // [d]
   __shared__ unsigned long long keys[128];
   const long long row = blockIdx.x;
@@ -430,13 +431,13 @@ rescore_sort_kernel(const float* __restrict__ q, const float* __restrict__ qn,
   }
   const float* qrow = staged ? qs : (q + row * d);
   __syncthreads();
-  const float an = __ldg(qn + row);
+  const float an = __ldg(qn + row * sq_stride);
   for (int c = wid; c < 128; c += 4) {
     unsigned long long key = ~0ull;
     if (c < kc) {
       const long long ci = cand_i[row * kc + c];
       if (ci >= 0) {
-        key = rank_key(d1_exact(qrow, db + ci * d, d, lane, an, __ldg(dbn + ci)), (unsigned)ci);
+        key = rank_key(d1_exact(qrow, db + ci * d, d, lane, an, __ldg(dbn + ci * sq_stride)), (unsigned)ci);
       }
     }
     if (lane == 0) keys[c] = key;
@@ -447,7 +448,7 @@ rescore_sort_kernel(const float* __restrict__ q, const float* __restrict__ qn,
 
 int launch_rescore_sort(const float* q, const float* qn, int m, const float* db, const float* dbn, int d,
                         const long long* cand_i, int kc, int k_out, long long idx_base, float* out_dist,
-                        long long* out_idx, cudaStream_t s) {
+                        long long* out_idx, cudaStream_t s, int sq_stride) {
   IBL_REQUIRE(kc >= 1 && kc <= 128 && k_out >= 1 && k_out <= 128, "rescore: 1 <= k <= 128");
   IBL_REQUIRE(d % 4 == 0, "rescore: dim must be a multiple of 4");
   static DeviceOnce attr_done;   // the attribute is per device
@@ -457,7 +458,7 @@ int launch_rescore_sort(const float* q, const float* qn, int m, const float* db,
   }
   if (m == 0) return IBL_OK;
   rescore_sort_kernel<<<m, 128, d <= 16384 ? d * sizeof(float) : 16, s>>>(q, qn, db, dbn, d, cand_i, kc, k_out, idx_base,
-                                                       out_dist, out_idx);
+                                                       out_dist, out_idx, sq_stride);
   IBL_CUDA_OK(cudaGetLastError());
   return IBL_OK;
 }

@@ -13,16 +13,26 @@ constexpr unsigned long long TK_MAX = ~0ull;
 // the candidates appended since.  CAP = 2048 serves k <= 128, CAP = 4096 serves k <= 1024 (the reference's
 // evaluate_all accepts any recall_topk, evaluators.py:142-153).  Invariant before every iteration:
 // k + cnt + TK_PER_ITER <= CAP.
+// blockIdx.y selects a segment of `seg` columns: a row split over several blocks writes one sorted list per segment,
+// out_* [segments][m][k], with the segment's first column added to idx_base (one segment: the whole row).
 template <int CAP>
 __global__ void __launch_bounds__(256)
 topk_rows_kernel(const float* __restrict__ dist, long long ld, int n_valid, int k,
                  long long idx_base, float* __restrict__ out_dist,
-                 long long* __restrict__ out_idx) {
+                 long long* __restrict__ out_idx, int seg = 0) {
   __shared__ unsigned long long buf[CAP];
   __shared__ int cnt;
   __shared__ unsigned long long thr_s;
   const long long row = blockIdx.x;
   const float* d = dist + row * ld;
+  if (gridDim.y > 1) {
+    const int c0 = blockIdx.y * seg;
+    d += c0;
+    idx_base += c0;
+    n_valid = min(seg, n_valid - c0);
+    out_dist += (long long)blockIdx.y * gridDim.x * k;
+    out_idx += (long long)blockIdx.y * gridDim.x * k;
+  }
   for (int i = threadIdx.x; i < CAP; i += blockDim.x) buf[i] = TK_MAX;
   if (threadIdx.x == 0) { cnt = 0; thr_s = TK_MAX; }
   __syncthreads();
@@ -67,6 +77,20 @@ int launch_topk_rows(const float* dist, long long ld, int m, int n_valid, int k,
   else
     topk_rows_kernel<4096><<<m, 256, 0, s>>>(dist, ld, n_valid, k, (long long)idx_base, out_dist,
                                              reinterpret_cast<long long*>(out_idx));
+  IBL_CUDA_OK(cudaGetLastError());
+  return IBL_OK;
+}
+
+// Per-row top-k of dist [m][n_valid] (row stride ld) in `segs` segments of `seg` columns (segs * seg >= n_valid):
+// out_* [segs][m][k], each list ascending by (distance, index), indices idx_base + column
+int launch_topk_rows_seg(const float* dist, long long ld, int m, int n_valid, int k, int segs, int seg,
+                         int64_t idx_base, float* out_dist, int64_t* out_idx, cudaStream_t s) {
+  IBL_REQUIRE(k >= 1 && k <= 128 && segs >= 1 && (long long)segs * seg >= n_valid &&
+                  (long long)(segs - 1) * seg < n_valid,
+              "segmented top-k: 1 <= k <= 128, the segments cover the row");
+  if (m == 0) return IBL_OK;
+  topk_rows_kernel<2048><<<dim3(m, segs), 256, 0, s>>>(dist, ld, n_valid, k, (long long)idx_base, out_dist,
+                                                      reinterpret_cast<long long*>(out_idx), seg);
   IBL_CUDA_OK(cudaGetLastError());
   return IBL_OK;
 }

@@ -52,6 +52,23 @@ def _ptr(t: Optional[torch.Tensor]) -> c_void_p:
     return c_void_p(0 if t is None else t.data_ptr())
 
 
+class PreparedDB:
+    """A database prepared once for many searches (Engine.prepare_database): the fp32 rows [n,d], which the exact
+    re-scoring reads, their fp16 plane [n,d], per-row {|x|^2, scale, residual norm, max|x|} [n,4] and the maxima [4]
+    the screening guard needs.  The rows must not change while the prepared form is in use."""
+
+    def __init__(self, rows: torch.Tensor, plane: torch.Tensor, aux: torch.Tensor, dbmax: torch.Tensor):
+        self.rows, self.plane, self.aux, self.dbmax = rows, plane, aux, dbmax
+
+    @property
+    def n(self) -> int:
+        return self.rows.shape[0]
+
+    @property
+    def d(self) -> int:
+        return self.rows.shape[1]
+
+
 class Engine:
     """One per (process, GPU).  Use Engine.get(device)."""
 
@@ -568,6 +585,31 @@ class Engine:
                                        _ptr(od), _ptr(oi), _stream(self.device)), "ibl_l2dist_topk")
         return od, oi
 
+    def prepare_database(self, db: torch.Tensor) -> PreparedDB:
+        """Prepare db [n,d] fp32 once for search_prepared: its fp16 plane, per-row terms and maxima."""
+        db = _require_cuda(db, "database")
+        n, d = db.shape
+        plane = torch.empty(n, d, device=db.device, dtype=torch.float16)
+        aux = torch.empty(n, 4, device=db.device)
+        dbmax = torch.empty(4, device=db.device)
+        check(self.lib.ibl_db_prepare(self.h, _ptr(db), n, d, _ptr(plane), _ptr(aux), _ptr(dbmax),
+                                      _stream(self.device)), "ibl_db_prepare")
+        return PreparedDB(db, plane, aux, dbmax)
+
+    def search_prepared(self, q: torch.Tensor, prep: PreparedDB, k: int, idx_base: int = 0):
+        """Top-k of the queries q [m,d] over a prepared database: (dist [m,k], idx_base + row [m,k]), bit-identical
+        to l2dist_topk(q, prep.rows, k, idx_base)."""
+        q = _require_cuda(q, "queries")
+        m, d = q.shape
+        if d != prep.d:
+            raise ValueError(f"queries have {d} dimensions, the prepared database {prep.d}")
+        od = torch.empty(m, k, device=q.device)
+        oi = torch.empty(m, k, device=q.device, dtype=torch.int64)
+        check(self.lib.ibl_db_topk(self.h, _ptr(q), m, _ptr(prep.rows), _ptr(prep.plane), _ptr(prep.aux),
+                                   _ptr(prep.dbmax), prep.n, d, int(k), int(idx_base), _ptr(od), _ptr(oi),
+                                   _stream(self.device)), "ibl_db_topk")
+        return od, oi
+
     def topk_rows(self, dist: torch.Tensor, k: int):
         dist = _require_cuda(dist, "distance matrix")
         m, n = dist.shape
@@ -666,14 +708,16 @@ class Engine:
         return out_dist_host, out_idx_host
 
     def dist_flagged(self) -> int:
-        """Queries re-ranked by exact brute force in the last l2dist_topk call (-1: it took the exact fp32 path)."""
+        """Queries re-ranked by exact brute force in the last l2dist_topk or search_prepared call (-1: it took the
+        exact fp32 path)."""
         c = c_int()
         check(self.lib.ibl_debug_dist_flagged(self.h, byref(c), _stream(self.device)), "ibl_debug_dist_flagged")
         return c.value
 
     def dist_path(self) -> int:
-        """Ranking path of the last l2dist_topk call: 0 exact fp32, 1 single-pass fp16 screening, 2 bf16x3 top-16
-        screening, 3 bf16x3 dense screening (-1: no call yet)."""
+        """Ranking path of the last l2dist_topk or search_prepared call: 0 exact fp32, 1 single-pass fp16 screening,
+        2 bf16x3 top-16 screening, 3 bf16x3 dense screening, 4 streaming scan of a prepared database (-1: no call
+        yet)."""
         c = c_int()
         check(self.lib.ibl_debug_dist_path(self.h, byref(c)), "ibl_debug_dist_path")
         return c.value

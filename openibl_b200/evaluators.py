@@ -24,7 +24,7 @@ from .utils.data.gpu_jpeg import check_decode_errors, decode_batch, is_encoded_b
 from .utils.data.sampler import slice_bounds
 
 __all__ = ["extract_cnn_feature", "extract_features", "pairwise_distance", "spatial_nms",
-           "evaluate_all", "recalls_from_topk", "sharded_topk", "sharded_rerank_topk", "Evaluator"]
+           "evaluate_all", "recalls_from_topk", "sharded_topk", "gather_merge_topk", "sharded_rerank_topk", "Evaluator"]
 
 
 def _rank_world():
@@ -213,10 +213,18 @@ def sharded_topk(q: torch.Tensor, db_shard: torch.Tensor, k: int, idx_base: int,
         _rank_fn = lambda qq, dd, kk, base, nv: eng.l2dist_topk(qq, dd, kk, idx_base=base, n_valid=nv)
         _merge_fn = eng.topk_merge
     cd, ci = _rank_fn(q, db_shard, k, idx_base, n_valid)
+    if world > 1 and int(idx_base) + int(db_shard.shape[0]) >= 2 ** 31:
+        raise ValueError("sharded_topk packs global indices as int32: the gallery must have < 2^31 rows")
+    return gather_merge_topk(cd, ci, k, _merge_fn)
+
+
+def gather_merge_topk(cd: torch.Tensor, ci: torch.Tensor, k: int, merge_fn):
+    """This rank's [m,k] candidates (distance, global index) -> the merged [m,k] over all ranks, identical on every
+    rank: ONE all_gather_into_tensor of the candidates packed as (fp32 distance bits, int32 index), 8 bytes each,
+    then merge_fn(dist [world,m,k], idx [world,m,k], k)."""
+    _, world = _rank_world()
     if world == 1:
         return cd, ci
-    if int(idx_base) + int(db_shard.shape[0]) >= 2 ** 31:
-        raise ValueError("sharded_topk packs global indices as int32: the gallery must have < 2^31 rows")
     m = cd.shape[0]
     packed = torch.empty(m, k, 2, dtype=torch.int32, device=cd.device)
     packed[..., 0] = cd.contiguous().view(torch.int32)
@@ -226,7 +234,7 @@ def sharded_topk(q: torch.Tensor, db_shard: torch.Tensor, k: int, idx_base: int,
     gathered = gathered.view(world, m, k, 2)
     gd = gathered[..., 0].contiguous().view(torch.float32)
     gi = gathered[..., 1].to(torch.int64)
-    return _merge_fn(gd, gi, k)
+    return merge_fn(gd, gi, k)
 
 
 def sharded_rerank_topk(x: torch.Tensor, shard: torch.Tensor, k: int, idx_base: int, n_valid: int, k1: int = 20,

@@ -242,10 +242,9 @@ constexpr int TC_A_BYTES = TC_BM * TC_BK * 2;   // 16 KiB per plane
 // An 8x16 patch (chosen where it wastes fewer rows, e.g. 120x160 maps) has an 18 x 10 halo: the same 180 rows, taps
 // (kh*18 + kw) rows in, 8-row groups 18 rows (2304 B) apart, and the second m64 half (columns 8-15 of every patch row)
 // 8 rows in.
-constexpr int TC_HALO_W = 10, TC_HALO_H = 18;   // the 16x8 patch's halo (also the fused conv1 kernel's)
+constexpr int TC_HALO_W = 10, TC_HALO_H = 18;   // the 16x8 patch's halo
 constexpr int TC_HALO_ROWS = TC_HALO_W * TC_HALO_H;
 constexpr int TC_HALO_PLANE = 23 * 1024;        // 180 rows x 128 B = 23040 B, padded to the swizzle period
-constexpr int TC_HALO_STAGE = 2 * TC_HALO_PLANE;
 
 // The wide tiles' halo: (16+2) x (16+2) = 324 rows of 128 B per plane, padded to the swizzle period.  Two stages of both
 // planes and three 16 KiB weight taps leave no room for epilogue staging.
@@ -848,51 +847,61 @@ int launch_conv3x3_tc(const __nv_bfloat16* x_hi, const __nv_bfloat16* x_lo, cons
 // conv1_1 + conv1_2 (+ ReLU + 2x2 max-pool) in ONE kernel  (vgg.py:40-42 slots 0 and 2)
 //
 // conv1_1's output -- 64 channels at full resolution, 2.5 GB per batch of 32 as hi/lo planes -- is the largest tensor
-// of the network and would be written to HBM by one kernel only to be read back by the next.  Here a CTA owns 16 x 8
-// patches of conv1_2 outputs and RECOMPUTES the conv1_1 activations each needs, the (16+2) x (8+2) = 180-pixel halo,
-// straight into the shared-memory halo tile that conv1_2's nine tap views read (the HALO staging above).
+// of the network and would be written to HBM by one kernel only to be read back by the next.  Here a CTA owns 16 x 16
+// patches of conv1_2 outputs and RECOMPUTES the conv1_1 activations each needs, the (16+2) x (16+2) = 324-pixel halo,
+// straight into a shared-memory halo tile laid out as the wide tiles' (18-pixel rows, TC_WIDE_HALO_PLANE per plane).
 //
 //   producer (warpgroup 0)     warp 0: TMA ring of conv1_2's weight taps (16 KiB each); the warpgroup's registers go
 //                              to the consumers (setmaxnreg)
 //   consumers (warpgroups 1-2) consumer j takes the CTA's tiles j, j + 2, ... and, per tile:
-//     A1  im2col of the 3-channel input for the 180 halo pixels: K = 27 -> 32, bf16 hi/lo, 64-byte K-major SW64 rows,
-//         192 rows = 3 m64 tiles, built in the consumer's own halo buffer (free until C1's epilogue fills it)
-//     C1  conv1_1: 3 M tiles x 2 K steps x 3 wgmma (N = 64) -> bias, ReLU, ZERO outside the image (conv1_2's padding),
-//         hi/lo straight from the accumulator fragment into the halo tile's swizzled rows
-//     C2  conv1_2: 9 taps x 4 K steps x 3 wgmma (N = 64) over the halo's tap views -> bias, ReLU, 2x2 max-pool, hi/lo
-//         planes -> HBM                                                                       [conv_epilogue_tile]
-// so one consumer's C2 MMAs run while the other does its C2 epilogue, its next tile's A1, C1 and C1 epilogue.
+//     A1  im2col of the 3-channel input for the 324 halo pixels: K = 27 -> 32, bf16 hi/lo, 64-byte K-major SW64 rows,
+//         384 rows = 6 m64 tiles, built in the consumer's own halo buffer (f1_a1_off)
+//     C1  conv1_1 per m64 tile: 2 K steps x 3 wgmma (N = 64) -> bias, ReLU, ZERO outside the image (conv1_2's padding),
+//         hi/lo straight from the accumulator fragment into the halo tile's swizzled rows; two tiles in flight, so one
+//         tile's MMAs run during the epilogue of the tile before.  (Two more tiles' accumulators, 128 registers, make
+//         ptxas spill and serialise C2's register-A MMAs.)
+//     C2  conv1_2 with the wide tiles' operand roles: M = the 64 output channels, A = the tap's weights in registers
+//         (ldsm_a_sw128), N = the 256 pixels as two n128 views of the halo tile; 9 taps x 4 K steps x 2 views x 3 wgmma
+//         -> 2x2 max-pool, bias, ReLU, hi/lo planes -> HBM, register-local                   [conv_wide_epilogue]
+// so one consumer's C2 MMAs run while the other does its C2 epilogue, its next tile's A1, C1 and C1 epilogue.  Both
+// convolutions add their products in the order of the unfused path (conv1_1_tc_kernel, then conv3x3_tc_kernel on
+// conv1_2): lo.hi, hi.lo, hi.hi per k16 step into one accumulator.
 // =====================================================================================================================
 struct Conv1FusedArgs {
   const float* x;       // [N,3,H,W]
   const float* w1;      // conv1_1 OIHW [64,3,3,3]
   const float* bias1;   // [64]
-  ConvTcArgs c2;        // conv1_2: N,H,W, cin = cout = 64, tw_log2 = 3, tiles, relu, pool, bias, y_hi / y_lo
+  ConvTcArgs c2;        // conv1_2: N,H,W, cin = cout = 64, tw_log2 = 4, tiles, relu, pool, bias, y_hi / y_lo
 };
 
-constexpr int F1_A1_ROWS = 192;                      // the 180 halo pixels in three m64 tiles
-constexpr int F1_A1_PLANE = F1_A1_ROWS * 64;         // 64-byte rows: K = 32
-constexpr int F1_W1_PLANE = 64 * 64;                 // conv1_1 filters: 64 rows x 64 B per plane
-constexpr int F1_W2_STAGE = 2 * 64 * TC_BK * 2;      // one tap of conv1_2: W_hi 8 KiB | W_lo 8 KiB
-constexpr int F1_W2_STAGES = 4;
-// [halo 0 | halo 1] [W1 hi | W1 lo] [4 weight taps] [staging 0 | staging 1] [barriers, bias1]
-constexpr int F1_OFF_W1 = 2 * TC_HALO_STAGE;         // 92 KiB
-constexpr int F1_OFF_W2 = F1_OFF_W1 + 2 * F1_W1_PLANE;
-constexpr int F1_OFF_STG = F1_OFF_W2 + F1_W2_STAGES * F1_W2_STAGE;
-constexpr int F1_OFF_BAR = F1_OFF_STG + 2 * ACC_STG_BYTES;
+constexpr int F1_HALO_W = 18;                             // halo row pitch (pixels) of a 16x16 patch
+constexpr int F1_HALO_ROWS = F1_HALO_W * F1_HALO_W;       // 324
+constexpr int F1_HALO_STAGE = 2 * TC_WIDE_HALO_PLANE;     // hi | lo
+constexpr int F1_A1_TILE = 64 * 64;                      // one m64 tile of A1 per plane: 64-byte rows, K = 32
+constexpr int F1_W1_PLANE = 64 * 64;                      // conv1_1 filters: 64 rows x 64 B per plane
+constexpr int F1_W2_STAGE = 2 * 64 * TC_BK * 2;           // one tap of conv1_2: W_hi 8 KiB | W_lo 8 KiB
+constexpr int F1_W2_STAGES = 3;
+// [halo 0 | halo 1] [3 weight taps] [W1 hi | W1 lo] [barriers, bias1]
+constexpr int F1_OFF_W2 = 2 * F1_HALO_STAGE;              // 164 KiB
+constexpr int F1_OFF_W1 = F1_OFF_W2 + F1_W2_STAGES * F1_W2_STAGE;
+constexpr int F1_OFF_BAR = F1_OFF_W1 + 2 * F1_W1_PLANE;
 constexpr int F1_SMEM = F1_OFF_BAR + 512 + 1024;
-static_assert(2 * F1_A1_PLANE <= TC_HALO_STAGE, "A1 (hi | lo) is built inside the consumer's halo buffer");
-static_assert(TC_HALO_STAGE % 1024 == 0 && F1_OFF_W1 % 512 == 0 && F1_OFF_W2 % 1024 == 0, "swizzle atom alignment");
-static_assert(F1_SMEM <= 232448, "shared-memory budget of the fused conv1 kernel");
 
-// d[0:32] += A . B^T as m64n64k16 (A, B descriptors): the columns 0-63 of an N = 128 fragment d[64] (fused conv1 kernel)
-__device__ __forceinline__ void wgmma_n64_into_n128(float (&d)[64], uint64_t a, uint64_t b) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-      : "l"(a), "l"(b));
+// A1 plane `plane` (0 hi, 1 lo) of m64 tile g (rows 64 g .. 64 g + 63), as a byte offset into the consumer's halo
+// buffer.  Tile g's C1 epilogue writes halo rows 64 g .. 64 g + 63 of both planes while tile g + 1's MMAs still read, so
+// tiles 0-4 keep both A1 planes in their own rows of the hi halo plane.  Tile 5 (halo rows 320-323; the hi plane has no
+// room for its 8 KiB there) goes first and keeps its A1 in the lo plane's rows 0-63, which tile 0's epilogue overwrites
+// only after tile 5 has retired.
+__host__ __device__ constexpr int f1_a1_off(int g, int plane) {
+  return (g < 5 ? g * 2 * F1_A1_TILE : TC_WIDE_HALO_PLANE) + plane * F1_A1_TILE;
 }
+static_assert(2 * F1_A1_TILE == 64 * 128, "a tile's A1 fills its own halo rows of the hi plane");
+static_assert(5 * 64 < F1_HALO_ROWS && 6 * 64 >= F1_HALO_ROWS && f1_a1_off(4, 1) + F1_A1_TILE <= TC_WIDE_HALO_PLANE &&
+                  F1_HALO_ROWS * 128 <= TC_WIDE_HALO_PLANE,
+              "six m64 tiles cover the halo, only tile 5 reaches past halo row 319, and the halo tile fits in a plane");
+static_assert(F1_HALO_STAGE % 1024 == 0 && F1_OFF_W2 % 1024 == 0 && F1_OFF_W1 % 512 == 0 && f1_a1_off(5, 1) % 512 == 0,
+              "swizzle atom alignment");
+static_assert(F1_SMEM <= 232448, "shared-memory budget of the fused conv1 kernel");
 
 __global__ void __launch_bounds__(384, 1)
 conv1_fused_tc_kernel(const __grid_constant__ CUtensorMap tm_whi, const __grid_constant__ CUtensorMap tm_wlo,
@@ -902,10 +911,9 @@ conv1_fused_tc_kernel(const __grid_constant__ CUtensorMap tm_whi, const __grid_c
   const ConvTcArgs& a = fa.c2;
   uint8_t* w1 = smem + F1_OFF_W1;
   uint8_t* w2 = smem + F1_OFF_W2;
-  float* stg = reinterpret_cast<float*>(smem + F1_OFF_STG);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + F1_OFF_BAR);
-  uint64_t* w_full = bars;                           // [4] producer
-  uint64_t* w_empty = bars + F1_W2_STAGES;           // [4] 4 warps of the consumer of the tile
+  uint64_t* w_full = bars;                           // [3] producer
+  uint64_t* w_empty = bars + F1_W2_STAGES;           // [3] 4 warps of the consumer of the tile
   uint64_t* order_bar = bars + 2 * F1_W2_STAGES;     // [2] 4 warps of the other consumer
   float* bias1_s = reinterpret_cast<float*>(bars + 16);   // [64]
 
@@ -948,7 +956,7 @@ conv1_fused_tc_kernel(const __grid_constant__ CUtensorMap tm_whi, const __grid_c
     img = tile / tiles_per_img;
     const int rem = tile - img * tiles_per_img;
     h0 = (rem / a.tiles_w) * 16;
-    w0 = (rem % a.tiles_w) * 8;
+    w0 = (rem % a.tiles_w) * 16;
   };
 
   if (warp < 4) setmaxnreg_dec<40>();
@@ -973,16 +981,19 @@ conv1_fused_tc_kernel(const __grid_constant__ CUtensorMap tm_whi, const __grid_c
     setmaxnreg_inc<232>();
     const int cw = warp / 4 - 1;                      // consumer 0 / 1
     const int bar = 1 + cw;                           // its named barrier
-    float* my_stg = stg + cw * (ACC_STG_BYTES / 4);
-    uint8_t* halo = smem + cw * TC_HALO_STAGE;        // this consumer's halo tile; A1 hi | lo at its start until C1 retires
+    uint8_t* halo = smem + cw * F1_HALO_STAGE;        // this consumer's halo tile; A1 inside it until C1 retires
     const int t = threadIdx.x & 127;                  // thread inside the warpgroup
-    const int r = t >> 3, c = t & 7;                  // C2 accumulator row t = pixel (r, c) of the 8-wide, 16-tall patch
     const uint32_t ha = smem_u32(halo);
+    const uint32_t w2a = smem_u32(w2);
     const uint64_t b1h = gmma_desc_kmajor_sw64(smem_u32(w1)), b1l = gmma_desc_kmajor_sw64(smem_u32(w1) + F1_W1_PLANE);
-    const uint64_t a1h = gmma_desc_kmajor_sw64(ha), a1l = gmma_desc_kmajor_sw64(ha + F1_A1_PLANE);
     constexpr uint64_t kA1Tile = 64 * 64 / 16;         // the next m64 tile of A1: +4 KiB
-    constexpr uint64_t kHaloDesc = ((uint64_t)1 << 16) | ((uint64_t)((TC_HALO_W * 128) >> 4) << 32) | ((uint64_t)1 << 62);
-    constexpr uint64_t kHaloHalf = 8 * TC_HALO_W * 128 / 16;   // pixel rows 64-127 of a tap view: groups 8-15
+    // K-major SW128 view of the halo tile: 8-pixel groups one halo row (2304 B) apart; view v starts 8v pixels into
+    // patch row 0 (+1 KiB)
+    constexpr uint64_t kHaloDesc = ((uint64_t)1 << 16) | ((uint64_t)((F1_HALO_W * 128) >> 4) << 32) | ((uint64_t)1 << 62);
+    // conv1_2's weight row map, as in the wide halo kernel: accumulator rows 16w + j and 16w + j + 8 (j < 8) read output
+    // channels 16w + 2j + s and 16w + 2j + (s ^ 1), s = j >> 2, so a thread's two rows are adjacent channels
+    const int wq = (threadIdx.x >> 5) & 3, jl = lane & 7, hl8 = (lane >> 3) & 1;
+    const int wrow = 16 * wq + 2 * jl + (hl8 ^ (jl >> 2));
     const long long HW = (long long)a.H * a.W;
     // Consumer cw takes the CTA's tiles cw, cw + 2, ...  The producer fills the weight ring in tile order, so the taps of
     // CTA-local tile i start at running index 9 i.  The order barrier lets a consumer wait on its first tap only after
@@ -991,102 +1002,107 @@ conv1_fused_tc_kernel(const __grid_constant__ CUtensorMap tm_whi, const __grid_c
     for (int i = cw; blockIdx.x + i * gridDim.x < a.total_tiles; i += 2) {
       int img, h0, w0;
       coords(blockIdx.x + i * gridDim.x, img, h0, w0);
-      // the per-row index math below is recomputed for every tile: hoisted out of the loop it would hold ~20 registers
+      // the per-row index math below is recomputed for every tile: hoisted out of the loop it would hold registers
       // through the C2 main loop and epilogue
       int tl = t;
       asm volatile("" : "+r"(tl));
-      // ---- A1: rows t and t + 128 (halo pixels; rows >= 180 are zero).  The previous tile's C2 has retired: every warp
-      // passed its wgmma_wait<0> before the named barriers of that tile's epilogue.
+      // ---- A1: rows t, t + 128, t + 256 (halo pixels; rows >= 324 are zero).  The epilogue has no barrier, so the
+      // warpgroup meets here: every warp's previous C2 MMAs, the last readers of this buffer, have retired.
+      wg_sync(bar);
 #pragma unroll
-      for (int q = 0; q < 2; ++q) {
+      for (int q = 0; q < 3; ++q) {
         const int p = q * 128 + tl;
-        if (p < F1_A1_ROWS) {
-          float v[32];
+        float v[32];
 #pragma unroll
-          for (int k = 0; k < 32; ++k) v[k] = 0.f;
-          const int hl = p / TC_HALO_W, wl = p - hl * TC_HALO_W;
-          const int ph = h0 - 1 + hl, pw = w0 - 1 + wl;
-          if (p < TC_HALO_ROWS && ph >= 0 && ph < a.H && pw >= 0 && pw < a.W && img < a.N) {
-            const float* xb = fa.x + (long long)img * 3 * HW;
+        for (int k = 0; k < 32; ++k) v[k] = 0.f;
+        const int hl = p / F1_HALO_W, wl = p - hl * F1_HALO_W;
+        const int ph = h0 - 1 + hl, pw = w0 - 1 + wl;
+        if (p < F1_HALO_ROWS && ph >= 0 && ph < a.H && pw >= 0 && pw < a.W && img < a.N) {
+          const float* xb = fa.x + (long long)img * 3 * HW;
 #pragma unroll
-            for (int tap = 0; tap < 9; ++tap) {
-              const int ih = ph + tap / 3 - 1, iw = pw + tap % 3 - 1;
-              if (ih >= 0 && ih < a.H && iw >= 0 && iw < a.W) {
-                const long long o = (long long)ih * a.W + iw;
+          for (int tap = 0; tap < 9; ++tap) {
+            const int ih = ph + tap / 3 - 1, iw = pw + tap % 3 - 1;
+            if (ih >= 0 && ih < a.H && iw >= 0 && iw < a.W) {
+              const long long o = (long long)ih * a.W + iw;
 #pragma unroll
-                for (int ci = 0; ci < 3; ++ci) v[tap * 3 + ci] = __ldg(xb + ci * HW + o);
-              }
+              for (int ci = 0; ci < 3; ++ci) v[tap * 3 + ci] = __ldg(xb + ci * HW + o);
             }
           }
-          uint8_t* rh = halo + p * 64;
+        }
+        const int g = p >> 6, r = p & 63;              // row r of m64 tile g
+        uint8_t* rh = halo + f1_a1_off(g, 0) + r * 64;
+        uint8_t* rl = halo + f1_a1_off(g, 1) + r * 64;
 #pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            uint32_t hi[4], lo[4];
+        for (int j = 0; j < 4; ++j) {
+          uint32_t hi[4], lo[4];
 #pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const float x0 = v[8 * j + 2 * e], x1 = v[8 * j + 2 * e + 1];
-              const __nv_bfloat16 h0b = __float2bfloat16_rn(x0), h1b = __float2bfloat16_rn(x1);
-              __nv_bfloat162 hv(h0b, h1b);
-              hi[e] = *reinterpret_cast<uint32_t*>(&hv);
-              lo[e] = pack_bf16x2(x0 - __bfloat162float(h0b), x1 - __bfloat162float(h1b));
-            }
-            const int pos = (j ^ ((p >> 1) & 3)) * 16;
-            *reinterpret_cast<uint4*>(rh + pos) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-            *reinterpret_cast<uint4*>(rh + F1_A1_PLANE + pos) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+          for (int e = 0; e < 4; ++e) {
+            const float x0 = v[8 * j + 2 * e], x1 = v[8 * j + 2 * e + 1];
+            const __nv_bfloat16 h0b = __float2bfloat16_rn(x0), h1b = __float2bfloat16_rn(x1);
+            __nv_bfloat162 hv(h0b, h1b);
+            hi[e] = *reinterpret_cast<uint32_t*>(&hv);
+            lo[e] = pack_bf16x2(x0 - __bfloat162float(h0b), x1 - __bfloat162float(h1b));
           }
+          const int pos = (j ^ ((r >> 1) & 3)) * 16;
+          *reinterpret_cast<uint4*>(rh + pos) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+          *reinterpret_cast<uint4*>(rl + pos) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
         }
       }
       fence_proxy_async();                             // generic-proxy writes of A1 -> visible to the tensor core
       wg_sync(bar);
-      // ---- C1: conv1_1 on the 192 A1 rows
-      float c1[3][32];
-      wgmma_fence();
+      // ---- C1: conv1_1 on the six m64 tiles of A1 in the order 5, 0, 1, 2, 3, 4 (f1_a1_off), two in flight: step s
+      // takes tile g from c1[s & 1] to halo rows 64 g .. 64 g + 63, then issues step s + 2's tile into c1[s & 1]
+      float c1[2][32];
+      auto issue_c1 = [&](int g, float (&acc)[32]) {
+        const uint64_t a1h = gmma_desc_kmajor_sw64(ha + f1_a1_off(g, 0));
+        const uint64_t a1l = gmma_desc_kmajor_sw64(ha + f1_a1_off(g, 1));
+        wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < 2; ++k) {                    // K = 32: two 16-wide steps
-        const uint64_t ko = (uint64_t)(k * 2);
-#pragma unroll
-        for (int f = 0; f < 3; ++f) {
-          const uint64_t fo = f * kA1Tile + ko;
-          Wgmma<64, false, 0, 0>::mma(c1[f], a1l + fo, b1h + ko, k > 0 ? 1u : 0u);
-          Wgmma<64, false, 0, 0>::mma(c1[f], a1h + fo, b1l + ko, 1u);
-          Wgmma<64, false, 0, 0>::mma(c1[f], a1h + fo, b1h + ko, 1u);
+        for (int k = 0; k < 2; ++k) {                  // K = 32: two 16-wide steps
+          const uint64_t ko = (uint64_t)(k * 2);
+          Wgmma<64, false, 0, 0>::mma(acc, a1l + ko, b1h + ko, k > 0 ? 1u : 0u);
+          Wgmma<64, false, 0, 0>::mma(acc, a1h + ko, b1l + ko, 1u);
+          Wgmma<64, false, 0, 0>::mma(acc, a1h + ko, b1h + ko, 1u);
         }
-      }
-      wgmma_commit();
-      wgmma_wait<0>();
+        wgmma_commit();
+      };
+      issue_c1(5, c1[0]);
+      issue_c1(0, c1[1]);
 #pragma unroll
-      for (int f = 0; f < 3; ++f)
+      for (int step = 0; step < 6; ++step) {
+        const int g = step == 0 ? 5 : step - 1;
+        float (&acc)[32] = c1[step & 1];
+        if (step < 5) wgmma_wait<1>(); else wgmma_wait<0>();   // the groups are committed in step order
 #pragma unroll
-        for (int j = 0; j < 32; ++j) asm volatile("" : "+f"(c1[f][j])::"memory");
-      wg_sync(bar);                                    // no warp reads A1 any more: the halo rows may overwrite it
-      // ---- C1 epilogue: bias, ReLU, image mask, hi/lo -> halo row p, from the fragment.  Thread 32 w + l holds
-      // rows 16 w + l/4 (+ 8) of each m64 tile, channel pairs 8 j + 2 (l % 4): one 4-byte store per plane and pair,
-      // eight distinct rows x four lanes per 16-byte chunk position -> conflict-free.
-#pragma unroll
-      for (int f = 0; f < 3; ++f) {
+        for (int j = 0; j < 32; ++j) asm volatile("" : "+f"(acc[j])::"memory");
+        wg_sync(bar);                                  // no warp reads tile g's A1 any more: its halo rows may overwrite it
+        // bias, ReLU, image mask, hi/lo -> halo row p, from the fragment.  Thread 32 w + l holds rows 16 w + l/4 (+ 8)
+        // of the m64 tile, channel pairs 8 j + 2 (l % 4): one 4-byte store per plane and pair, eight distinct rows x
+        // four lanes per 16-byte chunk position -> conflict-free.
 #pragma unroll
         for (int hf = 0; hf < 2; ++hf) {
-          const int p = 64 * f + (tl & ~31) / 2 + ((tl & 31) >> 2) + 8 * hf;
-          if (p < TC_HALO_ROWS) {
-            const int hl = p / TC_HALO_W, wl = p - hl * TC_HALO_W;
+          const int p = 64 * g + (tl & ~31) / 2 + ((tl & 31) >> 2) + 8 * hf;
+          if (p < F1_HALO_ROWS) {
+            const int hl = p / F1_HALO_W, wl = p - hl * F1_HALO_W;
             const int ph = h0 - 1 + hl, pw = w0 - 1 + wl;
             const bool inside = ph >= 0 && ph < a.H && pw >= 0 && pw < a.W && img < a.N;
             uint8_t* rh = halo + p * 128 + (tl & 3) * 4;
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
               const int ch = 8 * j + 2 * (tl & 3);
-              float x0 = fmaxf(c1[f][4 * j + 2 * hf] + bias1_s[ch], 0.f);
-              float x1 = fmaxf(c1[f][4 * j + 2 * hf + 1] + bias1_s[ch + 1], 0.f);
+              float x0 = fmaxf(acc[4 * j + 2 * hf] + bias1_s[ch], 0.f);
+              float x1 = fmaxf(acc[4 * j + 2 * hf + 1] + bias1_s[ch + 1], 0.f);
               if (!inside) { x0 = 0.f; x1 = 0.f; }       // conv1_2 pads its INPUT with zeros
               const __nv_bfloat16 h0b = __float2bfloat16_rn(x0), h1b = __float2bfloat16_rn(x1);
               __nv_bfloat162 hv(h0b, h1b);
               const int pos = (j ^ (p & 7)) * 16;
               *reinterpret_cast<uint32_t*>(rh + pos) = *reinterpret_cast<uint32_t*>(&hv);
-              *reinterpret_cast<uint32_t*>(rh + TC_HALO_PLANE + pos) =
+              *reinterpret_cast<uint32_t*>(rh + TC_WIDE_HALO_PLANE + pos) =
                   pack_bf16x2(x0 - __bfloat162float(h0b), x1 - __bfloat162float(h1b));
             }
           }
         }
+        if (step + 2 < 6) issue_c1(step + 1, acc);     // step s + 2 takes tile s + 1
       }
       fence_proxy_async();                             // generic-proxy writes of the halo -> visible to the tensor core
       wg_sync(bar);                                    // every halo row is written
@@ -1094,52 +1110,50 @@ conv1_fused_tc_kernel(const __grid_constant__ CUtensorMap tm_whi, const __grid_c
       int stage = (i * 9) % F1_W2_STAGES;
       uint32_t phase = (uint32_t)((i * 9) / F1_W2_STAGES) & 1u;
       if (i > 0) mbar_wait(&order_bar[cw], (uint32_t)((i - 1) >> 1) & 1u);
-      // A tap's weight stage is W_hi (64 rows) then W_lo (64 rows): one K-major N = 128 operand.  Per k16 step and m64
-      // half, A_hi . [W_hi; W_lo] is one m64n128k16 (A_hi W_hi in columns 0-63, A_hi W_lo in 64-127) and A_lo . W_hi one
-      // m64n64k16 into the first 32 registers of the same fragment (columns 0-63): 10 KiB of shared-memory operands
-      // instead of 12 KiB for the three N = 64 products.  The epilogue adds the two column halves.
-      float d[2][64];
-#pragma unroll
-      for (int hm = 0; hm < 2; ++hm)
-#pragma unroll
-        for (int j = 0; j < 64; ++j) d[hm][j] = 0.f;   // the first MMA ignores it, but its live range starts here, not before C1
+      AccWide acc;
+      // the weight fragments of one k16 step go into fw[k & 1] while the previous step's MMAs run
+      uint32_t fw[2][2][4];
       int prev = -1;
+#pragma unroll 1
       for (int tap = 0; tap < 9; ++tap) {
         mbar_wait(&w_full[stage], phase);
-        const uint32_t toff = (uint32_t)((tap / 3) * TC_HALO_W + tap % 3) * 128u;
-        const uint64_t a_hi = kHaloDesc | (uint64_t)(((ha + toff) >> 4) & 0x3fffu);
-        const uint64_t a_lo = kHaloDesc | (uint64_t)(((ha + TC_HALO_PLANE + toff) >> 4) & 0x3fffu);
-        const uint64_t b_w = gmma_desc_kmajor_sw128(smem_u32(w2 + stage * F1_W2_STAGE));
-        wgmma_fence();
+        const uint32_t sb = w2a + stage * F1_W2_STAGE;
+        ldsm_a_sw128(fw[0][0], sb, wrow, 0);
+        ldsm_a_sw128(fw[0][1], sb + F1_W2_STAGE / 2, wrow, 0);
+        const uint32_t toff = (uint32_t)((tap / 3) * F1_HALO_W + tap % 3) * 128u;
+        const uint64_t x_hi = kHaloDesc | (uint64_t)(((ha + toff) >> 4) & 0x3fffu);
+        const uint64_t x_lo = kHaloDesc | (uint64_t)(((ha + TC_WIDE_HALO_PLANE + toff) >> 4) & 0x3fffu);
 #pragma unroll
         for (int k = 0; k < TC_BK / 16; ++k) {
+          const uint32_t(&fh)[4] = fw[k & 1][0];
+          const uint32_t(&fl)[4] = fw[k & 1][1];
           const uint64_t ko = (uint64_t)(k * 2);
+          wgmma_fence();
 #pragma unroll
-          for (int hm = 0; hm < 2; ++hm) {
-            const uint64_t ho = hm ? kHaloHalf : 0;
-            Wgmma<128, false, 0, 0>::mma(d[hm], a_hi + ho + ko, b_w + ko, (tap > 0 || k > 0) ? 1u : 0u);
-            wgmma_n64_into_n128(d[hm], a_lo + ho + ko, b_w + ko);
+          for (int v = 0; v < 2; ++v) WgmmaRS<128>::mma(acc.d[v], fh, x_lo + 64 * v + ko, (tap > 0 || k > 0) ? 1u : 0u);
+#pragma unroll
+          for (int v = 0; v < 2; ++v) WgmmaRS<128>::mma(acc.d[v], fl, x_hi + 64 * v + ko, 1u);
+#pragma unroll
+          for (int v = 0; v < 2; ++v) WgmmaRS<128>::mma(acc.d[v], fh, x_hi + 64 * v + ko, 1u);
+          wgmma_commit();
+          if (k == 3 && tap == 8 && lane == 0) mbar_arrive(&order_bar[cw ^ 1]);
+          wgmma_wait<1>();                             // the previous k16 step's MMAs have retired: its fragments are
+          if (k == 0 && prev >= 0 && lane == 0) mbar_arrive(&w_empty[prev]);   // free, after k = 0 the previous tap's slot
+          if (k + 1 < TC_BK / 16) {
+            ldsm_a_sw128(fw[(k + 1) & 1][0], sb, wrow, k + 1);
+            ldsm_a_sw128(fw[(k + 1) & 1][1], sb + F1_W2_STAGE / 2, wrow, k + 1);
           }
         }
-        wgmma_commit();
-        if (tap == 8 && lane == 0) mbar_arrive(&order_bar[cw ^ 1]);
-        wgmma_wait<1>();
-        if (prev >= 0 && lane == 0) mbar_arrive(&w_empty[prev]);
         prev = stage;
         if (++stage == F1_W2_STAGES) { stage = 0; phase ^= 1; }
       }
       wgmma_wait<0>();
 #pragma unroll
-      for (int hm = 0; hm < 2; ++hm)
+      for (int v = 0; v < 2; ++v)
 #pragma unroll
-        for (int j = 0; j < 64; ++j) asm volatile("" : "+f"(d[hm][j])::"memory");
+        for (int e = 0; e < 64; ++e) asm volatile("" : "+f"(acc.d[v][e])::"memory");
       if (lane == 0) mbar_arrive(&w_empty[prev]);
-      Acc128<64> acc;
-#pragma unroll
-      for (int hm = 0; hm < 2; ++hm)
-#pragma unroll
-        for (int j = 0; j < 32; ++j) acc.h[hm][j] = d[hm][j] + d[hm][32 + j];
-      conv_epilogue_tile<64>(a, acc, my_stg, img, h0, w0, 0, 0, r, c, 8, bar);
+      conv_wide_epilogue(a, acc, img, h0, w0, 0);
     }
   }
   __syncthreads();
@@ -1153,8 +1167,8 @@ int launch_conv1_fused_tc(const float* x_nchw, const float* w1_oihw, const float
   fa.x = x_nchw; fa.w1 = w1_oihw; fa.bias1 = bias1;
   ConvTcArgs& a = fa.c2;
   a.N = N; a.H = H; a.W = W; a.cin = 64; a.cout = 64;
-  a.tw_log2 = 3;
-  a.tiles_w = cdiv(W, 8);
+  a.tw_log2 = 4;
+  a.tiles_w = cdiv(W, 16);
   a.tiles_h = cdiv(H, 16);
   a.n_tiles = 1;
   a.total_tiles = (int)((long long)N * a.tiles_h * a.tiles_w);

@@ -194,14 +194,12 @@ int launch_dist_top16_tc(const __nv_bfloat16* q_hi, const __nv_bfloat16* q_lo, c
 int launch_dist_dense_tc(const __nv_bfloat16* q_hi, const __nv_bfloat16* q_lo, const float* qn, int m,
                          const __nv_bfloat16* d_hi, const __nv_bfloat16* d_lo, const float* dn, int n, int K,
                          float* out, long long ld_out, cudaStream_t s);
-// tc_dist1.cu  (single-pass fp16 screening + exact re-scoring + guard + exact fallback)
-size_t dist1_workspace_bytes(int m, int n, int d, size_t* off /*[9]*/);
-int launch_dist_topk_1pass(const float* q, int m, const float* db, int n, int n_valid, int d, int k, long long idx_base,
-                           void* ws, float* out_dist, long long* out_idx, uint64_t* launches, cudaStream_t s);
-const int* dist1_flag_counter(const void* ws, int m, int n, int d);
-// ... on a database prepared once by ibl_db_prepare (plane, aux, maxima as rows_f16_kernel / dist_colmax_kernel
-// make them): the same screening with the database conversion skipped, and the small-batch streaming search
+// tc_dist1.cu  (fp16 screening + exact re-scoring + guard + exact fallback) on a database prepared by
+// launch_db_prepare (plane, aux, maxima as rows_f16_kernel / dist_colmax_kernel make them): the single-pass screening
+// and the small-batch streaming search
 int launch_db_prepare(const float* db, int n, int d, __half* plane, float4* aux, float* dbmax, cudaStream_t s);
+size_t dist1_workspace_bytes(int m, int d, size_t* off /*[7]*/);
+const int* dist1_flag_counter(const void* ws, int m, int d);
 int launch_dist_topk_1pass_prepared(const float* q, int m, const float* db, const __half* plane, const float4* aux,
                                     const float* dbmax, int n, int d, int k, long long idx_base, void* ws,
                                     float* out_dist, long long* out_idx, uint64_t* launches, cudaStream_t s);

@@ -82,8 +82,8 @@ struct ibl_engine {
   DevBuf pca_gy_pl;                     // PCA backward: bf16 hi|lo planes of dL/dy, rows padded to 8 columns
   DevBuf mrg_d, mrg_i;
   DevBuf bw_g, bw_x, bw_part, bw_w;      // conv backward: dY planes, X planes, wgrad/bias partials, dgrad filter planes
-  DevBuf d1_ws;                          // workspace of the single-pass distance/top-k path (tc_dist1.cu)
-  DevBuf db_ws;                          // workspace of the searches over a prepared database (ibl_db_topk)
+  DevBuf screen_ws;                      // workspace of the fp16 screening paths over a prepared database (tc_dist1.cu)
+  DevBuf db_prep;                        // ibl_l2dist_topk's prepared database: fp16 plane | aux rows | maxima
   DevBuf q_err, db_err, guard_ws;        // guard of the bf16x3 screening paths: per-row error norms, workspace
   DevBuf knn_ws;                         // neighbour pass of the re-ranking (rerank.cu)
   const int* knn_flag_counter = nullptr; // its count of rows sent to the exact scan (null: no call yet)
@@ -280,7 +280,7 @@ int ibl_engine_destroy(ibl_engine* e) {
   DevBuf* bufs[] = {&e->act[0], &e->act[1], &e->feat, &e->nv_assign, &e->nv_inv, &e->nv_raw, &e->vlad,
                     &e->pca_partial, &e->qn, &e->dbn, &e->dist_chunk, &e->cand_d, &e->cand_i,
                     &e->stage_in, &e->stage_out, &e->stage_out2, &e->stage_u8, &e->q_pl, &e->db_pl, &e->v_pl, &e->pca_pl,
-                    &e->mrg_d, &e->mrg_i, &e->d1_ws, &e->bw_g, &e->bw_x, &e->bw_part, &e->bw_w, &e->ssq, &e->nv_part, &e->nv_asum, &e->nvw_pl, &e->nv_ticket, &e->pca_gy_pl};
+                    &e->mrg_d, &e->mrg_i, &e->screen_ws, &e->db_prep, &e->bw_g, &e->bw_x, &e->bw_part, &e->bw_w, &e->ssq, &e->nv_part, &e->nv_asum, &e->nvw_pl, &e->nv_ticket, &e->pca_gy_pl};
   for (DevBuf* b : bufs) b->release();
   e->knn_ws.release();
   rerank_ws_destroy(e->rr_ws);
@@ -1063,6 +1063,26 @@ int ibl_l2dist_self(ibl_engine* e, const float* x, int n, int d, float* out, voi
   return IBL_OK;
 }
 
+// k <= 12 on the tensor cores over a prepared database (launch_db_prepare): m > 128, the single-pass screening (path
+// 1); m <= 128, the streaming scan (path 4).
+static int prepared_topk(ibl_engine* e, const float* q, int m, const float* db, const __half* plane, const float4* aux,
+                         const float* dbmax, int n, int d, int k, int64_t idx_base, float* out_dist, int64_t* out_idx,
+                         cudaStream_t s) {
+  if (m > 128) {
+    size_t off[7];
+    IBL_RET(e->screen_ws.ensure(dist1_workspace_bytes(m, d, off)));
+    e->flag_counter = dist1_flag_counter(e->screen_ws.p, m, d);
+    e->dist_path = 1;
+    return launch_dist_topk_1pass_prepared(q, m, db, plane, aux, dbmax, n, d, k, (long long)idx_base, e->screen_ws.p,
+                                           out_dist, reinterpret_cast<long long*>(out_idx), &e->launches, s);
+  }
+  IBL_RET(e->screen_ws.ensure(db_scan_workspace_bytes(m, n, d)));
+  e->flag_counter = db_scan_flag_counter(e->screen_ws.p, m, n, d);
+  e->dist_path = 4;
+  return launch_db_scan_topk(q, m, db, plane, aux, dbmax, n, d, k, (long long)idx_base, e->screen_ws.p, out_dist,
+                             reinterpret_cast<long long*>(out_idx), &e->launches, s);
+}
+
 int ibl_l2dist_topk(ibl_engine* e, const float* q, int m, const float* db, int n, int n_valid, int d,
                     int k, int64_t idx_base, float* out_dist, int64_t* out_idx, void* stream) {
   IBL_REQUIRE(e && q && db && out_dist && out_idx, "null argument");
@@ -1071,13 +1091,17 @@ int ibl_l2dist_topk(ibl_engine* e, const float* q, int m, const float* db, int n
   IBL_REQUIRE(k >= 1 && k <= 128, "top-k supports 1 <= k <= 128");
   DeviceGuard g(e->device);
   if (e->gemm_mode == IBL_CONV_TC_BF16X3 && d % 64 == 0 && n_valid > 0 && k <= 12 && m > 128) {
-    // single fp16 tensor-core pass to screen, exact fp32 to decide, guard + exact fallback on the device
-    size_t off[9];
-    IBL_RET(e->d1_ws.ensure(dist1_workspace_bytes(m, n, d, off)));
-    e->flag_counter = dist1_flag_counter(e->d1_ws.p, m, n, d);
-    e->dist_path = 1;
-    return launch_dist_topk_1pass(q, m, db, n, n_valid, d, k, (long long)idx_base, e->d1_ws.p, out_dist,
-                                  reinterpret_cast<long long*>(out_idx), &e->launches, S(stream));
+    // single fp16 tensor-core pass to screen, exact fp32 to decide, guard + exact fallback on the device: the n_valid
+    // rows prepared as ibl_db_prepare does, then ibl_db_topk's path
+    cudaStream_t s = S(stream);
+    const size_t plane_bytes = (size_t)n_valid * d * 2;   // d % 64 == 0: the aux rows start 16-byte aligned
+    IBL_RET(e->db_prep.ensure(plane_bytes + (size_t)n_valid * 16 + 16));
+    __half* plane = e->db_prep.as<__half>();
+    float4* aux = reinterpret_cast<float4*>(e->db_prep.as<uint8_t>() + plane_bytes);
+    float* dbmax = reinterpret_cast<float*>(aux + n_valid);
+    IBL_RET(launch_db_prepare(db, n_valid, d, plane, aux, dbmax, s));
+    e->launches += 2;
+    return prepared_topk(e, q, m, db, plane, aux, dbmax, n_valid, d, k, idx_base, out_dist, out_idx, s);
   }
   if (e->gemm_mode == IBL_CONV_TC_BF16X3 && d % 64 == 0 && n_valid > 0) {
     cudaStream_t s = S(stream);
@@ -1210,22 +1234,8 @@ int ibl_db_topk(ibl_engine* e, const float* q, int m, const float* db, const voi
   if (e->gemm_mode != IBL_CONV_TC_BF16X3 || d % 64 != 0 || k > 12)
     return ibl_l2dist_topk(e, q, m, db, n, n, d, k, idx_base, out_dist, out_idx, stream);
   DeviceGuard g(e->device);
-  const __half* plane = reinterpret_cast<const __half*>(plane_f16);
-  const float4* a4 = reinterpret_cast<const float4*>(aux);
-  if (m > 128) {
-    // the single-pass screening of ibl_l2dist_topk on the prepared plane
-    size_t off[9];
-    IBL_RET(e->db_ws.ensure(dist1_workspace_bytes(m, 0, d, off)));
-    e->flag_counter = dist1_flag_counter(e->db_ws.p, m, 0, d);
-    e->dist_path = 1;
-    return launch_dist_topk_1pass_prepared(q, m, db, plane, a4, dbmax, n, d, k, (long long)idx_base, e->db_ws.p,
-                                           out_dist, reinterpret_cast<long long*>(out_idx), &e->launches, S(stream));
-  }
-  IBL_RET(e->db_ws.ensure(db_scan_workspace_bytes(m, n, d)));
-  e->flag_counter = db_scan_flag_counter(e->db_ws.p, m, n, d);
-  e->dist_path = 4;
-  return launch_db_scan_topk(q, m, db, plane, a4, dbmax, n, d, k, (long long)idx_base, e->db_ws.p, out_dist,
-                             reinterpret_cast<long long*>(out_idx), &e->launches, S(stream));
+  return prepared_topk(e, q, m, db, reinterpret_cast<const __half*>(plane_f16), reinterpret_cast<const float4*>(aux),
+                       dbmax, n, d, k, idx_base, out_dist, out_idx, S(stream));
 }
 
 int ibl_topk_rows(ibl_engine* e, const float* dist, int m, int n, int k, float* out_dist, int64_t* out_idx,

@@ -6,7 +6,8 @@
 //   1. rows_f16_kernel        one pass per matrix: fp16 plane of each row scaled by a power of two (row max in
 //                             [0.5,1): no overflow, 11 significant bits), exact fp32 |x|^2 (same summation order as
 //                             planes_sqnorm_kernel, so the exact distances below are unchanged) and the norm of
-//                             each row's rounding residual x - 2^e plane (error model of the guard);
+//                             each row's rounding residual x - 2^e plane (error model of the guard); the database's
+//                             pass runs in launch_db_prepare, before the screening;
 //   2. gemm_f16_top16_kernel  wgmma f16 (fp16 x fp16 -> fp32 in registers), ONE MMA per K step and 64-row
 //                             half, 128 queries x 128 database rows per tile, 5-stage TMA ring, running
 //                             top-16 per query in registers across the CTA's database range;
@@ -595,24 +596,22 @@ static int pick_runs1(int m_tiles, int n_tiles) {
   return best;
 }
 
-size_t dist1_workspace_bytes(int m, int n, int d, size_t* off /*[8]*/) {
-  // layout: q plane | db plane | q aux | db aux | db max2 + flag count (256 B) | flag list | cand_d | cand_i | scratch
+size_t dist1_workspace_bytes(int m, int d, size_t* off /*[7]*/) {
+  // layout: q plane | q aux | flag count (256 B) | flag list | cand_d | cand_i | scratch
   size_t o = 0;
   auto take = [&](size_t bytes) { const size_t at = o; o += (bytes + 255) & ~(size_t)255; return at; };
   off[0] = take((size_t)m * d * 2);
-  off[1] = take((size_t)n * d * 2);
-  off[2] = take((size_t)m * 16);
-  off[3] = take((size_t)n * 16);
-  off[4] = take(256);
-  off[5] = take((size_t)m * 4 + (size_t)m * 4);     // guard list | shared gates
-  off[6] = take((size_t)8 * m * 16 * 4);
-  off[7] = take((size_t)8 * m * 16 * 4);
-  off[8] = take(dx_lists_at(m) + (size_t)m * DX_CAP * 8);   // list counters | lists of the exact fallback
+  off[1] = take((size_t)m * 16);
+  off[2] = take(256);
+  off[3] = take((size_t)m * 4 + (size_t)m * 4);     // guard list | shared gates
+  off[4] = take((size_t)8 * m * 16 * 4);
+  off[5] = take((size_t)8 * m * 16 * 4);
+  off[6] = take(dx_lists_at(m) + (size_t)m * DX_CAP * 8);   // list counters | lists of the exact fallback
   return o;
 }
 
-// Database preparation of ibl_db_prepare: the fp16 plane and aux rows of rows_f16_kernel, and in dbmax[0..2] the
-// maxima of dist_colmax_kernel, exactly as the single-pass screening makes them on every call.
+// Database preparation (ibl_db_prepare, and ibl_l2dist_topk before its single-pass screening): the fp16 plane and aux
+// rows of rows_f16_kernel, and in dbmax[0..2] the maxima of dist_colmax_kernel.
 int launch_db_prepare(const float* db, int n, int d, __half* plane, float4* aux, float* dbmax, cudaStream_t s) {
   IBL_CUDA_OK(cudaMemsetAsync(dbmax, 0, 16, s));
   rows_f16_kernel<<<n, 256, 0, s>>>(db, d, plane, aux);
@@ -621,37 +620,28 @@ int launch_db_prepare(const float* db, int n, int d, __half* plane, float4* aux,
   return IBL_OK;
 }
 
-// q [m,d], db [n,d] fp32 (device); n_valid <= n; k <= 12.  plane / aux / dbmax: the prepared database
-// (launch_db_prepare over the n_valid rows), or null to prepare it here in the workspace.
-// ws: dist1_workspace_bytes(m, plane ? 0 : n, d).
-static int dist_topk_1pass(const float* q, int m, const float* db, int n, int n_valid, int d, int k, long long idx_base,
-                           const __half* plane, const float4* aux, const float* dbmax, void* ws, float* out_dist,
-                           long long* out_idx, uint64_t* launches, cudaStream_t s) {
-  IBL_REQUIRE(d % 64 == 0 && k >= 1 && k <= 12 && n_valid >= 1, "1-pass distance: d % 64 == 0, 1 <= k <= 12");
-  size_t off[9];
-  dist1_workspace_bytes(m, plane ? 0 : n, d, off);
+// q [m,d] fp32; db [n,d] fp32 and its prepared plane / aux / maxima (launch_db_prepare); 1 <= k <= 12, d % 64 == 0.
+// ws: dist1_workspace_bytes(m, d).
+int launch_dist_topk_1pass_prepared(const float* q, int m, const float* db, const __half* plane, const float4* aux,
+                                    const float* dbmax, int n, int d, int k, long long idx_base, void* ws,
+                                    float* out_dist, long long* out_idx, uint64_t* launches, cudaStream_t s) {
+  IBL_REQUIRE(d % 64 == 0 && k >= 1 && k <= 12 && n >= 1, "1-pass distance: d % 64 == 0, 1 <= k <= 12");
+  size_t off[7];
+  dist1_workspace_bytes(m, d, off);
   uint8_t* w = reinterpret_cast<uint8_t*>(ws);
   __half* qp = reinterpret_cast<__half*>(w + off[0]);
-  const __half* dp = plane ? plane : reinterpret_cast<__half*>(w + off[1]);
-  float4* qa = reinterpret_cast<float4*>(w + off[2]);
-  const float4* da = plane ? aux : reinterpret_cast<float4*>(w + off[3]);
-  const float* dmax2 = plane ? dbmax : reinterpret_cast<float*>(w + off[4]);
-  int* fcount = reinterpret_cast<int*>(w + off[4] + 16);
-  int* flist = reinterpret_cast<int*>(w + off[5]);
-  unsigned* gate = reinterpret_cast<unsigned*>(w + off[5] + (size_t)m * 4);
-  float* cd = reinterpret_cast<float*>(w + off[6]);
-  int* ci = reinterpret_cast<int*>(w + off[7]);
-  int* lcnt = reinterpret_cast<int*>(w + off[8]);
-  unsigned long long* lists = reinterpret_cast<unsigned long long*>(w + off[8] + dx_lists_at(m));
+  float4* qa = reinterpret_cast<float4*>(w + off[1]);
+  int* fcount = reinterpret_cast<int*>(w + off[2]);
+  int* flist = reinterpret_cast<int*>(w + off[3]);
+  unsigned* gate = reinterpret_cast<unsigned*>(w + off[3] + (size_t)m * 4);
+  float* cd = reinterpret_cast<float*>(w + off[4]);
+  int* ci = reinterpret_cast<int*>(w + off[5]);
+  int* lcnt = reinterpret_cast<int*>(w + off[6]);
+  unsigned long long* lists = reinterpret_cast<unsigned long long*>(w + off[6] + dx_lists_at(m));
 
-  IBL_CUDA_OK(cudaMemsetAsync(w + off[4], 0, 32, s));
+  IBL_CUDA_OK(cudaMemsetAsync(fcount, 0, 16, s));
   IBL_CUDA_OK(cudaMemsetAsync(gate, 0xFF, (size_t)m * 4, s));      // orderable +max: no gate yet
   rows_f16_kernel<<<m, 256, 0, s>>>(q, d, qp, qa);
-  if (!plane) {
-    rows_f16_kernel<<<n, 256, 0, s>>>(db, d, reinterpret_cast<__half*>(w + off[1]), reinterpret_cast<float4*>(w + off[3]));
-    dist_colmax_kernel<<<cdiv(n_valid, 256) < 64 ? cdiv(n_valid, 256) : 64, 256, 0, s>>>(
-        reinterpret_cast<float4*>(w + off[3]), n_valid, reinterpret_cast<float*>(w + off[4]));
-  }
   IBL_CUDA_OK(cudaGetLastError());
 
   CUtensorMap ma, mb;
@@ -660,18 +650,18 @@ static int dist_topk_1pass(const float* q, int m, const float* db, int n, int n_
     uint64_t str[1] = {(uint64_t)d * 2};
     uint32_t box[2] = {64, 128};
     IBL_RET(make_tmap(&ma, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, qp, dims_a, str, box));
-    IBL_RET(make_tmap(&mb, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, dp, dims_b, str, box));
+    IBL_RET(make_tmap(&mb, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, plane, dims_b, str, box));
   }
   Dist1Args g{};
   g.M = m; g.N = n; g.K = d;
-  g.n_tiles = cdiv(n_valid, D1_BN);
+  g.n_tiles = cdiv(n, D1_BN);
   const int m_tiles = cdiv(m, 128);
   const int runs = pick_runs1(m_tiles, g.n_tiles);
   g.nt_per_item = cdiv(g.n_tiles, runs);
   g.items_per_mtile = cdiv(g.n_tiles, g.nt_per_item);
   g.total_items = m_tiles * g.items_per_mtile;
-  g.n_valid = n_valid;
-  g.a_aux = qa; g.b_aux = da; g.cand_d = cd; g.cand_i = ci; g.gate = gate;
+  g.n_valid = n;
+  g.a_aux = qa; g.b_aux = aux; g.cand_d = cd; g.cand_i = ci; g.gate = gate;
   static DeviceOnce attr_done;   // the attributes are per device
   if (!attr_done.done()) {
     IBL_CUDA_OK(cudaFuncSetAttribute(gemm_f16_top16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, D1_SMEM));
@@ -683,44 +673,31 @@ static int dist_topk_1pass(const float* q, int m, const float* db, int n, int n_
   IBL_CUDA_OK(cudaGetLastError());
 
   FinishArgs f{};
-  f.q = q; f.db = db; f.q_aux = qa; f.db_aux = da; f.db_max2 = dmax2; f.cand_d = cd; f.cand_i = ci;
-  f.m = m; f.d = d; f.runs = g.items_per_mtile; f.k_out = k; f.n_valid = n_valid; f.idx_base = idx_base;
+  f.q = q; f.db = db; f.q_aux = qa; f.db_aux = aux; f.db_max2 = dbmax; f.cand_d = cd; f.cand_i = ci;
+  f.m = m; f.d = d; f.runs = g.items_per_mtile; f.k_out = k; f.n_valid = n; f.idx_base = idx_base;
   f.out_dist = out_dist; f.out_idx = out_idx; f.flag_count = fcount; f.flag_list = flist; f.list_cnt = lcnt;
   const size_t qsm = d <= 16384 ? (size_t)d * sizeof(float) : 16;
   dist_finish_kernel<<<m, 128, qsm, s>>>(f);
   IBL_CUDA_OK(cudaGetLastError());
 
   ExactArgs x{};
-  x.q = q; x.db = db; x.q_sq = reinterpret_cast<const float*>(qa); x.db_sq = reinterpret_cast<const float*>(da);
-  x.sq_stride = 4; x.m = m; x.d = d; x.n_valid = n_valid; x.k = k;
+  x.q = q; x.db = db; x.q_sq = reinterpret_cast<const float*>(qa); x.db_sq = reinterpret_cast<const float*>(aux);
+  x.sq_stride = 4; x.m = m; x.d = d; x.n_valid = n; x.k = k;
   x.idx_base = idx_base; x.flag_count = fcount; x.flag_list = flist; x.list_cnt = lcnt; x.lists = lists;
   x.out_dist = out_dist; x.out_idx = out_idx;
   IBL_RET(dx_scan_attr());
   dist_exact_scan_kernel<<<device_sm_count(), DX_SCAN_WARPS * 32, dx_scan_smem(d), s>>>(x);   // exits at once when nothing is listed
   dist_exact_finish_kernel<<<64, 256, 0, s>>>(x);
   IBL_CUDA_OK(cudaGetLastError());
-  if (launches) *launches += plane ? 5 : 7;
+  if (launches) *launches += 5;
   return IBL_OK;
 }
 
-int launch_dist_topk_1pass(const float* q, int m, const float* db, int n, int n_valid, int d, int k, long long idx_base,
-                           void* ws, float* out_dist, long long* out_idx, uint64_t* launches, cudaStream_t s) {
-  return dist_topk_1pass(q, m, db, n, n_valid, d, k, idx_base, nullptr, nullptr, nullptr, ws, out_dist, out_idx,
-                         launches, s);
-}
-
-// ws: dist1_workspace_bytes(m, 0, d)
-int launch_dist_topk_1pass_prepared(const float* q, int m, const float* db, const __half* plane, const float4* aux,
-                                    const float* dbmax, int n, int d, int k, long long idx_base, void* ws,
-                                    float* out_dist, long long* out_idx, uint64_t* launches, cudaStream_t s) {
-  return dist_topk_1pass(q, m, db, n, n, d, k, idx_base, plane, aux, dbmax, ws, out_dist, out_idx, launches, s);
-}
-
 // the guard's counter of listed queries in this workspace (test hook ibl_debug_dist_flagged)
-const int* dist1_flag_counter(const void* ws, int m, int n, int d) {
-  size_t off[9];
-  dist1_workspace_bytes(m, n, d, off);
-  return reinterpret_cast<const int*>(reinterpret_cast<const uint8_t*>(ws) + off[4] + 16);
+const int* dist1_flag_counter(const void* ws, int m, int d) {
+  size_t off[7];
+  dist1_workspace_bytes(m, d, off);
+  return reinterpret_cast<const int*>(reinterpret_cast<const uint8_t*>(ws) + off[2]);
 }
 
 // layout: flag count, database maxima (256 B) | flag list [m], list counters [m] | lists [m][DX_CAP] keys
